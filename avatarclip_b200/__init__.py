@@ -1,4 +1,4 @@
-"""avatarclip_b200 -- B200-native (sm_100a) implementation of the AvatarCLIP appearance-optimisation
+"""avatarclip_b200 -- H100-native (sm_90a) implementation of the AvatarCLIP appearance-optimisation
 hot path behind the reference's own Python surface (AvatarGen/AppearanceGen):
 
     NeuSRenderer / SDFNetwork / RenderingNetwork / SingleVarianceNetwork   (models/renderer.py, fields.py)

@@ -63,7 +63,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise AvcError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  avatarclip_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a).  avatarclip_b200 has no CPU or PyTorch fallback.")
     L = C.CDLL(LIB_PATH)
     vp, i64, i32, f32, sz = C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_size_t
     P = C.POINTER

@@ -9,7 +9,7 @@
 // fp16 weight matrix exactly once: by bytes they are weight-bandwidth bound, in practice latency bound (~200 dependent
 // kernels per step), so the tiles are small and split over K where N alone cannot fill the SMs, and every kernel issues
 // all its global loads in one batch (DESIGN.md 3.3).  Two GEMM kernels: k_gemm16_tc (default when M <= 128: TMA-fed
-// tcgen05 tiles of 128 x 32, the constant weight tiles issued before the programmatic-dependency wait) and k_gemm16
+// wgmma tiles of 128 x 32, the constant weight tiles issued before the programmatic-dependency wait) and k_gemm16
 // (mma.sync m16n8k16, 64 x 32 tiles, 6-stage cp.async; larger batches, the persistent variant, AVC_CLIP_TC=0).
 #include <cuda_fp16.h>
 
@@ -231,52 +231,41 @@ int gemm16(cudaStream_t st, const __half* A, int lda, const __half* Wt, int ldw,
 }
 
 // ------------------------------------------------------------------------------------------------
-// The same GEMM on tcgen05 (AVC_CLIP_TC, the chained structure's default when M <= 128): all token rows of the batch
-// (M = 100 at B = 2) are ONE 128-row MMA tile, so a CTA owns a 128 x 32 output tile for its K range.
-//   warp 0   TMA producer: W tiles (constants) go out BEFORE griddepcontrol.wait, the A tiles right after it;
-//            8-stage ring of (A 16 KB + W 4 KB), K-major SWIZZLE_128B;
-//   warp 1   TMEM (32 columns) + tcgen05.mma.kind::f16 (fp16 operands, fp32 accumulate), M = 128, N = 32;
-//   warps 2-5  epilogue: tcgen05.ld 32x32b.x32 (thread <-> row), transposed through shared memory so that lanes <->
-//            column pairs (two rows x 128 B per warp instruction), same functors as the mma.sync kernel.
+// The same GEMM on the warpgroup MMA (AVC_CLIP_TC, the chained structure's default when M <= 128): all token rows of the
+// batch (M = 100 at B = 2) are ONE 128-row tile, so a CTA owns a 128 x 32 output tile for its K range.
+//   warps 0-7  two consumer warpgroups (rows 0-63 / 64-127): wgmma m64n32k16 (fp16 operands, fp32 accumulate) into
+//              16 registers per thread, then the functor straight from the fragment (column pairs, as mma.sync gives);
+//   warp 8     TMA producer: W tiles (constants) go out BEFORE griddepcontrol.wait, the A tiles right after it;
+//              8-stage ring of (A 16 KB + W 4 KB), K-major SWIZZLE_128B.
 // grid (N / 32, ksplit); rows >= M of the A box are zero-filled by TMA and never stored.
 // ------------------------------------------------------------------------------------------------
 constexpr int TBN = 32, TBK = 64, TST = 8;
 constexpr int T_A_BYTES = 128 * TBK * 2, T_W_BYTES = TBN * TBK * 2, T_STAGE = T_A_BYTES + T_W_BYTES;
-constexpr int T_EPI_BYTES = 4 * 32 * 33 * 4;
-constexpr int T_SMEM = 1024 + TST * T_STAGE + 256 + T_EPI_BYTES;
-// instruction descriptor, kind::f16 with F16 operands (format 0), F32 accumulator, both operands K-major
-constexpr uint32_t kIdescF16 = (1u << 4) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+constexpr int T_SMEM = 1024 + TST * T_STAGE + 256;
 
 template <typename Epi>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(tc::kTcThreads, 1)
 k_gemm16_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW, int M, int N, int K,
             int k_per_split, Epi epi) {
   using namespace avc::tc;
   extern __shared__ uint8_t t_smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)t_smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = (uint64_t*)(smem + TST * T_STAGE);
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * TST + 1);
-  float* stage_t = (float*)(smem + TST * T_STAGE + 256);
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * TST, tfull = empty0 + 8 * TST;
+  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * TST;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * TBN, ks = blockIdx.y;
   const int kb0 = ks * k_per_split, ke = min(K, kb0 + k_per_split);
   const int nk = (ke - kb0 + TBK - 1) / TBK;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&mapA); tma_prefetch_desc(&mapW);
-    for (int s = 0; s < TST; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-    mbar_init(tfull, 1);
+    for (int s = 0; s < TST; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 32);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       const int npre = nk < TST ? nk : TST;
       for (int s = 0; s < npre; ++s) {      // weights do not depend on the predecessor kernel
@@ -292,61 +281,47 @@ k_gemm16_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         tma_load_2d(smem_base + s * T_STAGE + T_A_BYTES, &mapW, kb0 + kb * TBK, n0, full0 + 8 * s);
         tma_load_2d(smem_base + s * T_STAGE, &mapA, kb0 + kb * TBK, 0, full0 + 8 * s);
       }
-      // the dependent kernel is released after the main loop, like in the mma.sync kernel (the first
-      // launch_dependents of a CTA is the one that counts: no early call from the producer)
-      mbar_wait(tfull, 0);
     }
-    __syncwarp();
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  } else if (warp == 1) {
-    for (int kb = 0; kb < nk; ++kb) {
-      const int s = kb % TST;
-      mbar_wait(full0 + 8 * s, (kb / TST) & 1);
-      tc_fence_after();
-      if (elect_one_sync()) {
-        const uint64_t da = make_smem_desc(smem_base + s * T_STAGE, 0, 1024);
-        const uint64_t db = make_smem_desc(smem_base + s * T_STAGE + T_A_BYTES, 0, 1024);
-#pragma unroll
-        for (int k4 = 0; k4 < TBK / 16; ++k4) umma_f16(tmem_base, da + 2 * k4, db + 2 * k4, kIdescF16, (kb | k4) ? 1u : 0u);
-        umma_commit(empty0 + 8 * s);
-        if (kb == nk - 1) umma_commit(tfull);
-      }
-      __syncwarp();
-    }
-    mbar_wait(tfull, 0);
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  } else {
-    const int q = warp & 3;                       // TMEM lane quarter of this warp (warps 2..5 -> 2, 3, 0, 1)
-    const int rsub = lane >> 4, cp = lane & 15;   // after the transpose: lanes 0-15 one row, 16-31 the next; 2 columns each
-    const int col = n0 + 2 * cp;
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    float2 pre[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int row = q * 32 + 2 * i + rsub;
-      pre[i] = row < M ? epi.prefetch(row, col, ks) : make_float2(0.f, 0.f);
-    }
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    uint32_t r[32];
-    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16), r);
-    float* st = stage_t + (warp - 2) * (32 * 33);
-#pragma unroll
-    for (int j = 0; j < 32; ++j) st[lane * 33 + j] = __uint_as_float(r[j]);
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int rl = 2 * i + rsub, row = q * 32 + rl;
-      if (row < M) epi(row, col, st[rl * 33 + 2 * cp], st[rl * 33 + 2 * cp + 1], ks, pre[i]);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 32);
+  const int g = warp >> 2, wq = warp & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int r0 = 64 * g + 16 * wq + (lane >> 2), cp = 2 * (lane & 3);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  float2 pre[4][2];
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      pre[j][h] = r0 + 8 * h < M ? epi.prefetch(r0 + 8 * h, n0 + 8 * j + cp, ks) : make_float2(0.f, 0.f);
+  float acc[16];
+  int prev = -1;
+  for (int kb = 0; kb < nk; ++kb) {
+    const int s = kb % TST;
+    mbar_wait(full0 + 8 * s, (kb / TST) & 1);
+    const uint64_t da = make_wgmma_desc(smem_base + s * T_STAGE + (uint32_t)g * 8192u, 16, 1024);
+    const uint64_t db = make_wgmma_desc(smem_base + s * T_STAGE + T_A_BYTES, 16, 1024);
+    wgmma_fence_acc(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k4 = 0; k4 < TBK / 16; ++k4) wgmma_f16_n32<0, 0>(acc, da + 2 * k4, db + 2 * k4, (kb | k4) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_fence_acc(acc);
+    wgmma_wait<1>();
+    if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
+    prev = s;
   }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  // the dependent kernel is released after the main loop, like in the mma.sync kernel
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      if (row < M) epi(row, n0 + 8 * j + cp, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], ks, pre[j][h]);
+    }
 }
 
 int clip_tc_enabled() {      // AVC_CLIP_TC=0: the mma.sync GEMM for every launch (A-B knob; read on every call)
@@ -367,7 +342,7 @@ int gemm16_tc(cudaStream_t st, const __half* A, int lda, const __half* Wt, int l
     AVC_CUDA_TRY(cudaFuncSetAttribute(k_gemm16_tc<Epi>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM));
     attr_set = true;
   }
-  AVC_CUDA_TRY(launch_pdl(k_gemm16_tc<Epi>, dim3(N / TBN, ksplit), dim3(192), T_SMEM, st, mA, mW, M, N, K, kper, epi));
+  AVC_CUDA_TRY(launch_pdl(k_gemm16_tc<Epi>, dim3(N / TBN, ksplit), dim3(tc::kTcThreads), T_SMEM, st, mA, mW, M, N, K, kper, epi));
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -1698,8 +1673,8 @@ int launch_mega(bool fwd, const MegaArgs& args, cudaStream_t st) {
 }
 
 int mega_enabled() {      // AVC_CLIP_MEGA=1: one persistent cooperative kernel per pass instead of the chain of stand-alone
-  const char* e = getenv("AVC_CLIP_MEGA");      // kernels.  Measured on B200 (r2): 0.91 + 1.33 ms against 0.59 + 0.88 ms
-  return (e && atoi(e) == 1) ? 1 : 0;           // for the chain -> off by default; read on every call (A-B knob)
+  const char* e = getenv("AVC_CLIP_MEGA");      // kernels (grid-wide barriers between its stages); off by default
+  return (e && atoi(e) == 1) ? 1 : 0;           // read on every call (A-B knob)
 }
 
 }  // namespace
@@ -1756,8 +1731,8 @@ int avc_clip_loss_fwd(const avc_clip_cfg* cfg, const avc_clip_weights* wt, const
   AVC_CUDA_TRY(launch_pdl(k_layernorm, dim3(ceil_div(M, 8)), dim3(256), 0, st, w.tok_pre, M, Wd, wt->ln_pre_g, wt->ln_pre_b, w.x, nullptr, nullptr));
   AVC_LAUNCH_TRY();
   // AVC_CLIP_FUSED_ATTN=1 (opt-in): ln_1 / in_proj / attention / out_proj as ONE kernel per (image, head) instead of four
-  // kernels.  Measured on B200 (r2): forward 1.05 ms against 0.60 ms -- 24 fat CTAs serialise what the chain spreads over
-  // 100-190 CTAs per kernel (7 LayerNorm rows per warp, 256-thread softmax, 38 k atomics per CTA) -- so it is off by default.
+  // kernels: 24 fat CTAs serialise what the chain spreads over 100-190 CTAs per kernel (7 LayerNorm rows per warp,
+  // 256-thread softmax, 38 k atomics per CTA), so it is off by default.
   const char* fa_env = getenv("AVC_CLIP_FUSED_ATTN");
   const bool fused_attn = (fa_env && atoi(fa_env) == 1) && T <= AT && Wd == 768 && Wd / cfg->heads == AD;
   if (fused_attn) {

@@ -1,4 +1,4 @@
-// avc_common.cuh -- shared helpers for the sm_100a kernels of libavc_b200.so.
+// avc_common.cuh -- shared helpers for the sm_90a kernels of libavc_b200.so.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

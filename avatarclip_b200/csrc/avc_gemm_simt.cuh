@@ -221,7 +221,9 @@ static inline int launch_gemm_tn(cudaStream_t st, int64_t P, int N1, int N2, con
                                  const float* B, int ldb, float* C, int ldc) {
   if (P <= 0 || N1 <= 0 || N2 <= 0) return 0;
   int tiles = ceil_div(N1, 128) * ceil_div(N2, 128);
-  int splits = (2 * 148 + tiles - 1) / tiles;
+  static thread_local int sms = 0;
+  if (!sms) { int dev = 0; AVC_CUDA_TRY(cudaGetDevice(&dev)); AVC_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)); }
+  int splits = (2 * sms + tiles - 1) / tiles;      // two CTAs per SM
   int rows_per_split = (int)round_up(ceil_div(P, splits), 16);
   splits = ceil_div(P, rows_per_split);
   dim3 grid(ceil_div(N2, 128), ceil_div(N1, 128), splits);

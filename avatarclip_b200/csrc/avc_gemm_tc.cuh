@@ -1,19 +1,20 @@
-// avc_gemm_tc.cuh -- tcgen05 (5th-gen tensor core) GEMM tiles for sm_100a with TMA-fed operands and
-// TMEM accumulators; engine 1 of the NeuS MLP contractions.
+// avc_gemm_tc.cuh -- Hopper (sm_90a) warpgroup-MMA GEMM tiles with TMA-fed operands; engine 1 of the NeuS MLP
+// contractions.
 //
 // Precision: the NeuS SDF trunk cannot run on single-pass 16-bit tensor-core math (SURVEY.md Appendix C:
 // inv_s ~ 500 amplifies SDF error; bf16 gives 2.6e-2 RGB error, TF32 3e-3).  Operands are therefore kept as
 // TWO-TERM bf16 splits  x = hi + lo  (hi = bf16(x), lo = bf16(x - hi), ~16 mantissa bits) and every product is
-// three MMAs  hi*hi + hi*lo + lo*hi  accumulated in fp32 in TMEM (the dropped lo*lo term is ~2^-16 relative).
+// three MMAs  hi*hi + hi*lo + lo*hi  accumulated in fp32 (the dropped lo*lo term is ~2^-16 relative).
 //
 //   gemm_tc_nt : C[m,n] = sum_k A[m,k] B[n,k]     A:[M,lda] B:[N,ldb], both K-contiguous (K-major operands)
 //   gemm_tc_tn : C[i,j] += sum_p A[p,i] B[p,j]    reduction over rows (weight gradients; MN-major operands)
 //
-// Kernel shape: warp 0 TMA producer, warp 1 TMEM owner + one elect.sync lane issuing the MMAs, the remaining warps
-// the epilogue (TMEM lane quarter = warp_id % 4).  NT: persistent, 576 threads (16 epilogue warps), tile 128 x 64/128,
-// 4 TMEM accumulator buffers, B panel resident in shared memory when K <= 256.  TN: 320 threads (8 epilogue warps), one
-// tile per CTA, split over the reduction dimension.  K step 64 (one 128-byte swizzle atom), shared-memory ring with
-// full/empty mbarriers, accumulator hand-off through tcgen05.commit.
+// Kernel shape (288 threads): warps 0-7 are two consumer warpgroups, warpgroup g owning rows [64 g, 64 g + 64) of the
+// 128-row tile: it issues wgmma.mma_async m64nBNk16 on shared-memory descriptors, keeps its fp32 accumulator in
+// registers and runs the epilogue straight from that fragment; warp 8 is the TMA producer.  K step 64 (one 128-byte
+// swizzle atom), shared-memory ring with full (TMA transaction count) / empty (one arrival per consumer warpgroup)
+// mbarriers.  NT: persistent, one column tile per CTA, B panel resident in shared memory when K <= 256.  TN: one tile
+// per CTA, split over the reduction dimension.
 #pragma once
 #include <type_traits>
 #include <cuda.h>
@@ -22,6 +23,7 @@
 #include <cstdlib>
 
 #include "avc_common.cuh"
+#include "avc_wgmma.cuh"
 
 namespace avc {
 namespace tc {
@@ -35,7 +37,10 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// Bounded spin: a protocol bug must trap (CUDA error) instead of hanging the GPU box.
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// Bounded spin: a protocol bug must trap (CUDA error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done = 0;
   for (uint32_t spins = 0; !done; ++spins) {
@@ -44,21 +49,23 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
         "selp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (spins > (1u << 26)) __trap();      // ~seconds: far beyond any legitimate wait, short of the box's watchdog
+    if (spins > (1u << 26)) __trap();      // ~seconds: far beyond any legitimate wait, short of the driver's watchdog
   }
 }
 // Optional stall probe of the NT kernel (compile with -DAVC_NT_PROBE=1, see tools/nt_probe.py): cycles the TMA warp waits
-// for a free stage, the MMA warp for operands / for a drained accumulator, one epilogue warp for a finished accumulator,
-// and each role's total loop time, summed over the CTAs of every launch, per epilogue functor (Epi::kProbeId).
+// for a free stage, consumer warpgroup 0 waits for operands, and each role's total loop time, summed over the CTAs of
+// every launch, per epilogue functor (Epi::kProbeId).
 #ifdef AVC_NT_PROBE
 static __device__ unsigned long long g_nt_probe[16][8];
 #define AVC_PROBE_WAIT(acc, bar, par) do { long long t__ = clock64(); mbar_wait(bar, par); (acc) += clock64() - t__; } while (0)
 #define AVC_PROBE_DECL(name) long long name = 0
+#define AVC_PROBE_START(name) const long long name = clock64()
 #define AVC_PROBE_NOW() clock64()
 #define AVC_PROBE_ADD(id, slot, v) atomicAdd(&g_nt_probe[id][slot], (unsigned long long)(v))
 #else
 #define AVC_PROBE_WAIT(acc, bar, par) mbar_wait(bar, par)
 #define AVC_PROBE_DECL(name)
+#define AVC_PROBE_START(name)
 #define AVC_PROBE_NOW() 0
 #define AVC_PROBE_ADD(id, slot, v)
 #endif
@@ -71,9 +78,9 @@ struct EpiProbeId { static constexpr int value = 0; };
 template <typename E>
 struct EpiProbeId<E, std::void_t<decltype(E::kProbeId)>> { static constexpr int value = E::kProbeId; };
 
-// Programmatic dependent launch (the tcgen05 kernels of a step run back to back in one stream / graph): a kernel launched
+// Programmatic dependent launch (the GEMM kernels of a step run back to back in one stream / graph): a kernel launched
 // with launch_pdl may start while its predecessor is still running -- as SMs free up its CTAs do their set-up (barriers,
-// TMEM, tensor-map prefetch) and load what does NOT depend on the predecessor (the packed weights) -- and calls
+// tensor-map prefetch) and load what does NOT depend on the predecessor (the packed weights) -- and calls
 // pdl_wait() before it touches anything the predecessor may have written.  pdl_trigger() lets the NEXT kernel do the same;
 // it is only issued after this kernel's own pdl_wait(), so everything older than the predecessor is complete by induction.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -93,8 +100,10 @@ static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 blo
 
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// bar.sync on a named barrier: the 128 threads of one consumer warpgroup (ids 1 + g; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
   asm volatile(
@@ -108,75 +117,6 @@ __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int x, i
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
-}
-
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One lane of a converged warp (elect.sync): code under `if (elect_one_sync())` is known to run on exactly one
-// thread, so the uniform-datapath instructions in it (UTCHMMA, UTCBAR) need no per-instruction election.
-__device__ __forceinline__ bool elect_one_sync() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16 / fp16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ------------------------------------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor (sm_100): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48)
-// | layout type [61,64) (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Instruction descriptor, kind::f16: c_format F32 (1) @4, a/b format BF16 (1) @7/@10, a_major @15, b_major @16
-// (0 = K-major, 1 = MN-major), N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // ------------------------------------------------------------------------------------------------ host: tensor maps
@@ -235,60 +175,27 @@ struct SplitPtr {            // two-term bf16 split of an fp32 matrix, both [row
 };
 
 constexpr int kBM = 128, kBK = 64;
-constexpr int kTcThreads = 320;   // TN kernel: warp 0 TMA, warp 1 MMA/TMEM, warps 2-9 epilogue (two per TMEM lane quarter)
-constexpr int kEpiWarps = 8;
-// NT kernel: EW epilogue warps (EW/4 per TMEM lane quarter) and PFB registers per thread of prefetched epilogue
-// operands are template parameters; the launcher uses 16 warps / 32 registers (see launch_gemm_tc_nt).
+constexpr int kConsumerThreads = 256;                      // two consumer warpgroups
+constexpr int kTcThreads = kConsumerThreads + 32;          // + the TMA producer warp
+constexpr int kProducerWarp = kConsumerThreads / 32;
+constexpr int kSmemMax = 232448;                           // 227 KB of shared memory per CTA
 
 // RESB: the CTA keeps its whole B panel (BN rows x up to kResK k-blocks, hi and lo) resident in shared memory and only
-// streams A: with the panel re-fetched for every 128-row tile the operand traffic L2 -> SM (262 KB per 128 x 128 tile)
-// was what bounded the launches with a light epilogue; resident, it is half of that.
+// streams A: re-fetched for every 128-row tile, the B panel would double the L2 -> SM operand traffic of a tile.
 constexpr int kResK = 4;          // k-blocks (of 64) a resident panel holds: K <= 256
-template <int BN, int NPROD, int EW = 8, bool RESB = false>
+template <int BN, int NPROD, bool RESB = false>
 struct TcCfg {
   static constexpr int A_BYTES = kBM * kBK * 2;                    // one (hi or lo) A slab: 16 KB
   static constexpr int B_BYTES = BN * kBK * 2;
   static constexpr int NOP = (NPROD == 3) ? 2 : 1;                 // slabs per operand (hi, lo)
-  static constexpr int EPI_BYTES = EW * 32 * 16 * 4;       // per-warp 32x16 fp32 transpose buffers (XOR-swizzled)
   static constexpr int BRES_BYTES = RESB ? kResK * NOP * B_BYTES : 0;
   static constexpr int STAGE_BYTES = RESB ? NOP * A_BYTES : NOP * (A_BYTES + B_BYTES);
-  static constexpr int kBudget = 232448 - 1024 - 256 - EPI_BYTES - BRES_BYTES;
-  static constexpr int STAGES = RESB ? (kBudget / STAGE_BYTES >= 4 ? 4 : kBudget / STAGE_BYTES)
-                                     : ((200 * 1024) / STAGE_BYTES >= 4 ? 4 : ((200 * 1024) / STAGE_BYTES));
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BRES_BYTES + 1024 /*align*/ + 256 /*barriers*/ + EPI_BYTES;
+  static constexpr int kBudget = kSmemMax - 1024 /*align*/ - 256 /*barriers*/ - BRES_BYTES;
+  static constexpr int STAGES = kBudget / STAGE_BYTES >= 4 ? 4 : kBudget / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BRES_BYTES + 1024 + 256;
   static_assert(STAGES >= 2, "tile too large for shared memory");
-  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory per CTA");
+  static_assert(SMEM_BYTES <= kSmemMax, "exceeds the 227 KB of shared memory per CTA");
 };
-
-// TMEM -> registers gives every thread one ROW (32 consecutive columns).  Writing that out directly would make each
-// warp store touch 32 different rows.  The 32x32 block is therefore transposed through a padded shared-memory tile so
-// that in the epilogue functor lane <-> column: every global access of the functor is one coalesced row segment.
-template <typename F>
-__device__ __forceinline__ void epilogue_block_transposed(float* stage /*[32][33]*/, const uint32_t (&r)[32], int lane,
-                                                          int row0, int nrows_valid, int col0, int ncols_valid, F&& f) {
-#pragma unroll
-  for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = __uint_as_float(r[j]);
-  __syncwarp();
-  if (lane < ncols_valid) {
-    for (int i = 0; i < nrows_valid; ++i) f(row0 + i, col0 + lane, stage[i * 33 + lane]);
-  }
-  __syncwarp();
-}
-
-// ------------------------------------------------------------------------------------------------ NT kernel
-// Epilogue: epi.one(row, col, value) for row < M, col < N; consecutive lanes hold consecutive columns.
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
-}
 
 // Epilogue functor interface (see avc_neus_kernels.cuh): functors with a nested `Aux` type split into
 // prefetch(row, col) -> Aux and operator()(row, col, acc, aux); plain functors only have operator()(row, col, acc).
@@ -305,13 +212,9 @@ struct EpiTraits<E, std::void_t<typename E::Aux>> {
   static __device__ __forceinline__ Aux prefetch(const E& e, int r, int c) { return e.prefetch(r, c); }
   static __device__ __forceinline__ void apply(const E& e, int r, int c, float4 a, const Aux& x) { e(r, c, a, x); }
 };
-// A full 32-row sub-block hands every thread FOUR groups of the same 4 columns, rows r, r + 8, r + 16, r + 24.  Functors
-// with a member `quad(row, col, acc[4], aux[4])` take them together: the column-range test and the null checks of the
-// optional outputs (uniform per launch, but each one a branch that ends a scheduling region) are then made once per four
-// groups and the four groups' loads / math / stores sit in one straight-line region the scheduler can interleave.
-// The epilogue's own global operands (stashes written passes ago: always DRAM misses) are register-prefetched only one
-// sub-block ahead -- far less than a loaded DRAM latency.  Functors with `l2_prefetch(m0, n0, bn, M, et, nth)` get the
-// chance to pull the NEXT row tile's operand lines into L2 a whole tile ahead (thread et of nth epilogue threads).
+// The epilogue's own global operands (stashes written passes ago: always DRAM misses) are loaded right before use.
+// Functors with `l2_prefetch(m0, n0, bn, M, et, nth)` get the chance to pull the NEXT row tile's operand lines into L2 a
+// whole tile ahead (thread et of nth epilogue threads).
 template <int ES>   // element size in bytes; [rows][ld] row-major array, tile rows [m0, m0 + 128) x columns [n0, n0 + bn)
 __device__ __forceinline__ void l2_prefetch_tile(const void* base, int ld, int ncols, int m0, int n0, int bn, int M,
                                                  int et, int nth) {
@@ -334,60 +237,54 @@ struct EpiL2<E, std::void_t<decltype(&E::l2_prefetch)>> {
   }
 };
 
-// Operands of the four groups of a sub-block (rows row + 8 p, clamped to row_last).  Functors whose operands depend on
-// the column only (biases) provide `prefetch4(col, aux[4])` and load them once instead of four times.
-template <typename E, typename = void>
-struct EpiPrefetch4 {
-  template <typename Aux>
-  static __device__ __forceinline__ void run(const E& e, int row, int row_last, int col, Aux (&dst)[4]) {
+// ------------------------------------------------------------------------------------------------ NT kernel
+// The accumulator fragment gives a thread column PAIRS of two rows r and r + 8 (avc_wgmma.cuh).  One exchange with the
+// neighbouring lane (lane ^ 1) turns them into one group of 4 consecutive columns per 8-column group -- even lanes take
+// row r, odd lanes row r + 8 -- so the functors see (row, col..col+3) with col % 4 == 0, as from the fp32 engine.  A warp
+// covers 16 rows x 32 bytes per group: every global access of a functor is whole 32-byte sectors.
+template <int BN, typename Epi>
+__device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[BN / 2], int row, int col0, int M, int N,
+                                            int lane) {
+  using Tr = EpiTraits<Epi>;
+  const bool odd = lane & 1;
+  constexpr int kB = 4;      // groups whose functor operands are loaded together, ahead of the arithmetic
 #pragma unroll
-    for (int p = 0; p < 4; ++p) dst[p] = EpiTraits<E>::prefetch(e, min(row + 8 * p, row_last), col);
-  }
-};
-template <typename E>
-struct EpiPrefetch4<E, std::void_t<decltype(&E::prefetch4)>> {
-  template <typename Aux>
-  static __device__ __forceinline__ void run(const E& e, int, int, int col, Aux (&dst)[4]) { e.prefetch4(col, dst); }
-};
-template <typename E, typename = void>
-struct EpiQuad {
-  template <typename Aux>
-  static __device__ __forceinline__ void run(const E& e, int r, int c, const float4 (&a)[4], const Aux (&x)[4]) {
+  for (int j0 = 0; j0 < BN / 8; j0 += kB) {
+    float4 v[kB];
+    typename Tr::Aux aux[kB];
 #pragma unroll
-    for (int p = 0; p < 4; ++p) EpiTraits<E>::apply(e, r + 8 * p, c, a[p], x[p]);
+    for (int u = 0; u < kB; ++u) {
+      const int j = j0 + u;
+      const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+      const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+      v[u] = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
+      const int col = col0 + 8 * j;
+      if (row < M && col < N) aux[u] = Tr::prefetch(epi, row, col);
+    }
+#pragma unroll
+    for (int u = 0; u < kB; ++u) {
+      const int col = col0 + 8 * (j0 + u);
+      if (row < M && col < N) Tr::apply(epi, row, col, v[u], aux[u]);
+    }
   }
-};
-template <typename E>
-struct EpiQuad<E, std::void_t<decltype(&E::quad)>> {
-  template <typename Aux>
-  static __device__ __forceinline__ void run(const E& e, int r, int c, const float4 (&a)[4], const Aux (&x)[4]) {
-    e.quad(r, c, a, x);
-  }
-};
+}
 
 // Persistent: gridDim.x CTAs (<= one per SM, a multiple of the number of column tiles); a CTA keeps one column tile
-// and walks the row tiles m_first, +m_stride, ...  The accumulator is multi-buffered in TMEM (NBUF x BN columns) so
-// the epilogue of tile i runs while the TMA/MMA warps already work on the next tiles:
-// tfull[b] (MMA -> epilogue, tcgen05.commit)  /  tempty[b] (epilogue -> MMA, one arrive per warp).
-template <int BN, int NPROD, int EW, int PFB, bool RESB, typename Epi>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
+// and walks the row tiles m_first, +m_stride, ...  While the consumers run the epilogue of tile i the producer already
+// fills the ring with the first k-blocks of tile i + 1.
+template <int BN, int NPROD, bool RESB, typename Epi>
+__global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapBhi, const __grid_constant__ CUtensorMap mapBlo,
                   int M, int N, int K, Epi epi, int l2pf, int b_const) {
-  using Cfg = TcCfg<BN, NPROD, EW, RESB>;
+  using Cfg = TcCfg<BN, NPROD, RESB>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B wants 1024-B tiles
   constexpr int kOpBytes = Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BRES_BYTES;     // stages, then the resident B panel
   uint64_t* bars = (uint64_t*)(smem + kOpBytes);
-  // accumulators: NBUF x BN TMEM columns (all 512 for BN = 128), so the TMA/MMA side can run up to NBUF - 1 tiles
-  // ahead of the epilogue instead of one
-  constexpr int NBUF = (512 / BN) > 4 ? 4 : (512 / BN);
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * Cfg::STAGES + 2 * NBUF + kResK);
-  float* epi_stage = (float*)(smem + kOpBytes + 256);
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bres_base = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * Cfg::STAGES, tfull0 = empty0 + 8 * Cfg::STAGES,
-                 tempty0 = tfull0 + 8 * NBUF, bfull = tempty0 + 8 * NBUF;
+  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * Cfg::STAGES, bfull = empty0 + 8 * Cfg::STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_n = (N + BN - 1) / BN;
@@ -399,21 +296,16 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   const int n0 = (int)(blockIdx.x % tiles_n) * BN;
   const int m_first = (int)(blockIdx.x / tiles_n), m_stride = (int)(gridDim.x / tiles_n);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&mapAhi); tma_prefetch_desc(&mapBhi);
     if (NPROD == 3) { tma_prefetch_desc(&mapAlo); tma_prefetch_desc(&mapBlo); }
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-    for (int b2 = 0; b2 < NBUF; ++b2) { mbar_init(tfull0 + 8 * b2, 1); mbar_init(tempty0 + 8 * b2, EW); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }
     for (int kb = 0; kb < kResK; ++kb) mbar_init(bfull + 8 * kb, 1);     // one per k-block of the resident B panel
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), NBUF * BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       // b_const: B holds constants of the step (the packed weights, written many kernels ago): its resident panel is
       // loaded while the predecessor kernel may still be running
@@ -437,7 +329,7 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
         }
       int it = 0;
       AVC_PROBE_DECL(w_empty);
-      const long long t_tma0 = AVC_PROBE_NOW();
+      AVC_PROBE_START(t_tma0);
       for (int mt = m_first; mt < tiles_m; mt += m_stride) {
         const int m0 = mt * kBM;
         const bool pf = l2pf && (mt + m_stride < tiles_m);
@@ -462,144 +354,60 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
       AVC_PROBE_ADD(EpiProbeId<Epi>::value, 1, AVC_PROBE_NOW() - t_tma0);
       AVC_PROBE_ADD(EpiProbeId<Epi>::value, 7, 1);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // The whole warp walks the loop converged (all lanes poll the barriers); one elected lane issues the MMAs.  The
-    // issue rate matters: 48 MMAs of 64 tensor-cycles each per 128 x 128 x 256 tile leave ~64 cycles per instruction,
-    // so the descriptors are derived by adding constants to one base per operand and k-block.
-    constexpr uint32_t idesc = make_idesc_bf16(kBM, BN, 0, 0);
+  } else {
+    const int g = warp >> 2, wq = warp & 3;      // consumer warpgroup, warp within it
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int row_in = 64 * g + 16 * wq + (lane >> 2) + 8 * (lane & 1), col_in = 4 * ((lane >> 1) & 1);
+    pdl_wait();      // the functor's operands and outputs belong to predecessor kernels
+    float acc[BN / 2];
     int it = 0, lt = 0;
-    AVC_PROBE_DECL(w_tempty); AVC_PROBE_DECL(w_full);
-    const long long t_mma0 = AVC_PROBE_NOW();
+    AVC_PROBE_DECL(w_full);
+    AVC_PROBE_START(t_mma0);
+    EpiL2<Epi>::run(epi, m_first * kBM, n0, BN, M, (int)threadIdx.x, kConsumerThreads);
     for (int mt = m_first; mt < tiles_m; mt += m_stride, ++lt) {
-      const uint32_t buf = lt % NBUF;
-      AVC_PROBE_WAIT(w_tempty, tempty0 + 8 * buf, ((lt / NBUF) & 1) ^ 1);   // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * BN;
+      const int m0 = mt * kBM;
+      EpiL2<Epi>::run(epi, (mt + m_stride) * kBM, n0, BN, M, (int)threadIdx.x, kConsumerThreads);   // a tile ahead
+      int prev = -1;
       for (int kb = 0; kb < nk; ++kb, ++it) {
         const int s = it % Cfg::STAGES;
         if (RESB && lt == 0) mbar_wait(bfull + 8 * kb, 0);      // this k-block of the B panel has landed (first tile only)
         AVC_PROBE_WAIT(w_full, full0 + 8 * s, (it / Cfg::STAGES) & 1);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          const uint32_t a_hi = smem_base + s * Cfg::STAGE_BYTES;
-          const uint32_t b_hi = RESB ? bres_base + kb * (Cfg::NOP * Cfg::B_BYTES) : a_hi + Cfg::NOP * Cfg::A_BYTES;
-          // K-major SWIZZLE_128B: 8-row groups are 1024 B apart (SBO); a K step of 16 elements is +32 B = +2 in the
-          // descriptor's start-address field (no carry out of the field: shared addresses stay below 2^18)
-          const uint64_t da = make_smem_desc(a_hi, 0, 1024), db = make_smem_desc(b_hi, 0, 1024);
-          constexpr uint64_t kLoA = (uint64_t)(Cfg::A_BYTES >> 4), kLoB = (uint64_t)(Cfg::B_BYTES >> 4);
+        const uint32_t a_hi = smem_base + s * Cfg::STAGE_BYTES + (uint32_t)g * (64 * 128);   // this warpgroup's 64 rows
+        const uint32_t b_hi = RESB ? bres_base + kb * (Cfg::NOP * Cfg::B_BYTES) : smem_base + s * Cfg::STAGE_BYTES + Cfg::NOP * Cfg::A_BYTES;
+        const uint64_t da = make_wgmma_desc(a_hi, 16, 1024), db = make_wgmma_desc(b_hi, 16, 1024);
+        constexpr uint64_t kLoA = (uint64_t)(Cfg::A_BYTES >> 4), kLoB = (uint64_t)(Cfg::B_BYTES >> 4);
+        wgmma_fence_acc(acc);
+        wgmma_fence();
 #pragma unroll
-          for (int k4 = 0; k4 < kBK / 16; ++k4) {
-            umma_f16(d_tmem, da + 2 * k4, db + 2 * k4, idesc, (kb | k4) ? 1u : 0u);
-            if (NPROD == 3) {
-              umma_f16(d_tmem, da + 2 * k4, db + kLoB + 2 * k4, idesc, 1u);
-              umma_f16(d_tmem, da + kLoA + 2 * k4, db + 2 * k4, idesc, 1u);
-            }
+        for (int k4 = 0; k4 < kBK / 16; ++k4) {
+          wgmma_bf16<BN, 0, 0>(acc, da + 2 * k4, db + 2 * k4, (kb | k4) ? 1u : 0u);
+          if (NPROD == 3) {
+            wgmma_bf16<BN, 0, 0>(acc, da + 2 * k4, db + kLoB + 2 * k4, 1u);
+            wgmma_bf16<BN, 0, 0>(acc, da + kLoA + 2 * k4, db + 2 * k4, 1u);
           }
-          umma_commit(empty0 + 8 * s);      // frees this smem stage once the MMAs above have read it
-          if (kb == nk - 1) umma_commit(tfull0 + 8 * buf);      // accumulator complete
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_fence_acc(acc);
+        wgmma_wait<1>();                      // the previous k-block's MMAs are done: its stage can be refilled
+        if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
+        prev = s;
       }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (leader) mbar_arrive(empty0 + 8 * prev);
+      epilogue_nt<BN>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane);
     }
-    if (lane == 0) {
-      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 2, w_tempty);
+    if (threadIdx.x == 0) {
       AVC_PROBE_ADD(EpiProbeId<Epi>::value, 3, w_full);
       AVC_PROBE_ADD(EpiProbeId<Epi>::value, 4, AVC_PROBE_NOW() - t_mma0);
     }
-  } else {
-    using Tr = EpiTraits<Epi>;
-    using Aux = typename Tr::Aux;
-    // Sub-blocks of 16 columns: the EW/4 warps of a TMEM lane quarter interleave them (NSUB per warp and tile).  The
-    // global loads of the epilogue that do not depend on the accumulator (stashed activations, biases: Epi::prefetch)
-    // are issued NPF sub-blocks ahead, across tile boundaries, so that they are in flight while the warp waits for
-    // the MMA and works through the previous sub-block.  Prefetch addresses are clamped into the matrix instead of
-    // predicated (no divergence, no zero-filling): a clamped value is never used.
-    constexpr int NSUB = BN / 16 / (EW / 4);
-    constexpr int NPF0 = PFB / (int)sizeof(Aux);       // PFB = registers per thread spent on operands in flight
-    constexpr int NPF = NPF0 < 1 ? 1 : (NPF0 >= NSUB ? NSUB : (NPF0 >= 2 && NSUB % 2 == 0 ? 2 : 1));
-    const int q = warp & 3;               // TMEM lane quarter this warp may access
-    const int cw = (warp - 2) >> 2;       // first sub-block of this warp
-    const int cg = (lane & 3) * 4, ri = lane >> 2;
-    // per-warp 32 x 16 fp32 transpose tile, 16-byte chunks XOR-swizzled with (row >> 1) & 3: the row-per-lane
-    // st.shared.v4 of the TMEM values and the 8-rows-x-4-chunks ld.shared.v4 of a pass are both conflict free
-    const uint32_t stage = smem_u32(epi_stage) + (uint32_t)(warp - 2) * 2048u;
-    const uint32_t st_row = stage + (uint32_t)lane * 64u, st_sw = (uint32_t)((lane >> 1) & 3);
-    const uint32_t ld_addr = stage + (uint32_t)ri * 64u + (uint32_t)(((lane & 3) ^ ((ri >> 1) & 3)) * 16);
-    const int col_last = (N - 1) & ~3, row_last = M - 1;
-    pdl_wait();      // the functor's operands and outputs belong to predecessor kernels
-    Aux aux[NPF][4];
-    auto issue = [&](Aux (&dst)[4], int mt, int sb) {
-      const int row = min(mt, tiles_m - 1) * kBM + q * 32 + ri;
-      const int col = min(n0 + (cw + sb * (EW / 4)) * 16 + cg, col_last);
-      EpiPrefetch4<Epi>::run(epi, row, row_last, col, dst);
-    };
-#pragma unroll
-    for (int s = 0; s < NPF; ++s) issue(aux[s], m_first, s);
-    int lt = 0;
-    AVC_PROBE_DECL(w_tfull);
-    const long long t_epi0 = AVC_PROBE_NOW();
-    const int et = (int)threadIdx.x - 64;
-    EpiL2<Epi>::run(epi, m_first * kBM, n0, BN, M, et, 32 * EW);
-    for (int mt = m_first; mt < tiles_m; mt += m_stride, ++lt) {
-      const int m0 = mt * kBM;
-      const uint32_t buf = lt % NBUF;
-      EpiL2<Epi>::run(epi, (mt + m_stride) * kBM, n0, BN, M, et, 32 * EW);     // a whole tile ahead of its use
-      AVC_PROBE_WAIT(w_tfull, tfull0 + 8 * buf, (lt / NBUF) & 1);
-      tc_fence_after();
-      const int row0 = m0 + q * 32;
-      const int nrows = min(32, M - row0);
-#pragma unroll
-      for (int sb = 0; sb < NSUB; ++sb) {
-        const int c = cw + sb * (EW / 4);
-        const int col0 = n0 + c * 16;
-        if (col0 < N && nrows > 0) {
-          uint32_t r[16];
-          tmem_ld16(tmem_base + buf * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 16), r);
-#pragma unroll
-          for (int c4 = 0; c4 < 4; ++c4)
-            st_shared_v4(st_row + (((uint32_t)c4 ^ st_sw) << 4), r[4 * c4], r[4 * c4 + 1], r[4 * c4 + 2], r[4 * c4 + 3]);
-          __syncwarp();
-          if (col0 + cg < N) {
-            if (nrows == 32) {      // full sub-block: no row guards, the four groups go to the functor together
-              float4 acc[4];
-#pragma unroll
-              for (int p = 0; p < 4; ++p) acc[p] = ld_shared_v4(ld_addr + (uint32_t)p * 512u);
-              EpiQuad<Epi>::run(epi, row0 + ri, col0 + cg, acc, aux[sb % NPF]);
-            } else {
-#pragma unroll
-              for (int p = 0; p < 4; ++p) {
-                const int i = ri + 8 * p;
-                if (i < nrows) Tr::apply(epi, row0 + i, col0 + cg, ld_shared_v4(ld_addr + (uint32_t)p * 512u), aux[sb % NPF][p]);
-              }
-            }
-          }
-          __syncwarp();
-        }
-        // refill the slot just consumed: NPF sub-blocks ahead in this warp's (tile, sub-block) sequence
-        issue(aux[sb % NPF], mt + ((sb + NPF) / NSUB) * m_stride, (sb + NPF) % NSUB);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * buf);    // this warp no longer reads accumulator `buf`
-    }
-    if (warp == 2 && lane == 0) {
-      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 5, w_tfull);
-      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 6, AVC_PROBE_NOW() - t_epi0);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, NBUF * BN);
   }
 }
 
-template <int BN, int NPROD, int EW, int PFB, bool RESB, typename Epi>
+template <int BN, int NPROD, bool RESB, typename Epi>
 static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K, const SplitPtr& A, const SplitPtr& B,
                                        const Epi& epi, bool b_const) {
-  using Cfg = TcCfg<BN, NPROD, EW, RESB>;
+  using Cfg = TcCfg<BN, NPROD, RESB>;
   CUtensorMap mAh, mAl, mBh, mBl;
   AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kBM));
   AVC_TRY(make_map_bf16_cached(&mBh, B.hi, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
@@ -609,7 +417,7 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
   } else {
     mAl = mAh; mBl = mBh;
   }
-  auto kern = gemm_tc_nt_kernel<BN, NPROD, EW, PFB, RESB, Epi>;
+  auto kern = gemm_tc_nt_kernel<BN, NPROD, RESB, Epi>;
   static thread_local bool attr_set = false;    // per template instantiation and host thread (= device)
   if (!attr_set) {
     AVC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -627,44 +435,40 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
   g = (g / tiles_n) * tiles_n;                         // ... and a whole number of CTAs per column tile
   if (g < tiles_n) return AVC_E_BADCFG;
   dim3 grid(g);
-  // TMA-prefetch of the next row tile's A boxes into L2.  The stall probe (profiles/r2_nt_probe_*.json) shows the MMA warp
-  // of the launches with a LIGHT epilogue waiting for operands ~50 % of its loop (two 32 KB stages do not cover a loaded
-  // DRAM latency); with the prefetch 40 % (EpiValue: loop 63.0 k -> 56.8 k cycles per CTA).  Launches whose epilogue is
-  // the bound and pulls its own operands into L2 (Epi::kNoATilePrefetch) got slower with it and keep it off.
+  // TMA-prefetch of the next row tile's A boxes into L2, so that the ring's loads see L2 rather than DRAM latency.
+  // Launches whose epilogue pulls its own operands into L2 (Epi::kNoATilePrefetch) keep it off.
   // AVC_NT_L2PF=0 / 1 forces it off / on everywhere.
   static int l2pf_env = -2;
   if (l2pf_env == -2) { const char* e = getenv("AVC_NT_L2PF"); l2pf_env = e ? (atoi(e) != 0 ? 1 : 0) : -1; }
   const int l2pf = l2pf_env >= 0 ? l2pf_env : (EpiNoAPf<Epi>::value ? 0 : 1);
-  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(64 + 32 * EW), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, l2pf, b_const ? 1 : 0));
+  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, l2pf, b_const ? 1 : 0));
   AVC_LAUNCH_TRY();
   return 0;
 }
 
-// N <= 64 -> one 64-wide tile, else 128-wide tiles: with one 256-wide tile per 128 rows a 65536-row GEMM would have
-// 512 tiles = 3.46 waves over 148 persistent CTAs (13 % tail); 1024 tiles = 6.9 waves (1.4 % tail).
+// N <= 64 -> one 64-wide tile, else 128-wide tiles (a 65536-row GEMM then has 1024 tiles = 7.8 waves over 132
+// persistent CTAs instead of 3.9 with 256-wide tiles: a smaller tail).
 template <int NPROD, typename Epi>
 static inline int launch_gemm_tc_nt(cudaStream_t st, int64_t M, int N, int K, const SplitPtr& A, const SplitPtr& B,
                                     const Epi& epi, bool b_const = false) {
   if (M <= 0 || N <= 0) return 0;
-  // 16 epilogue warps, one (32-byte operands) or two (16-byte operands) sub-blocks of prefetch.  Measured per step
-  // (73 launches, B200): 16 warps / 32 regs 3.01 ms, 16 / 16 3.02 ms, 8 warps / 64 regs 3.32 ms, 8 / 32 3.34 ms.
   // K <= 256: the B panel stays resident in shared memory (RESB); longer reductions stream both operands.
   static int resb = -1;       // AVC_NT_RESB=0 forces the streaming variant (tuning knob)
   if (resb < 0) { const char* e = getenv("AVC_NT_RESB"); resb = (e && atoi(e) == 0) ? 0 : 1; }
   if (resb && K <= kResK * kBK) {
-    if (N <= 64) return launch_gemm_tc_nt_bn<64, NPROD, 16, 32, true, Epi>(st, M, N, K, A, B, epi, b_const);
-    return launch_gemm_tc_nt_bn<128, NPROD, 16, 32, true, Epi>(st, M, N, K, A, B, epi, b_const);
+    if (N <= 64) return launch_gemm_tc_nt_bn<64, NPROD, true, Epi>(st, M, N, K, A, B, epi, b_const);
+    return launch_gemm_tc_nt_bn<128, NPROD, true, Epi>(st, M, N, K, A, B, epi, b_const);
   }
-  if (N <= 64) return launch_gemm_tc_nt_bn<64, NPROD, 16, 32, false, Epi>(st, M, N, K, A, B, epi, b_const);
-  return launch_gemm_tc_nt_bn<128, NPROD, 16, 32, false, Epi>(st, M, N, K, A, B, epi, b_const);
+  if (N <= 64) return launch_gemm_tc_nt_bn<64, NPROD, false, Epi>(st, M, N, K, A, B, epi, b_const);
+  return launch_gemm_tc_nt_bn<128, NPROD, false, Epi>(st, M, N, K, A, B, epi, b_const);
 }
 
 // ------------------------------------------------------------------------------------------------ TN kernel
 // C[i*ldc + j] += sum_{p in slice} A[p,i] * B[p,j]   (i < N1, j < N2): weight gradients.  Both operands are read
 // "MN-major": the reduction index p is the row of the global arrays.  TMA boxes are 64 (i or j) x 64 (p); in shared
-// memory one box is an MN atom block [64 p][128 B] (SWIZZLE_128B); a 128-wide M tile is 2 blocks, a BN-wide N tile
-// BN/64 blocks.  Descriptor: SBO = 1024 B (8 p-rows), LBO = 8192 B (next 64-wide block), a K step of 16 p-rows
-// is +2048 B.  Split over p across blockIdx.z; partial tiles meet in fp32 red.global.add.
+// memory one box is an MN block [64 p][128 B] (SWIZZLE_128B); a 128-wide M tile is 2 blocks (one per consumer
+// warpgroup), a BN-wide N tile BN/64 blocks.  Descriptor: LBO = 8192 B (next 64-wide block), SBO = 1024 B (8 p-rows), a K
+// step of 16 p-rows is +2048 B.  Split over p across blockIdx.z; partial tiles meet in fp32 red.global.add.
 template <int BN, int NPROD>
 struct TcTnCfg {
   static constexpr int BLK = kBK * 128;                             // one 64 x 64 bf16 block: 8 KB
@@ -672,10 +476,10 @@ struct TcTnCfg {
   static constexpr int B_BYTES = (BN / 64) * BLK;
   static constexpr int NOP = (NPROD == 3) ? 2 : 1;
   static constexpr int STAGE_BYTES = NOP * (A_BYTES + B_BYTES);
-  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES >= 4 ? 4 : ((200 * 1024) / STAGE_BYTES);
-  static constexpr int EPI_BYTES = kEpiWarps * 32 * 33 * 4;        // 33,792 B (a multiple of 1024: the ones tile stays aligned)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + EPI_BYTES;
-  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory per CTA");
+  static constexpr int kBudget = kSmemMax - 1024 /*align*/ - 1024 /*ones*/ - 256 /*barriers*/;
+  static constexpr int STAGES = kBudget / STAGE_BYTES >= 4 ? 4 : kBudget / STAGE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 1024 + 256;
+  static_assert(SMEM_BYTES <= kSmemMax, "exceeds the 227 KB of shared memory per CTA");
   static_assert(STAGES >= 2, "tile too large for shared memory");
 };
 
@@ -688,15 +492,12 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   using Cfg = TcTnCfg<BN, NPROD>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * Cfg::STAGES + 1);
-  float* epi_stage = (float*)(smem + Cfg::STAGES * Cfg::STAGE_BYTES + 256);
-  // 2 KB of bf16 1.0 aliased onto the epilogue staging area: the MMAs that read it have all completed (tfull) before
-  // any epilogue warp writes its staging tile
-  uint8_t* ones_tile = reinterpret_cast<uint8_t*>(epi_stage);
+  // 1 KB of bf16 1.0: the K-major B operand of the column-sum MMA (any layout of an all-ones tile is the all-ones tile)
+  uint8_t* ones_tile = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
+  uint64_t* bars = (uint64_t*)(ones_tile + 1024);
   const bool do_colsum = (colsum != nullptr) && (blockIdx.y == 0);
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * Cfg::STAGES, tfull = empty0 + 8 * Cfg::STAGES;
+  const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * Cfg::STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i0 = blockIdx.x * kBM, j0 = blockIdx.y * BN;
@@ -704,23 +505,18 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   const int p_end = min(P, p_begin + rows_per_split);
   const int nk = (p_end - p_begin + kBK - 1) / kBK;     // host guarantees rows_per_split % 64 == 0 and nk >= 1
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&mapAhi); tma_prefetch_desc(&mapBhi);
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-    mbar_init(tfull, 1);
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 2 * BN);   // BN accumulator columns + 16 for the column sums (power of 2)
-  if (do_colsum) {   // any layout of an all-ones tile is the all-ones tile
-    for (int i = threadIdx.x; i < 2048 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(ones_tile)[i] = 0x3F803F80u;
+  if (do_colsum) {
+    for (int i = threadIdx.x; i < 1024 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(ones_tile)[i] = 0x3F803F80u;
     fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       pdl_wait();         // both operands are activations of predecessor kernels
       pdl_trigger();
@@ -745,69 +541,69 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // converged warp, one elected lane issues (see the NT kernel)
-    constexpr uint32_t idesc = make_idesc_bf16(kBM, BN, 1, 1);
-    constexpr uint32_t idesc1 = make_idesc_bf16(kBM, 16, 1, 1);
-    const uint32_t ones_addr = smem_u32(ones_tile);
+  } else {
+    const int g = warp >> 2, wq = warp & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const uint64_t dones = make_wgmma_desc(smem_u32(ones_tile), 16, 1024);
+    float acc[BN / 2], cs[4];
+    int prev = -1;
     for (int kb = 0; kb < nk; ++kb) {
       const int s = kb % Cfg::STAGES;
       mbar_wait(full0 + 8 * s, (kb / Cfg::STAGES) & 1);
-      tc_fence_after();
-      if (elect_one_sync()) {
-        const uint32_t a_hi = smem_base + s * Cfg::STAGE_BYTES;
-        const uint32_t b_hi = a_hi + Cfg::NOP * Cfg::A_BYTES;
-        // MN-major: a K step of 16 p-rows is +2048 B = +128 in the descriptor's start-address field
-        const uint64_t da = make_smem_desc(a_hi, Cfg::BLK, 1024), db = make_smem_desc(b_hi, Cfg::BLK, 1024);
-        const uint64_t dones = make_smem_desc(ones_addr, Cfg::BLK, 1024);
-        constexpr uint64_t kLoA = (uint64_t)(Cfg::A_BYTES >> 4), kLoB = (uint64_t)(Cfg::B_BYTES >> 4);
+      const uint32_t a_hi = smem_base + s * Cfg::STAGE_BYTES + (uint32_t)g * Cfg::BLK;   // this warpgroup's 64 columns i
+      const uint32_t b_hi = smem_base + s * Cfg::STAGE_BYTES + Cfg::NOP * Cfg::A_BYTES;
+      const uint64_t da = make_wgmma_desc(a_hi, Cfg::BLK, 1024), db = make_wgmma_desc(b_hi, Cfg::BLK, 1024);
+      constexpr uint64_t kLoA = (uint64_t)(Cfg::A_BYTES >> 4), kLoB = (uint64_t)(Cfg::B_BYTES >> 4);
+      wgmma_fence_acc(acc);
+      wgmma_fence_acc(cs);
+      // the column-sum switch is decided outside the batch: a branch between the MMAs of a batch would make the compiler
+      // serialise them
+      auto batch = [&](auto with_colsum) {
+        wgmma_fence();
 #pragma unroll
         for (int k4 = 0; k4 < kBK / 16; ++k4) {
-          umma_f16(tmem_base, da + 128 * k4, db + 128 * k4, idesc, (kb | k4) ? 1u : 0u);
+          wgmma_bf16<BN, 1, 1>(acc, da + 128 * k4, db + 128 * k4, (kb | k4) ? 1u : 0u);
           if (NPROD == 3) {
-            umma_f16(tmem_base, da + 128 * k4, db + kLoB + 128 * k4, idesc, 1u);
-            umma_f16(tmem_base, da + kLoA + 128 * k4, db + 128 * k4, idesc, 1u);
+            wgmma_bf16<BN, 1, 1>(acc, da + 128 * k4, db + kLoB + 128 * k4, 1u);
+            wgmma_bf16<BN, 1, 1>(acc, da + kLoA + 128 * k4, db + 128 * k4, 1u);
           }
-          if (do_colsum) {      // D2[128 x 16] += A^T . ones : every column of D2 is the column sum of A
-            umma_f16(tmem_base + BN, da + 128 * k4, dones, idesc1, (kb | k4) ? 1u : 0u);
-            if (NPROD == 3) umma_f16(tmem_base + BN, da + kLoA + 128 * k4, dones, idesc1, 1u);
+          if constexpr (decltype(with_colsum)::value) {      // cs[64 x 8] += A^T . ones: every column is A's column sum
+            wgmma_bf16<8, 1, 0>(cs, da + 128 * k4, dones, (kb | k4) ? 1u : 0u);
+            if (NPROD == 3) wgmma_bf16<8, 1, 0>(cs, da + kLoA + 128 * k4, dones, 1u);
           }
         }
-        umma_commit(empty0 + 8 * s);
-        if (kb == nk - 1) umma_commit(tfull);
-      }
-      __syncwarp();
+        wgmma_commit();
+      };
+      if (do_colsum) batch(std::true_type{});
+      else batch(std::false_type{});
+      wgmma_fence_acc(acc);
+      wgmma_fence_acc(cs);
+      wgmma_wait<1>();
+      if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
+      prev = s;
     }
-  } else {
-    const int q = warp & 3;
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(cs);
+    if (leader) mbar_arrive(empty0 + 8 * prev);
     pdl_wait();           // C is accumulated with atomics: not before the predecessors have drained
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    const int row0 = i0 + q * 32;
-    const int nrows = min(32, N1 - row0);
-    float* stage = epi_stage + (warp - 2) * 32 * 33;
-#pragma unroll 1
-    for (int c = (warp - 2) >> 2; c < BN / 32; c += kEpiWarps / 4) {
-      const int col0 = j0 + c * 32;
-      if (col0 >= N2) break;
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-      if (nrows > 0)
-        epilogue_block_transposed(stage, r, lane, row0, nrows, col0, min(32, N2 - col0),
-                                  [&](int rr, int cc, float v) { atomicAdd(C + (size_t)rr * ldc + cc, v); });
+    const int r0 = i0 + 64 * g + 16 * wq + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = j0 + 8 * j + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        if (r < N1) {
+          if (c < N2) atomicAdd(C + (size_t)r * ldc + c, acc[4 * j + 2 * h]);
+          if (c + 1 < N2) atomicAdd(C + (size_t)r * ldc + c + 1, acc[4 * j + 2 * h + 1]);
+        }
+      }
     }
-    if (do_colsum && warp < 6) {   // warps 2-5: one per TMEM lane quarter
-      uint32_t r16[16];
-      tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)BN, r16);
-      if (row0 + lane < N1) atomicAdd(colsum + row0 + lane, __uint_as_float(r16[0]));
+    if (do_colsum && (lane & 3) == 0) {
+      if (r0 < N1) atomicAdd(colsum + r0, cs[0]);
+      if (r0 + 8 < N1) atomicAdd(colsum + r0 + 8, cs[2]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * BN);
   }
 }
 

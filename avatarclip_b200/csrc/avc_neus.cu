@@ -26,11 +26,11 @@ namespace {
 inline int blocks_for(int64_t n, int threads) { return (int)((n + threads - 1) / threads); }
 
 // -------------------------------------------------------------------------------- engine dispatch
-// engine 0: fp32 FFMA tiles on the fp32 buffers; engine 1: tcgen05 tiles on the two-term bf16 copies.
+// engine 0: fp32 FFMA tiles on the fp32 buffers; engine 1: wgmma tiles on the two-term bf16 copies.
 // B operands are addressed by their offset in the packed-weight buffer (same offset in the bf16 split).
 inline Split16 with_ld(Split16 s, int ld) { s.ld = ld; return s; }
 
-// NP: MMAs per product on the tcgen05 engine: 3 = two-term split operands, 1 = the hi halves only (single-pass bf16).
+// NP: MMAs per product on the wgmma engine: 3 = two-term split operands, 1 = the hi halves only (single-pass bf16).
 template <int NP = 3, typename Epi>
 int gemm_nt(const NeusPlan& pl, const NeusWs& w, cudaStream_t st, int64_t M, int N, int K, const float* A, int lda,
             const Split16& A16, int64_t pk_off, int ldb, const Epi& epi) {
@@ -53,11 +53,8 @@ int gemm_nt_color(const NeusPlan& pl, const NeusWs& w, cudaStream_t st, int64_t 
 
 int colsum(cudaStream_t st, const float* X, int ld, int NC, int64_t P, float scale, float* out);
 
-// (Measured and removed, r2: recording the ~21 weight-gradient GEMMs of a backward and running them as ONE persistent grouped
-// launch at the end -- a stand-alone launch has 9.5 us of fixed cost, profiles/r2_tn_scaling_probe.json -- gave 4.734 vs
-// 4.732 ms per step: under programmatic dependent launch the interleaved launches already hide that cost.)
 // C[N1][ldc] += A^T B ; optionally bias_out[i] += sum_p A[p,i] (the bias gradient of the same linear): fused into the
-// tcgen05 kernel as one extra 16-wide MMA against a tile of ones, a separate column-sum kernel for the fp32 engine.
+// wgmma kernel as one extra 8-wide MMA against a tile of ones, a separate column-sum kernel for the fp32 engine.
 inline int gemm_tn(const NeusPlan& pl, const NeusWs& w, cudaStream_t st, int64_t P, int N1, int N2, const float* A,
                    int lda, const Split16& A16, const float* B, int ldb, const Split16& B16, float* C, int ldc,
                    float* bias_out = nullptr, bool single = false) {
@@ -142,7 +139,7 @@ int zero_pack(const NeusPlan& pl, float* pack, cudaStream_t st) {
   return 0;
 }
 
-// zero + pack (+ bf16 split for the tcgen05 engine)
+// zero + pack (+ bf16 split for the wgmma engine)
 int prepare_weights(const NeusPlan& pl, const NeusWs& w, const float* params, cudaStream_t st) {
   AVC_TRY(zero_pack(pl, w.pack, st));
   AVC_TRY(pack_weights(pl, params, w.pack, st));
@@ -158,7 +155,7 @@ int prepare_weights(const NeusPlan& pl, const NeusWs& w, const float* params, cu
 EncodeTargets make_targets(const NeusPlan& pl, const NeusWs& w) {
   EncodeTargets t;
   memset(&t, 0, sizeof(t));
-  const bool tc1 = pl.cfg.engine == 1;      // tcgen05 engine: every consumer of the encoding reads the bf16 pairs ...
+  const bool tc1 = pl.cfg.engine == 1;      // wgmma engine: every consumer of the encoding reads the bf16 pairs ...
   t.in0 = tc1 ? nullptr : w.in[0]; t.ld0 = pl.sdf[0].Kp;
   t.in0_16 = w.in16[0];
   for (int l = 1; l <= pl.L; ++l) {
@@ -176,7 +173,7 @@ EncodeTargets make_targets(const NeusPlan& pl, const NeusWs& w) {
 // -------------------------------------------------------------------------------- value chain
 // in[0] (and the skip columns) must hold the encoding of Pn points.  stash: keep z[l].
 // Leaves in[L] ready; writes sdf[Pn] (thin) and, when want_feat, feat[Pn][Fp].
-// tcgen05 engine, no stash, no features (sample placement, sdf queries): the whole chain of a 128-point tile in ONE
+// wgmma engine, no stash, no features (sample placement, sdf queries): the whole chain of a 128-point tile in ONE
 // kernel (avc_chain.cu), activations resident in shared memory.  Returns 1 when the fused kernel does not cover this
 // network shape (the caller then runs the layer-by-layer launches), 0 on success.
 int value_chain_fused(const NeusPlan& pl, const NeusWs& w, int64_t Pn, float* sdf_out, cudaStream_t st, int sdf_nz,
@@ -223,7 +220,7 @@ int value_chain(const NeusPlan& pl, const NeusWs& w, int64_t Pn, bool stash, boo
     EpiValue<false> e;
     e.bias = pack + d.pk_b;
     e.D1 = stash ? w.z[l] : nullptr; e.ldz = d.Np;     // w.z[l] holds softplus'(z_l), see EpiValue
-    // tcgen05 engine: the fp32 copy of a hidden activation is only read by the thin sdf head (layer L)
+    // wgmma engine: the fp32 copy of a hidden activation is only read by the thin sdf head (layer L)
     e.OUT = (pl.cfg.engine == 1 && l + 1 < pl.L) ? nullptr : w.in[l + 1]; e.ldo = pl.sdf[l + 1].Kp;
     e.oscale = pl.sdf[l + 1].skip ? kSqrtHalf : 1.f;
     e.N = d.N;
@@ -241,7 +238,7 @@ int value_chain(const NeusPlan& pl, const NeusWs& w, int64_t Pn, bool stash, boo
                                                            pack + pl.pk_bsdf, Pn, os);
   AVC_LAUNCH_TRY();
   if (want_feat) {
-    // tcgen05 engine: every consumer of the features reads the split (colour lin0 A operand, its weight gradient)
+    // wgmma engine: every consumer of the features reads the split (colour lin0 A operand, its weight gradient)
     EpiBias e{pack + dl.pk_b, pl.cfg.engine == 1 ? nullptr : w.feat, pl.Fp, pl.F, w.feat16};
     AVC_TRY(gemm_nt(pl, w, st, Pn, pl.F, dl.K, w.in[pl.L], dl.Kp, w.in16[pl.L], dl.pk_W, dl.Kp, e));
   }
@@ -255,7 +252,7 @@ int gradient_chain(const NeusPlan& pl, const NeusWs& w, int64_t P, float* grad_o
   const float* pack = w.pack;
   const LinDim& dL = pl.sdf[pl.L];
   const LinDim& dp = pl.sdf[pl.L - 1];
-  // tcgen05 engine: qt_l is only ever consumed as a split operand (gradient chain, second-order sweep, dW)
+  // wgmma engine: qt_l is only ever consumed as a split operand (gradient chain, second-order sweep, dW)
   const bool tc1 = pl.cfg.engine == 1;
   int64_t tot = P * (int64_t)(dp.Np / 4 > pl.EP ? dp.Np / 4 : pl.EP);   // threads: 4 qt columns each, 1 ge entry each
   k_chain_start<<<blocks_for(tot, 256), 256, 0, st>>>(pack + pl.pk_wsdf, dL.K, dL.skip ? 1 : 0, pl.E, pl.EP,
@@ -353,7 +350,7 @@ int fine_forward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, bool wr
   // ---- colour net
   {
     const LinDim& c0 = pl.col[0];
-    // tcgen05 engine: the fp32 copy of a hidden colour activation is only read by the heads (layer Lc)
+    // wgmma engine: the fp32 copy of a hidden colour activation is only read by the heads (layer Lc)
     const bool tc1 = pl.cfg.engine == 1;
     // ... and the split of the LAST hidden activation has no reader at all (the heads and their backward are thin fp32 ops)
     const Split16 none16{nullptr, nullptr, 0};
@@ -431,7 +428,7 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
     // both heads read the same activation: one pass, rows 0..2 -> lin{Lc}, rows 3..5 -> extra_lin
     AVC_TRY(thin_tn<6>(st, w.y6bar, 8, 1.f, w.ch[pl.Lc], pl.Hc, pl.Hc, P, wbar + dh.off_v, pl.Hc, 1, wbar + dh.off_b, 3,
                        wbar + dx.off_v, wbar + dx.off_b));
-    // tcgen05 engine: the hidden linears consume cbar as a split operand; its fp32 copy is only read at layer 0
+    // wgmma engine: the hidden linears consume cbar as a split operand; its fp32 copy is only read at layer 0
     k_heads_dgrad<<<blocks_for(P * pl.Hc / 4, 256), 256, 0, st>>>(w.y6bar, pack + pl.pk_W6, pl.Hc, w.ch[pl.Lc], P,
                                                               (pl.cfg.engine == 1 && pl.Lc > 1) ? nullptr : w.cbar[0],
                                                               w.cbar16[0]);
@@ -445,7 +442,7 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
     if (l > 0) {
       AVC_TRY(gemm_tn(pl, w, st, P, pl.Hc, pl.Hc, cb, pl.Hc, w.cbar16[cur], w.ch[l], pl.Hc, w.ch16[l], wbar + c.off_v, c.K,
                       wbar + c.off_b, color_single(pl)));
-      // tcgen05 engine: ReLU mask from the split of ch[l]; the fp32 copy of cbar is only read at layer 0 (thin ops)
+      // wgmma engine: ReLU mask from the split of ch[l]; the fp32 copy of cbar is only read at layer 0 (thin ops)
       const bool tc1 = pl.cfg.engine == 1;
       EpiDgradRelu e{tc1 ? nullptr : w.ch[l], w.ch16[l].hi, (tc1 && l > 1) ? nullptr : w.cbar[cur ^ 1], pl.Hc,
                      w.cbar16[cur ^ 1]};
@@ -471,7 +468,7 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
   int ucur = 0;
   {
     const LinDim& d0 = pl.sdf[0];
-    // tcgen05 engine: ubar_0 is only consumed as a split operand
+    // wgmma engine: ubar_0 is only consumed as a split operand
     k_dge<<<blocks_for(P * 8, 256), 256, 0, st>>>(w.cin, w.nbar, pl.EP, pl.E, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P,
                                                   pl.cfg.engine == 1 ? nullptr : w.ubar[0], d0.Kp, w.gebar,
                                                   with_ld(w.ubar16[0], d0.Kp));
@@ -491,7 +488,7 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
     EpiChainBwd e;
     e.N = d.N; e.Np = d.Np; e.D1 = w.z[l]; e.QT = pl.cfg.engine == 1 ? nullptr : w.qt[l]; e.qt16 = w.qt16[l];
     e.ZBAR = w.zbar[l];
-    // tcgen05 engine: the fp32 copy of ubar_{l+1} is only read by the column sum at the last linear
+    // wgmma engine: the fp32 copy of ubar_{l+1} is only read by the column sum at the last linear
     e.UNEXT = (pl.cfg.engine == 1 && l + 1 < pl.L) ? nullptr : w.ubar[ucur ^ 1];
     e.ldu = dn.Kp; e.s_next = dn.skip ? kSqrtHalf : 1.f;
     // the pair of ubar_L has no reader (the last linear only needs the column sum of the fp32 copy)
@@ -588,7 +585,7 @@ extern "C" {
 
 int avc_abi_version(void) { return AVC_ABI_VERSION; }
 
-// Stall probe of the tcgen05 NT tiles (diagnostic builds only: -DAVC_NT_PROBE=1).  out[16][8]: per functor slot the summed
+// Stall probe of the wgmma NT tiles (diagnostic builds only: -DAVC_NT_PROBE=1).  out[16][8]: per functor slot the summed
 // cycles {TMA waits empty, TMA loop, MMA waits tempty, MMA waits full, MMA loop, epilogue warp waits tfull, epilogue loop,
 // CTAs}.  Returns AVC_E_BADCFG in a regular build.
 int avc_nt_probe_read(unsigned long long* host_out, int reset) {
@@ -606,7 +603,7 @@ int avc_nt_probe_read(unsigned long long* host_out, int reset) {
   return AVC_E_BADCFG;
 #endif
 }
-const char* avc_build_arch(void) { return "sm_100a"; }
+const char* avc_build_arch(void) { return "sm_90a"; }
 
 int avc_neus_param_count(const avc_neus_cfg* cfg, int64_t* n_params) {
   if (!cfg || !n_params) return AVC_E_NULL;

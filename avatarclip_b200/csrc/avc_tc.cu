@@ -1,4 +1,4 @@
-// avc_tc.cu -- self-test entry points of the tcgen05 GEMM tiles (used by tests/test_tc_gemm_gpu.py).
+// avc_tc.cu -- self-test entry points of the wgmma GEMM tiles (used by tests/test_tc_gemm_gpu.py).
 #include "avc_gemm_tc.cuh"
 
 using namespace avc;
@@ -15,7 +15,7 @@ struct EpiPlainStore {
 
 extern "C" {
 
-// C[M][N] = A[M][K] . B[N][K]^T through the tcgen05 NT tiles.  nprod = 1 (single bf16 product) or 3 (two-term split).
+// C[M][N] = A[M][K] . B[N][K]^T through the wgmma NT tiles.  nprod = 1 (single bf16 product) or 3 (two-term split).
 // workspace >= 4 * (M + N) * round_up(K, 8) bytes.
 int avc_tc_gemm_nt_test(const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t nprod, float* C,
                         void* workspace, size_t workspace_bytes, avc_stream_t stream) {
@@ -38,7 +38,7 @@ int avc_tc_gemm_nt_test(const float* A, const float* B, int64_t M, int32_t N, in
   return tc::launch_gemm_tc_nt<1, EpiPlainStore>(st, M, N, K, a, b, e);
 }
 
-// C[N1][N2] += A[P][N1]^T . B[P][N2] through the tcgen05 TN (MN-major) tiles.  C must be initialised by the caller.
+// C[N1][N2] += A[P][N1]^T . B[P][N2] through the wgmma TN (MN-major) tiles.  C must be initialised by the caller.
 // workspace >= 4 * P * (round_up(N1,8) + round_up(N2,8)) + 2048 bytes.
 int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, int32_t N2, int32_t nprod, float* C,
                         float* colsum, void* workspace, size_t workspace_bytes, avc_stream_t stream) {

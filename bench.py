@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- appearance-optimisation steps/s (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- appearance-optimisation steps/s (BASELINE.json metric) on N H100s of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): one train_clip step = render 512 rays x (64+64) samples through the 8x256
 SDF + 4x256 colour MLPs (placement + fine pass), shading/canvas/losses on a 224x224 canvas, CLIP ViT-B/32 on the
@@ -35,9 +35,6 @@ METRIC = "appearance-optim steps/sec (512 rays x 128 samples, CLIP loss)"
 # config.workload of BOTH arms (the native line and `--impl reference`): the same string, so the two lines name one workload
 WORKLOAD = ("BASELINE configs[1]: 512 rays x (64+64) samples, 8x256 SDF + 4x256 colour, "
             "CLIP ViT-B/32 loss on 2 canvases 224x224, Adam; 1 view per GPU per step")
-# dram__bytes_read.sum + dram__bytes_write.sum per launch, ncu (profiles/r2_launches_tcgen05_engine.txt, final round-2
-# build): mean over the 41 NT / 21 TN launches of one step (all in the fine pass; 11.1 GB of DRAM traffic per step in total)
-TRAFFIC_PER_LAUNCH = {"avc::tc::gemm_tc_tn_kernel": 128.0e6, "avc::tc::gemm_tc_nt_kernel": 188.6e6}
 N_RAYS, CANVAS = 512, 224
 SDF_KW, COL_KW, REN_KW = WL.B2_SDF_KW, WL.B2_COL_KW, WL.B2_REN_KW
 VARIANCE = 0.3
@@ -94,11 +91,9 @@ def host_cores() -> int:
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1425.6), d.get("hbm_gbs", 6566.4), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    """Dense BF16 tensor rate and HBM3 bandwidth from NVIDIA's H100 SXM data sheet (a 700 W card): upper bounds, not
+    rates measured on the card at hand (its power limit is in the JSON line's `clocks`)."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense BF16, HBM3; 700 W)"
 
 
 class ClockSampler:
@@ -108,8 +103,16 @@ class ClockSampler:
 
     def __init__(self, gpu_index=0):
         self.rows, self.proc, self.gpu = [], None, gpu_index
+        self.gpu_name, self.power_limit = None, None
 
     def start(self):
+        try:      # the card and its power limit are part of every number this run reports
+            r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits",
+                                "-i", str(self.gpu)], capture_output=True, text=True, timeout=30)
+            name, limit = [c.strip() for c in r.stdout.strip().split(",")[:2]]
+            self.gpu_name, self.power_limit = name, float(limit)
+        except Exception:
+            pass
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
                                           "-lms", "100", "-i", str(self.gpu)], stdout=subprocess.PIPE, text=True)
@@ -139,7 +142,7 @@ class ClockSampler:
                     if v.lower().startswith("active"):
                         reasons.add(name)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "reasons": sorted(reasons), "samples": len(sm), "gpu": self.gpu_name, "power_limit_w": self.power_limit}
 
 
 def synth_weights():
@@ -215,6 +218,26 @@ def count_my_launches(fn):
         return None, None, {"error": repr(e)}
 
 
+def snapshot_outputs(tr, loss):
+    """What the timed step hands its caller, as float32 host arrays: the loss, the two CLIP cosines and the rendered
+    colours / opacities of the step, and the flat gradient and parameters (after Adam) it leaves in the trainer."""
+    out = {"loss": loss.reshape(1), "clip_cos": tr.cos, "color_fine": tr._out["color_fine"],
+           "extra_color_fine": tr._out["extra_color_fine"], "weight_sum": tr._out["weight_sum"],
+           "grad": tr.grad, "params": tr.fp.flat}
+    return {k: v.detach().float().cpu().numpy() for k, v in out.items()}
+
+
+def write_outputs(dirname, arrays, limit_bytes=64 << 20):
+    """DIR/<name>.npy for every array (float32); refuses to write more than limit_bytes in all."""
+    import numpy as np
+    total = sum(a.nbytes for a in arrays.values())
+    if total > limit_bytes:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {limit_bytes}-byte limit")
+    os.makedirs(dirname, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(dirname, k + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def run_native(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -262,7 +285,7 @@ def run_native(args):
     barrier()
     # one extra step on EVERY rank (it contains the all-reduce); only rank 0 records it with CUPTI
     launches_per_step, total_launches, table = (None, None, {})
-    # The profiled step runs with PLAIN launches of the tcgen05 NeuS kernels (AVC_TC_PDL=0, read per launch): under
+    # The profiled step runs with PLAIN launches of the wgmma NeuS kernels (AVC_TC_PDL=0, read per launch): under
     # programmatic dependent launch a kernel's CUPTI record starts when its first CTA becomes resident and includes the
     # wait for its predecessor, so durations overlap; the roofline wants the kernel's own duration.
     old_pdl = os.environ.get("AVC_TC_PDL")
@@ -299,10 +322,11 @@ def run_native(args):
 
     ev[0].record()
     for i in range(K):
-        one_step(i)
+        loss_t = one_step(i)
     ev[1].record()
     barrier()
     ms_value = ev[0].elapsed_time(ev[1])
+    dumped = snapshot_outputs(tr, loss_t) if args.dump_outputs and rank == 0 else None
     clocks = sampler.stop() if rank == 0 else None
 
     # render-only share (events around the two render calls) for the roofline of the MLP contractions
@@ -373,7 +397,7 @@ def run_native(args):
         plain = {k: v for k, v in table.items() if isinstance(v, list) and k.startswith("avc::")}
         dom = max(plain.items(), key=lambda kv: kv[1][1])[0] if plain else None
         # dominant kernel: algorithmic FLOP its launches execute per step / the sum of their device durations in the
-        # profiled step (CUPTI kernel records taken live in this process, not under ncu)
+        # profiled step (CUPTI kernel records taken live in this process)
         kern_us = {k: v for k, v in table.items() if isinstance(v, list)}
         chain_on = "avc::chain::k_sdf_chain" in kern_us
         if chain_on:
@@ -392,8 +416,8 @@ def run_native(args):
             "warmup": Wm, "ms_per_step": ms_value / K, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32" if args.engine == 0 else "bf16x3(split)->f32", "data": "synthetic",
             "config": {"workload": WORKLOAD,
-                       "views_per_step": world, "engine": "fp32 FFMA tiles" if args.engine == 0 else "tcgen05 split",
-                       "l2": "per-step working set (activation stash ~2.4 GB) >> 126 MB L2; no flush needed",
+                       "views_per_step": world, "engine": "fp32 FFMA tiles" if args.engine == 0 else "wgmma split",
+                       "l2": "per-step working set (activation stash ~2.4 GB) >> 50 MB L2; no flush needed",
                        "parallelism": f"view-sharded dp{world}" if world > 1 else "single",
                        "launch": ("one CUDA graph per step" + ((" (NCCL all-reduce + Adam captured inside)" if tr._graph_has_adam
                                                                  else " + all-reduce + Adam after it") if world > 1 else ""))
@@ -405,7 +429,6 @@ def run_native(args):
             "clocks": clocks,
             "roofline": {"bound": "tensor", "kernel": dom, "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                          "frac": achieved / peak_tf,
-                         "traffic": TRAFFIC_PER_LAUNCH.get(dom),
                          "per_launch": per_launch,
                          "scope": "algorithmic FLOP executed by the dominant kernel's launches in one step (SURVEY 8d "
                                   "split: NT tiles 4.875 F_sdf + 2 F_col per point -- 4.0 F_sdf when the fused value-chain "
@@ -449,6 +472,8 @@ def run_native(args):
             if args.ref_gpu:
                 line["ref_gpu"] = reference_gpu(sp, cp, clip_sd, text, device, steps=max(5, min(K, 20)))
         real_stdout.emit(json.dumps(line))
+        if dumped is not None:
+            write_outputs(args.dump_outputs, dumped)
     if world > 1:
         tr.release_graph()          # the graph may hold the NCCL all-reduce: it has to go before the communicator
         del tr
@@ -749,7 +774,7 @@ model {{
                 "ms_per_step": ms / K, "higher_is_better": True, "scaling": scaling, "vs_baseline": None,
                 "dtype": "f32" if args.engine == 0 else "bf16x3(split)->f32", "data": "synthetic",
                 "config": {"workload": workload, "baseline_config": cfg, "parallelism": f"view-sharded dp{world}" if world > 1 else "single",
-                           "launch": "eager C-ABI calls", "l2": "working set >> 126 MB L2"},
+                           "launch": "eager C-ABI calls", "l2": "working set >> 50 MB L2"},
                 "clocks": clocks, "last_loss": float(tr.loss_value()) if cfg in (2, 3) else float(r.trainer.loss_value())}
         for k, v in extra.items():
             if not torch.is_tensor(v):
@@ -766,7 +791,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--engine", type=int, default=int(os.environ.get("AVC_ENGINE", "1")),
-                    help="MLP contraction engine: 1 = tcgen05 split-bf16 tiles (default), 0 = fp32 FFMA tiles")
+                    help="MLP contraction engine: 1 = wgmma split-bf16 tiles (default), 0 = fp32 FFMA tiles")
     ap.add_argument("--graph", type=int, default=int(os.environ.get("AVC_GRAPH", "1")),
                     help="1: replay the step as one captured CUDA graph (default); 0: eager C-ABI calls")
     ap.add_argument("--config", type=int, default=1, choices=[1, 2, 3, 4],
@@ -777,7 +802,14 @@ def main():
                     help="skip the cpu_baseline / parity / ref_gpu legs (kernel experiments)")
     ap.add_argument("--cpu-budget-s", type=float, default=20.0, help="CPU seconds the cpu_baseline leg may spend on steps")
     ap.add_argument("--ref-gpu", type=int, default=1, help="1: also time the unmodified reference renderer on this GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (loss, CLIP cosines, rendered colours, "
+                         "gradient, parameters) to DIR/<name>.npy as float32 (native arm, --config 1)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl != "native" or args.config != 1):
+        ap.error("--dump-outputs applies to the native arm of --config 1")
     if args.warmup < 3 and args.impl == "native":
         args.warmup = 3
     if args.impl == "reference":

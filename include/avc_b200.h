@@ -1,4 +1,4 @@
-/* avc_b200.h -- C ABI of libavc_b200.so: B200-native (sm_100a) kernels for the AvatarCLIP
+/* avc_b200.h -- C ABI of libavc_b200.so: H100-native (sm_90a) kernels for the AvatarCLIP
  * appearance-optimisation hot path.
  *
  * The reference (hongfz16/AvatarCLIP, AvatarGen/AppearanceGen) is pure Python/PyTorch and has
@@ -39,7 +39,7 @@ typedef void* avc_stream_t; /* cudaStream_t */
 
 #define AVC_ABI_VERSION 3
 int avc_abi_version(void);
-/* Compiled-for architecture string, e.g. "sm_100a". */
+/* Compiled-for architecture string, e.g. "sm_90a". */
 const char* avc_build_arch(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -69,13 +69,13 @@ typedef struct avc_neus_cfg {
   int32_t n_importance;
   int32_t up_sample_steps;
   /* arithmetic engine for the MLP contractions: 0 = fp32 CUDA-core (FFMA) tiles,
-   * 1 = tcgen05 tensor-core tiles with two-term split operands (3 MMAs per product) */
+   * 1 = wgmma tensor-core tiles with two-term split operands (3 MMAs per product) */
   int32_t engine;
-  /* tcgen05 engine only: MMAs per product in the COLOUR net (forward, dgrad, wgrad).  3 (or 0) = the same two-term split
+  /* wgmma engine only: MMAs per product in the COLOUR net (forward, dgrad, wgrad).  3 (or 0) = the same two-term split
    * as the SDF trunk; 1 = single-pass bf16 on the hi halves (SURVEY.md Appendix C: the colour net tolerates it in the
    * rendered RGB; the flat parameter gradient moves from ~4e-5 to 3e-4 .. 1e-3 rel-L2, DESIGN.md 3.1). */
   int32_t color_products;
-  /* tcgen05 engine only: MMAs per product in the WEIGHT-GRADIENT tiles (dW += zbar^T in, qt^T ubar, ... : sums over all
+  /* wgmma engine only: MMAs per product in the WEIGHT-GRADIENT tiles (dW += zbar^T in, qt^T ubar, ... : sums over all
    * sample points of a chunk).  3 (or 0) = two-term split operands; 1 = single-pass bf16 on the hi halves. */
   int32_t wgrad_products;
 } avc_neus_cfg;
@@ -311,7 +311,7 @@ int avc_lbs_fwd(const float* v_shaped, const float* pose, int32_t pose2rot, cons
                 size_t workspace_bytes, avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Self-test of the tcgen05 GEMM tiles (engine 1): C[M][N] = A[M][K] . B[N][K]^T, fp32 in/out, operands
+ * Self-test of the wgmma GEMM tiles (engine 1): C[M][N] = A[M][K] . B[N][K]^T, fp32 in/out, operands
  * split into bf16 (hi, lo) pairs; nprod = 1 (hi*hi only) or 3 (hi*hi + hi*lo + lo*hi).
  * workspace >= 4 * (M + N) * round_up(K, 8) + 1024 bytes.
  * ------------------------------------------------------------------------------------------ */
@@ -365,7 +365,7 @@ int avc_uniform_fill(uint32_t seed, int32_t n, float lo, float hi, float* out, a
  * counters ([0] MMA warp waiting for its A operand, [1] for weight slabs, [2] MMA warp total, [3] tile-layers,
  * [4] epilogue waiting for the accumulator, [5] epilogue work); this call synchronises the device and copies them. */
 int avc_chain_debug_read(long long* out8);
-/* Stall probe of the tcgen05 NT tiles: only in a diagnostic build (-DAVC_NT_PROBE=1, tools/nt_probe.py); a regular
+/* Stall probe of the wgmma NT tiles: only in a diagnostic build (-DAVC_NT_PROBE=1, tools/nt_probe.py); a regular
  * build returns AVC_E_BADCFG.  host_out[16][8]: per epilogue functor the summed cycles {TMA warp waiting for a free
  * stage, TMA loop, MMA warp waiting for a drained accumulator, MMA warp waiting for operands, MMA loop, one epilogue
  * warp waiting for the accumulator, its loop, CTAs}; reset != 0 clears the counters. */

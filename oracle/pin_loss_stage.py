@@ -35,7 +35,7 @@ import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/AvatarGen/AppearanceGen"
+REF = os.path.join(os.environ.get("AVC_REFERENCE", "/root/reference"), "AvatarGen/AppearanceGen")
 
 from oracle import clip_vit as cv          # noqa: E402
 from oracle import loss as ol              # noqa: E402

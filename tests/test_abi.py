@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(L, s), s
     assert L.avc_abi_version() == 3
-    assert L.avc_build_arch() == b"sm_100a"
+    assert L.avc_build_arch() == b"sm_90a"
 
 
 def test_param_layout_matches_reference_state_dict():

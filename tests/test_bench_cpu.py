@@ -1,6 +1,6 @@
 """bench.py's reference arm (`--impl reference`) runs on the host cores only, so its contract is checkable without a GPU: one
 JSON line with the native arm's metric / unit / workload string, `impl`, `cpu_baseline` (kind, cores, sample) and the e2e
-object; under torchrun every rank but 0 exits 0 without work.  (The native arm needs a B200: `pytest -m gpu` + the driver.)"""
+object; under torchrun every rank but 0 exits 0 without work.  (The native arm needs an H100: `pytest -m gpu`.)"""
 import json
 import os
 import subprocess

@@ -46,9 +46,9 @@ def test_sample():
         c["dataset.template_obj"]
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference checkout only exists in the build container")
-def test_all_shipped_confs_parse():
-    files = glob.glob("/root/reference/AvatarGen/AppearanceGen/confs/**/*.conf", recursive=True)
+def test_all_shipped_confs_parse(tmp_path):
+    from util_neus import reference_tree
+    files = glob.glob(reference_tree(tmp_path) + "/confs/**/*.conf", recursive=True)
     assert len(files) == 180
     for f in files:
         c = conf.parse_file(f)
@@ -58,14 +58,14 @@ def test_all_shipped_confs_parse():
         assert c.get_float("train.learning_rate") > 0
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference checkout only exists in the build container")
-def test_every_shipped_conf_constructs_its_networks_and_is_a_supported_loop():
+def test_every_shipped_conf_constructs_its_networks_and_is_a_supported_loop(tmp_path):
     """All 180 shipped confs: the model subtrees are accepted as constructor kwargs (main.py:137-151) -- 3 distinct network
     configurations, incl. the extra_color-less one of base_models/astrongman.conf -- and the train.* switches name a loop the
     Runner implements (train_clip: use_silhouettes + extra_color; --mode train: astrongman.conf)."""
     import json
     import avatarclip_b200 as ab
-    files = sorted(glob.glob("/root/reference/AvatarGen/AppearanceGen/confs/**/*.conf", recursive=True))
+    from util_neus import reference_tree
+    files = sorted(glob.glob(reference_tree(tmp_path) + "/confs/**/*.conf", recursive=True))
     built, n_clip = {}, 0
     for f in files:
         c = conf.parse_file(f)

@@ -1,18 +1,18 @@
 """SMPL_Dataset (avatarclip_b200/dataset.py) loading the directories the reference SHIPS (data/zero_beta_{tpose,standpose}_render:
 108 PNGs + transforms_train.json each) against the reference's own constructor lines (models/dataset.py:204-250) executed in
-place.  Build container only (the data lives under /root/reference).  Stand-ins: `imageio.imread` (not installed) -> cv2 with
+place; the render directories and what the reference made of them are stored under tests/golden/.  Stand-ins: `imageio.imread` (not installed) -> cv2 with
 BGR(A) -> RGB(A) reordering; `torch.device('cuda')` -> cpu (a device move, no arithmetic); `pose_spherical` (render_poses, unused by
 the Runner) -> a stub.  Everything else -- image scaling, the W-axis flip of :222, masks, poses, focal, K, bounding box -- is the
 reference's text."""
 import os
 import textwrap
+import types
 
 import numpy as np
 import pytest
 import torch
 
-REF = "/root/reference/AvatarGen/AppearanceGen"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout only exists in the build container")
+REF = os.path.join(os.environ.get("AVC_REFERENCE", ""), "AvatarGen/AppearanceGen")
 
 
 class _Conf(dict):
@@ -40,17 +40,31 @@ def _reference_dataset(data_dir):
     return obj
 
 
+def _digest(t):
+    import hashlib
+    return hashlib.sha256(t.contiguous().numpy().tobytes()).hexdigest()
+
+
 @pytest.mark.parametrize("name", ["zero_beta_tpose_render", "zero_beta_standpose_render"])
-def test_shipped_render_directory_loads_like_the_reference(name):
+def test_shipped_render_directory_loads_like_the_reference(name, tmp_path):
+    """The render directories are stored under tests/golden/ (util_neus.reference_tree), and so is what the reference's
+    constructor made of them (images and masks as sha256 digests of their bytes)."""
     from avatarclip_b200.dataset import SMPL_Dataset
-    data_dir = os.path.join(REF, "data", name)
-    ref = _reference_dataset(data_dir)
+    from util_neus import reference_golden, reference_tree
+    data_dir = os.path.join(reference_tree(tmp_path), "data", name)
+
+    def reference():
+        d = _reference_dataset(os.path.join(REF, "data", name))
+        return dict(n_images=d.n_images, H=d.H, W=d.W, focal=d.focal, image_pixels=d.image_pixels, images=_digest(d.images),
+                    masks=_digest(d.masks), poses=d.poses, K=d.K, object_bbox_min=d.object_bbox_min,
+                    object_bbox_max=d.object_bbox_max, images_lis=[os.path.relpath(f, REF) for f in d.images_lis])
+    ref = types.SimpleNamespace(**reference_golden(f"dataset_{name}", reference))
     ours = SMPL_Dataset(_Conf(data_dir=data_dir), device="cpu")
     assert ours.n_images == ref.n_images == 108 and (ours.H, ours.W) == (ref.H, ref.W) == (256, 256)
     assert ours.focal == ref.focal and ours.image_pixels == ref.image_pixels
-    assert torch.equal(ours.images, ref.images) and torch.equal(ours.masks, ref.masks)
+    assert _digest(ours.images) == ref.images and _digest(ours.masks) == ref.masks
     assert torch.equal(ours.poses, ref.poses) and torch.equal(ours.K, ref.K)
     assert np.array_equal(ours.object_bbox_min, ref.object_bbox_min) and np.array_equal(ours.object_bbox_max, ref.object_bbox_max)
-    assert ours.images_lis == ref.images_lis
+    assert [os.path.relpath(f, os.path.dirname(os.path.dirname(data_dir))) for f in ours.images_lis] == ref.images_lis
     img = ours.image_at(58, 4)                                   # the validation camera of train_clip (main.py:557)
     assert img.shape == (64, 64, 3)

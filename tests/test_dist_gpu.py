@@ -1,4 +1,4 @@
-"""2-rank NCCL test of the PRODUCT path (needs >= 2 GPUs; skipped on a 1-GPU box): two ranks each run the fused step
+"""2-rank NCCL test of the PRODUCT path (needs >= 2 GPUs; skipped on a 1-GPU machine): two ranks each run the fused step
 of avatarclip_b200.trainer on the view avatarclip_b200.dist.view_index assigns them (tcgen05 engine), all-reduce the
 flat gradient over NCCL and apply the fused Adam with grad_scale 1/2; the result must equal ONE rank accumulating the
 two views' gradients and applying the same Adam (SURVEY.md 8e: N ranks x 1 view == 1 rank x N views)."""
@@ -54,7 +54,7 @@ def _worker(rank, world, port, out):
     torch.distributed.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_rank_nccl_product_step_equals_two_view_accumulation(tmp_path):
     s = socket.socket()
     s.bind(("127.0.0.1", 0))

@@ -7,7 +7,7 @@ import pytest
 
 from avatarclip_b200 import handoff
 
-REF_RENDER = "/root/reference/AvatarGen/ShapeGen/render.py"
+REF_RENDER = os.path.join(os.environ.get("AVC_REFERENCE", ""), "AvatarGen/ShapeGen/render.py")
 
 
 def test_ply_round_trip_and_header(tmp_path):
@@ -48,19 +48,21 @@ def test_hand_off_cameras():
         assert np.allclose(R[:, 2], eye / np.linalg.norm(eye))                                    # camera looks down -z at the origin
 
 
-@pytest.mark.skipif(not os.path.exists(REF_RENDER), reason="reference checkout only exists in the build container")
 def test_camera_matrix_equals_the_reference_lines():
-    """ShapeGen/render.py:16-30 (norm_np_arr + lookat) executed in place against handoff.lookat_inverse_view."""
+    """ShapeGen/render.py:16-30 (norm_np_arr + lookat) against handoff.lookat_inverse_view (the reference's matrices are
+    stored under tests/golden/)."""
     import textwrap
-    lines = open(REF_RENDER).read().split("\n")[15:30]
-    assert lines[0].startswith("def norm_np_arr") and "return viewMatrix" in lines[-1]
-    ns = {"np": np}
-    exec(textwrap.dedent("\n".join(lines)), ns)
-    for a in range(0, 360, 40):
-        for e in (-60, -20, 0, 40):
-            eye = handoff.get_points_from_angles(2.2, e, a)
-            ref, _, _, _ = ns["lookat"](eye, np.array([0, 0, 0]), np.array([0, 1, 0]))
-            assert np.array_equal(ref, handoff.lookat_inverse_view(eye, np.array([0, 0, 0]), np.array([0, 1, 0])))
+    from util_neus import reference_golden
+    eyes = [handoff.get_points_from_angles(2.2, e, a) for a in range(0, 360, 40) for e in (-60, -20, 0, 40)]
+
+    def reference():
+        lines = open(REF_RENDER).read().split("\n")[15:30]
+        assert lines[0].startswith("def norm_np_arr") and "return viewMatrix" in lines[-1]
+        ns = {"np": np}
+        exec(textwrap.dedent("\n".join(lines)), ns)
+        return [ns["lookat"](eye, np.array([0, 0, 0]), np.array([0, 1, 0]))[0] for eye in eyes]
+    for eye, ref in zip(eyes, reference_golden("camera_matrices", reference), strict=True):
+        assert np.array_equal(ref, handoff.lookat_inverse_view(eye, np.array([0, 0, 0]), np.array([0, 1, 0])))
 
 
 def test_read_obj_triangulates_and_strips_texture_indices(tmp_path):
@@ -72,11 +74,10 @@ def test_read_obj_triangulates_and_strips_texture_indices(tmp_path):
     assert f.tolist() == [[0, 1, 2], [0, 2, 3], [0, 1, 2]] and f.dtype == np.int32          # quad -> fan of two triangles
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/AvatarGen/AppearanceGen/data/zero_beta_smpl.obj"),
-                    reason="reference checkout only exists in the build container")
-def test_read_obj_on_the_shipped_template():
+def test_read_obj_on_the_shipped_template(tmp_path):
     """dataset.template_obj of the shipped confs (main.py:292,316): the SMPL topology, 6890 vertices / 13 776 triangles."""
     from avatarclip_b200.views import read_obj
-    v, f = read_obj("/root/reference/AvatarGen/AppearanceGen/data/zero_beta_smpl.obj")
+    from util_neus import reference_tree
+    v, f = read_obj(os.path.join(reference_tree(tmp_path), "data/zero_beta_smpl.obj"))
     assert v.shape == (6890, 3) and f.shape == (13776, 3) and f.min() == 0 and f.max() == 6889
     assert np.abs(v).max() < 1.5

@@ -75,7 +75,6 @@ def test_loss_stage_kernels_match_reference_lines(case):
     print(f"case {case} (bg {c['choice_i']}, add_no_texture {no_tex}, texture_cast_light {cast}): canvases {e_tex:.2e} / {e_sh:.2e}; scalars {rel}; cotangents {g_err}")
     U.log_parity("loss_stage_direct", {"case": case, "bg": c["choice_i"], "flags": list(c["flags"]), "canvas_abs": max(e_tex, e_sh),
                                        "scalars_rel": max(rel.values()), "cotangents_rel_to_max": max(g_err.values())})
-    # measured on a B200 (profiles/r2_parity.json, "loss_stage_direct"): canvases <= 2.6e-7, scalars <= 5.2e-7, cotangents <= 3.2e-6
     assert e_tex < 2e-6 and e_sh < 2e-6
     assert max(rel.values()) < 5e-6, rel
     assert max(g_err.values()) < 5e-5, g_err

@@ -297,24 +297,24 @@ def test_extract_geometry_sphere_is_watertight_and_outward(tmp_path):
     assert torch.equal(sdf.sdf_hidden_appearance(pts.cuda()).cpu(), out)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/AvatarGen/AppearanceGen"),
-                    reason="reference checkout only exists in the build container")
 def test_shipped_example_conf_constructs_a_runner_and_loads_the_shipped_checkpoint(tmp_path):
-    """confs/examples/ironman.conf as shipped (only the three relative paths made absolute, because the reference tree is
-    read-only and the test does not run from inside it): the Runner builds the networks from the conf subtrees, reads every
-    train.* key and loads `train.pretrain` = pretrained_models/zero_beta_stand_pose.pth like main.py:153-160,612-619."""
+    """confs/examples_small/example.conf as shipped (only the three relative paths made absolute, because the test does not
+    run from inside the reference tree): the Runner builds the networks from the conf subtrees, reads every train.* key and
+    loads `train.pretrain` = pretrained_models/zero_beta_stand_pose_small.pth like main.py:153-160,612-619.  The conf, data
+    and checkpoint are the shipped files, stored under tests/golden/ (util_neus.reference_tree)."""
     from avatarclip_b200.runner import Runner
-    ag = "/root/reference/AvatarGen/AppearanceGen"
-    text = open(os.path.join(ag, "confs/examples/ironman.conf")).read()
+    from util_neus import reference_tree
+    ag = reference_tree(tmp_path / "ref")
+    text = open(os.path.join(ag, "confs/examples_small/example.conf")).read()
     for old, new in (("./exp/", str(tmp_path / "exp") + "/"), ("./data/", ag + "/data/"), ("./pretrained_models/", ag + "/pretrained_models/")):
         assert old in text
         text = text.replace(old, new)
-    p = tmp_path / "ironman.conf"
+    p = tmp_path / "example.conf"
     p.write_text(text)
     r = Runner(str(p), mode="validate", case="smpl", device="cpu")
     assert (r.use_silhouettes, r.add_no_texture, r.texture_cast_light, r.use_face_prompt, r.use_back_prompt, r.extra_color) == (True,) * 6
-    assert r.max_ray_num == 112 * 112 and r.end_iter == 100000 and r.renderer.n_samples == 32 and r.renderer.n_importance == 32
-    ck = torch.load(os.path.join(ag, "pretrained_models/zero_beta_stand_pose.pth"), map_location="cpu", weights_only=False)
+    assert r.max_ray_num == 7000 and r.end_iter == 30000 and r.renderer.n_samples == 32 and r.renderer.n_importance == 32
+    ck = torch.load(os.path.join(ag, "pretrained_models/zero_beta_stand_pose_small.pth"), map_location="cpu", weights_only=False)
     for k, v in ck["sdf_network_fine"].items():
         assert torch.equal(r.sdf_network.state_dict()[k], v), k
     assert torch.equal(r.deviation_network.variance.detach(), ck["variance_network_fine"]["variance"])

@@ -2,7 +2,8 @@
 place on the CPU: same fake dataset (random pixel batches from torch's global generator), same differentiable fake renderer
 over the network parameters, `torch.optim.Adam`, identical seeds.  Pins the loop's host logic -- image permutation cycling,
 mask handling, the loss formula, optimiser stepping, WHEN the learning rate is updated, what is logged under which name -- not
-the renderer (GPU parity tests).  Build container only."""
+the renderer (GPU parity tests).  What the reference's lines produced is stored under tests/golden/
+(util_neus.reference_golden)."""
 import copy
 import os
 import textwrap
@@ -12,9 +13,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-REF_MAIN = "/root/reference/AvatarGen/AppearanceGen/main.py"
+from util_neus import reference_golden
+
+REF_MAIN = os.path.join(os.environ.get("AVC_REFERENCE", ""), "AvatarGen/AppearanceGen/main.py")
 HERE = os.path.dirname(os.path.abspath(__file__))
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_MAIN), reason="reference checkout only exists in the build container")
 
 
 class FakeDataset:
@@ -78,22 +80,27 @@ def test_mode_train_loop_equals_the_reference_loop(tmp_path, mask_weight, white,
     p.write_text(conf)
     r = Runner(str(p), mode="train", case="smpl", device="cpu")
     r.dataset = FakeDataset()
-    # the reference side: independent copies of the same networks, torch.optim.Adam over sdf + variance + colour (main.py:141-145)
-    nets = [copy.deepcopy(m) for m in (r.sdf_network, r.deviation_network, r.color_network)]
-    ref_params = [q for m in nets for q in m.parameters()]
-    ns = _reference_methods()
-    wr_ref = Writer()
-    ns["SummaryWriter"] = lambda log_dir=None: wr_ref
-    ref = types.SimpleNamespace(
-        base_exp_dir=str(tmp_path / "ref"), end_iter=12, iter_step=0, dataset=FakeDataset(), batch_size=40, use_white_bkgd=white,
-        mask_weight=mask_weight, igr_weight=r.igr_weight, report_freq=3, save_freq=10 ** 9, val_freq=10 ** 9, val_mesh_freq=10 ** 9,
-        warm_up_end=4.0, anneal_end=0.0, learning_rate=r.learning_rate, learning_rate_alpha=r.learning_rate_alpha,
-        renderer=types.SimpleNamespace(render=make_render(ref_params)), optimizer=torch.optim.Adam(ref_params, lr=r.learning_rate))
-    for name in ("get_image_perm", "get_cos_anneal_ratio", "update_learning_rate"):
-        setattr(ref, name, types.MethodType(ns[name], ref))
-    torch.manual_seed(7)
-    ns["train"](ref)
-    ref_out = capsys.readouterr().out
+
+    def reference():
+        # independent copies of the same networks, torch.optim.Adam over sdf + variance + colour (main.py:141-145)
+        nets = [copy.deepcopy(m) for m in (r.sdf_network, r.deviation_network, r.color_network)]
+        ref_params = [q for m in nets for q in m.parameters()]
+        ns = _reference_methods()
+        wr_ref = Writer()
+        ns["SummaryWriter"] = lambda log_dir=None: wr_ref
+        ref = types.SimpleNamespace(
+            base_exp_dir=str(tmp_path / "ref"), end_iter=12, iter_step=0, dataset=FakeDataset(), batch_size=40, use_white_bkgd=white,
+            mask_weight=mask_weight, igr_weight=r.igr_weight, report_freq=3, save_freq=10 ** 9, val_freq=10 ** 9, val_mesh_freq=10 ** 9,
+            warm_up_end=4.0, anneal_end=0.0, learning_rate=r.learning_rate, learning_rate_alpha=r.learning_rate_alpha,
+            renderer=types.SimpleNamespace(render=make_render(ref_params)), optimizer=torch.optim.Adam(ref_params, lr=r.learning_rate))
+        for name in ("get_image_perm", "get_cos_anneal_ratio", "update_learning_rate"):
+            setattr(ref, name, types.MethodType(ns[name], ref))
+        torch.manual_seed(7)
+        ns["train"](ref)
+        return dict(rec=wr_ref.rec, params=[q.detach() for q in ref_params], lr=ref.optimizer.param_groups[0]["lr"],
+                    out=capsys.readouterr().out, iter_step=ref.iter_step)
+    want = reference_golden(f"mode_train_{mask_weight}_{white}", reference)
+    wr_ref, ref_params, ref_out = types.SimpleNamespace(rec=want["rec"]), want["params"], want["out"]
     # our side
     wr = Writer()
     r._make_writer = lambda: wr
@@ -101,14 +108,14 @@ def test_mode_train_loop_equals_the_reference_loop(tmp_path, mask_weight, white,
     r.renderer.render = make_render(r._all_params())
     torch.manual_seed(7)
     logs = []
-    assert r.train(log=logs.append, validate=False) == 12 == ref.iter_step
+    assert r.train(log=logs.append, validate=False) == 12 == want["iter_step"]
     assert [n for n, _, _ in wr.rec] == [n for n, _, _ in wr_ref.rec]                # same scalar names in the same order
     assert [s for _, _, s in wr.rec] == [s for _, _, s in wr_ref.rec]
     worst = max(abs(a - b) / max(abs(b), 1e-12) for (_, a, _), (_, b, _) in zip(wr.rec, wr_ref.rec))
     assert worst < 1e-6, worst
     for a, b in zip(r._all_params(), ref_params):                                    # the same parameters after 12 Adam steps
         assert torch.allclose(a.detach(), b.detach(), rtol=1e-6, atol=1e-9)
-    assert r.optimizer.param_groups[0]["lr"] == ref.optimizer.param_groups[0]["lr"]
+    assert r.optimizer.param_groups[0]["lr"] == want["lr"]
     lr_ours = [str(m).split("lr=")[1] for m in logs if "lr=" in str(m)]
     lr_ref = [l.split("lr=")[1] for l in ref_out.splitlines() if "lr=" in l]
     assert lr_ours == lr_ref and len(lr_ours) == 4                                   # the lr in force at steps 3, 6, 9, 12
@@ -122,8 +129,6 @@ def test_train_clip_host_logic_equals_the_reference_lines(tmp_path, monkeypatch)
     import numpy as np
     from avatarclip_b200 import views
     from avatarclip_b200.runner import Runner
-    from oracle.pin_loss_stage import cut
-    from oracle.pin_sampling import reference_draws
     conf = open(os.path.join(HERE, "runner_conf_sample.conf")).read().replace("./exp/CASE_NAME/demo", str(tmp_path / "ours"))
     conf = conf.replace("warm_up_end = 500", "warm_up_end = 5").replace("end_iter = 100000", "end_iter = 80")
     p = tmp_path / "c.conf"
@@ -163,23 +168,35 @@ def test_train_clip_host_logic_equals_the_reference_lines(tmp_path, monkeypatch)
     r._make_writer = lambda: __import__("avatarclip_b200.runner", fromlist=["_NullWriter"])._NullWriter()
     assert r.train_clip(max_steps=n_steps, log=lambda m: None, validate=False) == n_steps
     # ---- the reference's lines
-    ref = reference_draws(r.seed, n_steps + 1, r.head_height, face=True, bg_aug=True, shading=True)   # ours looks one step ahead
-    prompt_lines = cut("main.py", 499, 507, "if self.use_face_prompt and iter_i % 4 == 0", "current_no_texture_text_encoding = self.encoded_text")
-    sched = {"np": np}
-    exec(cut("main.py", 571, 586, "def get_cos_anneal_ratio", "g['lr']"), sched)
-    for i, got in enumerate(rec):
-        s = types.SimpleNamespace(use_face_prompt=True, use_back_prompt=True, encoded_text=body, encoded_face_text=face,
-                                  encoded_back_text=back)
-        loc = dict(self=s, iter_i=i, is_front=ref[i]["is_front"])
-        exec(prompt_lines, loc)
-        assert got["text"] == float(loc["current_text_encoding"][0, 0]), i
-        assert float(loc["current_no_texture_text_encoding"][0, 0]) == got["text"]
-        sch = types.SimpleNamespace(iter_step=i, warm_up_end=5.0, end_iter=80, learning_rate_alpha=r.learning_rate_alpha,
-                                    learning_rate=r.learning_rate, anneal_end=0.0,
-                                    optimizer=types.SimpleNamespace(param_groups=[{"lr": None}]))
-        sched["update_learning_rate"](sch)
-        assert got["lr"] == sch.optimizer.param_groups[0]["lr"], i
-        assert got["cos_anneal"] == float(sched["get_cos_anneal_ratio"](sch))
-        assert np.array_equal(got["pose"], np.asarray(ref[i]["pose"])) and got["bg"] == ref[i]["choice_i"], i
-        assert np.array_equal(got["light"], np.asarray(ref[i]["light_dir"]).astype(np.float32)) and got["ambience"] == ref[i]["ambience"]
+
+    def reference():
+        from oracle.pin_loss_stage import cut
+        from oracle.pin_sampling import reference_draws
+        ref = reference_draws(r.seed, n_steps + 1, r.head_height, face=True, bg_aug=True, shading=True)   # ours looks one step ahead
+        prompt_lines = cut("main.py", 499, 507, "if self.use_face_prompt and iter_i % 4 == 0", "current_no_texture_text_encoding = self.encoded_text")
+        sched = {"np": np}
+        exec(cut("main.py", 571, 586, "def get_cos_anneal_ratio", "g['lr']"), sched)
+        out = []
+        for i in range(n_steps):
+            s = types.SimpleNamespace(use_face_prompt=True, use_back_prompt=True, encoded_text=body, encoded_face_text=face,
+                                      encoded_back_text=back)
+            loc = dict(self=s, iter_i=i, is_front=ref[i]["is_front"])
+            exec(prompt_lines, loc)
+            sch = types.SimpleNamespace(iter_step=i, warm_up_end=5.0, end_iter=80, learning_rate_alpha=r.learning_rate_alpha,
+                                        learning_rate=r.learning_rate, anneal_end=0.0,
+                                        optimizer=types.SimpleNamespace(param_groups=[{"lr": None}]))
+            sched["update_learning_rate"](sch)
+            out.append(dict(text=float(loc["current_text_encoding"][0, 0]), no_texture=float(loc["current_no_texture_text_encoding"][0, 0]),
+                            lr=sch.optimizer.param_groups[0]["lr"], cos_anneal=float(sched["get_cos_anneal_ratio"](sch)),
+                            pose=np.asarray(ref[i]["pose"]), bg=ref[i]["choice_i"], light=np.asarray(ref[i]["light_dir"]).astype(np.float32),
+                            ambience=ref[i]["ambience"]))
+        return out
+    want = reference_golden("train_clip_host_logic", reference)
+    assert len(rec) == len(want) == n_steps
+    for i, (got, w) in enumerate(zip(rec, want)):
+        assert got["text"] == w["text"] == w["no_texture"], i
+        assert got["lr"] == w["lr"], i
+        assert got["cos_anneal"] == w["cos_anneal"]
+        assert np.array_equal(got["pose"], w["pose"]) and got["bg"] == w["bg"], i
+        assert np.array_equal(got["light"], w["light"]) and got["ambience"] == w["ambience"]
     assert {g["text"] for g in rec} == {0.0, 1.0, 2.0}             # body, face and back prompts all occurred

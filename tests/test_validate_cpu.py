@@ -1,6 +1,7 @@
 """Runner.validate_image's host side (batching, normal-image rotation, scaling, file names, image layout) against the reference's
 own method text (main.py:741-820) executed in place, both driven by the SAME fake dataset and the SAME fake renderer (deterministic
-functions of the rays, CPU tensors) -- the render itself is covered by the GPU parity tests.  Build container only."""
+functions of the rays, CPU tensors) -- the render itself is covered by the GPU parity tests.  What the reference's method
+produced is stored under tests/golden/ (util_neus.reference_golden)."""
 import os
 import textwrap
 import types
@@ -9,9 +10,10 @@ import numpy as np
 import pytest
 import torch
 
-REF_MAIN = "/root/reference/AvatarGen/AppearanceGen/main.py"
+from util_neus import reference_golden
+
+REF_MAIN = os.path.join(os.environ.get("AVC_REFERENCE", ""), "AvatarGen/AppearanceGen/main.py")
 HERE = os.path.dirname(os.path.abspath(__file__))
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_MAIN), reason="reference checkout only exists in the build container")
 
 
 class FakeDataset:
@@ -77,14 +79,19 @@ def test_validate_image_files_equal_the_reference_methods(tmp_path, extra_color)
     r.renderer.render = FakeRenderer().render
     r.renderer.n_samples, r.renderer.n_importance = 3, 2
     img, extra, normal = r.validate_image(idx=3, resolution_level=2)
-    ref_self = types.SimpleNamespace(dataset=FakeDataset(), iter_step=1234, batch_size=100, validate_resolution_level=1,
-                                     use_white_bkgd=False, extra_color=extra_color, renderer=FakeRenderer(),
-                                     base_exp_dir=str(tmp_path / "ref"), get_cos_anneal_ratio=lambda: 1.0)
-    _reference_validate_image()(ref_self, idx=3, resolution_level=2)
     name = "00001234_0_3.png"
-    for d in ("validations_fine", "normals") + (("validations_extra_fine",) if extra_color else ()):
+    dirs = ("validations_fine", "normals") + (("validations_extra_fine",) if extra_color else ())
+
+    def reference():
+        ref_self = types.SimpleNamespace(dataset=FakeDataset(), iter_step=1234, batch_size=100, validate_resolution_level=1,
+                                         use_white_bkgd=False, extra_color=extra_color, renderer=FakeRenderer(),
+                                         base_exp_dir=str(tmp_path / "ref"), get_cos_anneal_ratio=lambda: 1.0)
+        _reference_validate_image()(ref_self, idx=3, resolution_level=2)
+        return {d: cv.imread(os.path.join(str(tmp_path / "ref"), d, name), cv.IMREAD_UNCHANGED) for d in dirs}
+    want = reference_golden(f"validate_image_{extra_color}", reference)
+    for d in dirs:
         a = cv.imread(os.path.join(str(tmp_path / "ours"), d, name), cv.IMREAD_UNCHANGED)
-        b = cv.imread(os.path.join(str(tmp_path / "ref"), d, name), cv.IMREAD_UNCHANGED)
+        b = want[d]
         assert a is not None and b is not None and a.shape == b.shape and np.array_equal(a, b), d
     assert img.shape == (12, 12, 3) and normal.shape == (12, 12, 3) and (extra is None) == (not extra_color)
     if not extra_color:                       # the reference creates the directory but writes nothing into it
@@ -138,19 +145,24 @@ def test_validate_mesh_colours_equal_the_reference_methods(tmp_path, extra_color
     mr = MeshRenderer()
     r.renderer.render, r.renderer.extract_geometry = mr.render, mr.extract_geometry
     path = r.validate_mesh(resolution=64)
-    captured = {}
-    ds = FakeDataset()
-    ds.object_bbox_min, ds.object_bbox_max = np.array([-1.01] * 3), np.array([1.01] * 3)
-    ref_self = types.SimpleNamespace(dataset=ds, iter_step=77, batch_size=100, use_white_bkgd=False, extra_color=extra_color,
-                                     renderer=MeshRenderer(), base_exp_dir=str(tmp_path / "ref"), get_cos_anneal_ratio=lambda: 1.0)
-    saved_cuda = torch.Tensor.cuda
-    torch.Tensor.cuda = lambda self_, *a, **k: self_          # `.cuda()` (main.py:859,872): a device move, identity on this box
-    try:
-        _reference_validate_mesh(captured)(ref_self, resolution=64)
-    finally:
-        torch.Tensor.cuda = saved_cuda
+
+    def reference():
+        captured = {}
+        ds = FakeDataset()
+        ds.object_bbox_min, ds.object_bbox_max = np.array([-1.01] * 3), np.array([1.01] * 3)
+        ref_self = types.SimpleNamespace(dataset=ds, iter_step=77, batch_size=100, use_white_bkgd=False, extra_color=extra_color,
+                                         renderer=MeshRenderer(), base_exp_dir=str(tmp_path / "ref"), get_cos_anneal_ratio=lambda: 1.0)
+        saved_cuda = torch.Tensor.cuda
+        torch.Tensor.cuda = lambda self_, *a, **k: self_      # `.cuda()` (main.py:859,872): a device move, identity on the CPU
+        try:
+            _reference_validate_mesh(captured)(ref_self, resolution=64)
+        finally:
+            torch.Tensor.cuda = saved_cuda
+        captured["path"] = os.path.basename(captured["path"])
+        return captured
+    captured = reference_golden(f"validate_mesh_{extra_color}", reference)
     v, f, c = read_ply(path)
-    assert os.path.basename(path) == os.path.basename(captured["path"]) == "00000077.ply" and captured["file_type"] == "ply"
+    assert os.path.basename(path) == captured["path"] == "00000077.ply" and captured["file_type"] == "ply"
     assert np.array_equal(f, captured["triangles"].astype(np.int32)) and np.allclose(v, captured["vertices"].astype(np.float32))
     assert c.shape == captured["colors"].shape == (257, 3)
     assert np.array_equal(c, captured["colors"])                 # the same view wins for every vertex, the same 8-bit colour
@@ -162,18 +174,6 @@ def test_render_geometry_cast_light_equals_the_reference_method(tmp_path):
     import cv2 as cv
     from torchvision import transforms
     from avatarclip_b200.runner import Runner
-    lines = open(REF_MAIN).read().split("\n")
-    body = lines[633:739]
-    assert body[0].strip().startswith("def render_geometry_cast_light(self)") and body[-1].strip() == ")"
-    uns = dict(np=np, torch=torch)
-    utils = open(os.path.join(os.path.dirname(REF_MAIN), "models", "utils.py")).read().split("\n")
-    exec(textwrap.dedent("\n".join(utils[5:27])), uns)            # norm_np_arr, lookat (models/utils.py:6-27)
-    exec(textwrap.dedent("\n".join(utils[58:64])), uns)          # sphere_coord (:59-64)
-    captured = {}
-    ns = dict(np=np, torch=torch, os=os, transforms=transforms, lookat=uns["lookat"], sphere_coord=uns["sphere_coord"],
-              imageio=types.SimpleNamespace(imwrite=lambda path, arr: captured.update(path=path, img=np.asarray(arr))),
-              to8b=lambda x: (255 * np.clip(x, 0, 1)).astype(np.uint8))
-    exec(textwrap.dedent("\n".join(body)), ns)
 
     class DS(FakeDataset):
         def gen_rays_pose(self, pose, resolution_level=1):
@@ -195,18 +195,34 @@ def test_render_geometry_cast_light_equals_the_reference_method(tmp_path):
     np.random.seed(21)
     path = r.render_geometry_cast_light()
     next_ours = np.random.uniform()
-    ref_self = types.SimpleNamespace(dataset=DS(), batch_size=500, head_height=r.head_height, renderer=FakeRenderer(),
-                                     base_exp_dir=str(tmp_path / "ref"), get_cos_anneal_ratio=lambda: 1.0)
-    os.makedirs(ref_self.base_exp_dir, exist_ok=True)
-    saved_cuda = torch.Tensor.cuda
-    torch.Tensor.cuda = lambda self_, *a, **k: self_
-    np.random.seed(21)
-    try:
-        ns["render_geometry_cast_light"](ref_self)
-        next_ref = np.random.uniform()
-    finally:
-        torch.Tensor.cuda = saved_cuda
+
+    def reference():
+        lines = open(REF_MAIN).read().split("\n")
+        body = lines[633:739]
+        assert body[0].strip().startswith("def render_geometry_cast_light(self)") and body[-1].strip() == ")"
+        uns = dict(np=np, torch=torch)
+        utils = open(os.path.join(os.path.dirname(REF_MAIN), "models", "utils.py")).read().split("\n")
+        exec(textwrap.dedent("\n".join(utils[5:27])), uns)            # norm_np_arr, lookat (models/utils.py:6-27)
+        exec(textwrap.dedent("\n".join(utils[58:64])), uns)          # sphere_coord (:59-64)
+        captured = {}
+        ns = dict(np=np, torch=torch, os=os, transforms=transforms, lookat=uns["lookat"], sphere_coord=uns["sphere_coord"],
+                  imageio=types.SimpleNamespace(imwrite=lambda path, arr: captured.update(path=path, img=np.asarray(arr))),
+                  to8b=lambda x: (255 * np.clip(x, 0, 1)).astype(np.uint8))
+        exec(textwrap.dedent("\n".join(body)), ns)
+        ref_self = types.SimpleNamespace(dataset=DS(), batch_size=500, head_height=r.head_height, renderer=FakeRenderer(),
+                                         base_exp_dir=str(tmp_path / "ref"), get_cos_anneal_ratio=lambda: 1.0)
+        os.makedirs(ref_self.base_exp_dir, exist_ok=True)
+        saved_cuda = torch.Tensor.cuda
+        torch.Tensor.cuda = lambda self_, *a, **k: self_
+        np.random.seed(21)
+        try:
+            ns["render_geometry_cast_light"](ref_self)
+            next_ref = np.random.uniform()
+        finally:
+            torch.Tensor.cuda = saved_cuda
+        return dict(path=os.path.basename(captured["path"]), img=captured["img"], next=next_ref)
+    want = reference_golden("render_geometry_cast_light", reference)
     ours = cv.cvtColor(cv.imread(path, cv.IMREAD_UNCHANGED), cv.COLOR_BGR2RGB)
-    assert os.path.basename(path) == os.path.basename(captured["path"]) == "cast_light_texture_head_black.png"
-    assert ours.shape == captured["img"].shape == (48, 48, 3) and np.array_equal(ours, captured["img"])
-    assert next_ours == next_ref              # both sides consumed the same draws of numpy's global stream (main.py:671-674)
+    assert os.path.basename(path) == want["path"] == "cast_light_texture_head_black.png"
+    assert ours.shape == want["img"].shape == (48, 48, 3) and np.array_equal(ours, want["img"])
+    assert next_ours == want["next"]             # both sides consumed the same draws of numpy's global stream (main.py:671-674)

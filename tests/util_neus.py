@@ -12,19 +12,39 @@ from oracle import neus
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
+
+def reference_tree(dst) -> str:
+    """The reference's shipped data the tests read (confs, the SMPL template, the two render directories, the small
+    pretrained checkpoint), unpacked from tests/golden/ref_tree_*.tar* into dst, laid out like AvatarGen/AppearanceGen."""
+    import glob
+    import tarfile
+    for t in sorted(glob.glob(os.path.join(GOLDEN, "ref_tree_*.tar*"))):
+        with tarfile.open(t) as tf:
+            tf.extractall(str(dst), filter="data")
+    return str(dst)
+
+
+def reference_golden(name: str, compute):
+    """What the reference computed for a test, stored as tests/golden/ref_<name>.pt.  AVC_REGEN_GOLDEN=1 reruns `compute`
+    (it executes the reference's own code, so it needs the reference checkout at $AVC_REFERENCE) and rewrites the file."""
+    path = os.path.join(GOLDEN, f"ref_{name}.pt")
+    if os.environ.get("AVC_REGEN_GOLDEN") == "1":
+        torch.save(compute(), path)
+    return torch.load(path, weights_only=False)
+
 COT_KEYS = ["color_fine", "extra_color_fine", "s_val", "cdf_fine", "weight_sum", "weight_max", "gradients",
             "weights", "gradient_error"]
 
 
 def log_parity(name: str, rec: dict):
-    """Append one measured-parity record to gpurun_out/r2_parity.jsonl (merged into profiles/ by tools/collect_parity.py):
-    the tests assert bars, this file keeps the numbers actually measured on the GPU box."""
+    """Append one measured-parity record to $AVC_PARITY_LOG (a JSON-lines file) when that variable is set: the tests
+    assert bars, the log keeps the numbers actually measured."""
     import json
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    d = os.path.join(root, "gpurun_out")
+    path = os.environ.get("AVC_PARITY_LOG")
+    if not path:
+        return
     try:
-        os.makedirs(d, exist_ok=True)
-        with open(os.path.join(d, "r2_parity.jsonl"), "a") as f:
+        with open(path, "a") as f:
             f.write(json.dumps(dict(test=name, **rec)) + "\n")
     except OSError:
         pass

@@ -1,4 +1,4 @@
-"""Times SDFNetwork.sdf (value chain without a stash) on the tcgen05 engine, fused kernel vs layer-by-layer launches,
+"""Times SDFNetwork.sdf (value chain without a stash) on the wgmma engine, fused kernel vs layer-by-layer launches,
 for the point counts of the placement passes and of a mesh grid.  Run on the GPU box: python tools/chain_probe.py"""
 import json
 import os

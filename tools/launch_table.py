@@ -1,5 +1,5 @@
 """Turn an ncu launch list (`--metrics gpu__time_duration.sum,launch__grid_size,dram__bytes_read.sum,dram__bytes_write.sum
---csv`) of `bench.py --graph 0` into (1) a per-kernel summary of ONE step and (2) the table of that step's tcgen05 NT
+--csv`) of `bench.py --graph 0` into (1) a per-kernel summary of ONE step and (2) the table of that step's wgmma NT
 launches (epilogue, grid, duration, DRAM bytes).  Usage: python tools/launch_table.py launches.csv [launches_per_step]"""
 import collections
 import csv
@@ -53,7 +53,7 @@ def main():
             mb = (d.get("dram__bytes_read.sum", 0.0) + d.get("dram__bytes_write.sum", 0.0)) / 1e6
             print(f"  k_sdf_chain    grid {int(d.get('launch__grid_size', 0)):4d} {d['gpu__time_duration.sum']:7.1f} us {mb:7.1f} MB")
     print()
-    print("tcgen05 NT launches of the step, in launch order: epilogue, grid, us, DRAM MB (read+write), GB/s")
+    print("wgmma NT launches of the step, in launch order: epilogue, grid, us, DRAM MB (read+write), GB/s")
     for d in W:
         if "gemm_tc_nt" in d["name"]:
             mb = (d.get("dram__bytes_read.sum", 0.0) + d.get("dram__bytes_write.sum", 0.0)) / 1e6

@@ -1,8 +1,8 @@
-"""Stall probe of the tcgen05 NT tiles.
+"""Stall probe of the wgmma NT tiles.
 
     python tools/nt_probe.py --build      # here (nvcc): avatarclip_b200/libavc_b200_probe.so = product objects, with
                                           # avc_neus.cu recompiled with -DAVC_NT_PROBE=1
-    python tools/nt_probe.py --run OUT    # on the GPU box: a few steps of the bench workload through the probe build,
+    python tools/nt_probe.py --run OUT    # on the GPU: a few steps of the bench workload through the probe build,
                                           # per epilogue functor the share of its loop each warp role spent waiting
 
 The probe adds a clock64 pair around every mbarrier wait of the three warp roles (TMA producer, MMA issuer, one epilogue
@@ -30,7 +30,7 @@ def build():
     subprocess.check_call([nvcc] + g.NVCC_FLAGS + ["-DAVC_NT_PROBE=1", "-c", "-o", probe_obj,
                                                   os.path.join(ROOT, "avatarclip_b200", "csrc", "avc_neus.cu")], cwd=ROOT)
     objs = [os.path.join(obj_dir, f) for f in sorted(os.listdir(obj_dir)) if f.endswith(".o") and f != "avc_neus.o"]
-    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", PROBE_LIB, probe_obj] + objs,
+    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", PROBE_LIB, probe_obj] + objs,
                           cwd=ROOT)
     print("built", PROBE_LIB)
 
@@ -67,11 +67,10 @@ def run(out_path):
         ctas = v[7]
         rep[NAMES.get(i, str(i))] = {
             "ctas_per_step": ctas / steps,
-            "loop_kcycles_per_cta": {"tma": v[1] / ctas / 1e3, "mma": v[4] / ctas / 1e3, "epilogue_warp": v[6] / ctas / 1e3},
+            # producer warp; consumer warpgroup 0 (its MMAs and epilogues)
+            "loop_kcycles_per_cta": {"tma": v[1] / ctas / 1e3, "consumer": v[4] / ctas / 1e3},
             "tma_waits_free_stage": v[0] / max(v[1], 1),
-            "mma_waits_operands": v[3] / max(v[4], 1),
-            "mma_waits_drained_accumulator": v[2] / max(v[4], 1),
-            "epilogue_waits_accumulator": v[5] / max(v[6], 1),
+            "consumer_waits_operands": v[3] / max(v[4], 1),
         }
     with open(out_path, "w") as f:
         json.dump(rep, f, indent=1)

@@ -1,5 +1,5 @@
-// gridbar_probe.cu -- latency of grid-wide barrier variants on a cooperative launch (148 x 512 threads).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probes/gridbar_probe tools/probes/gridbar_probe.cu
+// gridbar_probe.cu -- latency of grid-wide barrier variants on a cooperative launch (one 512-thread CTA per SM).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probes/gridbar_probe tools/probes/gridbar_probe.cu
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
-"""Duration of the tcgen05 weight-gradient (TN) tile kernel against the reduction length P (N1 = N2 = 256, split operands):
+"""Duration of the wgmma weight-gradient (TN) tile kernel against the reduction length P (N1 = N2 = 256, split operands):
 the slope is the streaming cost, the intercept the fixed cost of a launch (set-up, first loads, atomics flush, tail).
-    python tools/tn_scaling_probe.py OUT.json        # on a B200"""
+    python tools/tn_scaling_probe.py OUT.json        # on an H100"""
 import ctypes as C
 import json
 import os
