@@ -56,7 +56,7 @@ __device__ __forceinline__ float rcp_ftz(float x) { float y; asm("rcp.approx.ftz
 // the discarded arm produces for large arguments).  FAST: SFU ex2 / lg2 / rcp;  else libm accuracy.
 template <bool FAST>
 __device__ __forceinline__ void softplus100_both(float z, float* h, float* d1) {
-  if (FAST) {       // same operations as softplus100_both4 (bit-identical results whichever form an epilogue path uses)
+  if (FAST) {
     const float e = ex2_ftz(z * (kBeta * 1.4426950408889634f));
     const float t = 1.0f + e;
     const bool big = z * kBeta > kThresh;
@@ -65,30 +65,6 @@ __device__ __forceinline__ void softplus100_both(float z, float* h, float* d1) {
   } else {
     *h = softplus100(z);
     *d1 = softplus100_d1(z);
-  }
-}
-
-// softplus and softplus' of four independent arguments.  FAST: staged so that the four SFU chains (ex2 -> lg2 / rcp)
-// are issued side by side and without branches -- the ternary form of softplus100_both<true> compiles to a branch
-// around each element's MUFUs, which serialises the four chains of an epilogue pass (ncu: stall_wait dominated).
-template <bool FAST>
-__device__ __forceinline__ void softplus100_both4(const float (&z)[4], float (&h)[4], float (&d1)[4]) {
-  if (FAST) {
-    constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
-    float e[4], lg[4], rc[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) e[i] = ex2_ftz(z[i] * (kBeta * kLog2e));
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { const float t = 1.0f + e[i]; lg[i] = lg2_ftz(t); rc[i] = rcp_ftz(t); }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const bool big = z[i] * kBeta > kThresh;        // the discarded arm may hold inf / NaN: selects, not arithmetic
-      h[i] = big ? z[i] : lg[i] * (kLn2 / kBeta);
-      d1[i] = big ? 1.0f : e[i] * rc[i];
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { h[i] = softplus100(z[i]); d1[i] = softplus100_d1(z[i]); }
   }
 }
 

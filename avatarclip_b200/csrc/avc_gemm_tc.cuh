@@ -9,12 +9,14 @@
 //   gemm_tc_nt : C[m,n] = sum_k A[m,k] B[n,k]     A:[M,lda] B:[N,ldb], both K-contiguous (K-major operands)
 //   gemm_tc_tn : C[i,j] += sum_p A[p,i] B[p,j]    reduction over rows (weight gradients; MN-major operands)
 //
-// Kernel shape (288 threads): warps 0-7 are two consumer warpgroups, warpgroup g owning rows [64 g, 64 g + 64) of the
-// 128-row tile: it issues wgmma.mma_async m64nBNk16 on shared-memory descriptors, keeps its fp32 accumulator in
-// registers and runs the epilogue straight from that fragment; warp 8 is the TMA producer.  K step 64 (one 128-byte
-// swizzle atom), shared-memory ring with full (TMA transaction count) / empty (one arrival per consumer warpgroup)
-// mbarriers.  NT: persistent, one column tile per CTA, B panel resident in shared memory when K <= 256.  TN: one tile
-// per CTA, split over the reduction dimension.
+// Consumer warpgroups issue wgmma.mma_async m64nBNk16 on shared-memory descriptors, keep their fp32 accumulator in
+// registers and run the epilogue straight from that fragment; a TMA producer fills a shared-memory ring (K step 64, one
+// 128-byte swizzle atom) guarded by full (TMA transaction count) / empty mbarriers.
+//   NT (384 threads): persistent ping-pong.  A producer warpgroup and two consumer warpgroups that take turns at the
+//      tensor pipe, one 64-row tile each, so that one's epilogue runs under the other's MMAs; one column tile per CTA,
+//      B panel resident in shared memory when K <= 256.
+//   TN (288 threads): warps 0-7 are two consumer warpgroups, warpgroup g owning rows [64 g, 64 g + 64) of the 128-row
+//      tile, warp 8 the producer; one tile per CTA, split over the reduction dimension.
 #pragma once
 #include <type_traits>
 #include <cuda.h>
@@ -52,27 +54,21 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (spins > (1u << 26)) __trap();      // ~seconds: far beyond any legitimate wait, short of the driver's watchdog
   }
 }
-// Optional stall probe of the NT kernel (compile with -DAVC_NT_PROBE=1, see tools/nt_probe.py): cycles the TMA warp waits
-// for a free stage, consumer warpgroup 0 waits for operands, and each role's total loop time, summed over the CTAs of
-// every launch, per epilogue functor (Epi::kProbeId).
+// Optional stall probe of the NT kernel (compile with -DAVC_NT_PROBE=1, see tools/nt_probe.py).  Cycles summed over the
+// CTAs of every launch, per epilogue functor (Epi::kProbeId), in the slots
+//   0 producer waits for a free stage   1 producer loop          2 consumers wait for operands   3 consumers wait for turn
+//   4 consumers' MMAs (turn to done)    5 consumers' epilogues   6 consumers' loops              7 CTAs
+// (the consumer slots add up both consumer warpgroups).  AVC_PROBE(...) code only exists in the probe build.
 #ifdef AVC_NT_PROBE
 static __device__ unsigned long long g_nt_probe[16][8];
+#define AVC_PROBE(...) __VA_ARGS__
 #define AVC_PROBE_WAIT(acc, bar, par) do { long long t__ = clock64(); mbar_wait(bar, par); (acc) += clock64() - t__; } while (0)
-#define AVC_PROBE_DECL(name) long long name = 0
-#define AVC_PROBE_START(name) const long long name = clock64()
-#define AVC_PROBE_NOW() clock64()
 #define AVC_PROBE_ADD(id, slot, v) atomicAdd(&g_nt_probe[id][slot], (unsigned long long)(v))
 #else
+#define AVC_PROBE(...)
 #define AVC_PROBE_WAIT(acc, bar, par) mbar_wait(bar, par)
-#define AVC_PROBE_DECL(name)
-#define AVC_PROBE_START(name)
-#define AVC_PROBE_NOW() 0
 #define AVC_PROBE_ADD(id, slot, v)
 #endif
-template <typename E, typename = void>
-struct EpiNoAPf { static constexpr bool value = false; };
-template <typename E>
-struct EpiNoAPf<E, std::void_t<decltype(E::kNoATilePrefetch)>> { static constexpr bool value = E::kNoATilePrefetch; };
 template <typename E, typename = void>
 struct EpiProbeId { static constexpr int value = 0; };
 template <typename E>
@@ -100,20 +96,18 @@ static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 blo
 
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// bar.sync on a named barrier: the 128 threads of one consumer warpgroup (ids 1 + g; 0 is __syncthreads)
+// bar.sync / bar.arrive on a named barrier (id >= 1; 0 is __syncthreads) over `count` threads
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"((uint64_t)map), "r"(bar), "r"(x), "r"(y) : "memory");
-}
-// TMA prefetch of one box into L2 (no shared memory, no barrier): decouples the HBM latency of the A stream from the
-// depth of the shared-memory ring
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int x, int y) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"((uint64_t)map), "r"(x), "r"(y) : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
@@ -180,18 +174,23 @@ constexpr int kTcThreads = kConsumerThreads + 32;          // + the TMA producer
 constexpr int kProducerWarp = kConsumerThreads / 32;
 constexpr int kSmemMax = 232448;                           // 227 KB of shared memory per CTA
 
+// NT kernel: a producer warpgroup and two consumer warpgroups; its work unit is one warpgroup's m64 row block.
+constexpr int kNtBM = 64;
+constexpr int kNtThreads = 384;
+constexpr int kNtTurnBar = 1;     // named barrier kNtTurnBar + c: consumer warpgroup c may issue its next tile's MMAs
+
 // RESB: the CTA keeps its whole B panel (BN rows x up to kResK k-blocks, hi and lo) resident in shared memory and only
-// streams A: re-fetched for every 128-row tile, the B panel would double the L2 -> SM operand traffic of a tile.
+// streams A: re-fetched for every row tile, the B panel would multiply the L2 -> SM operand traffic of a tile.
 constexpr int kResK = 4;          // k-blocks (of 64) a resident panel holds: K <= 256
 template <int BN, int NPROD, bool RESB = false>
 struct TcCfg {
-  static constexpr int A_BYTES = kBM * kBK * 2;                    // one (hi or lo) A slab: 16 KB
+  static constexpr int A_BYTES = kNtBM * kBK * 2;                  // one (hi or lo) A slab: 8 KB
   static constexpr int B_BYTES = BN * kBK * 2;
   static constexpr int NOP = (NPROD == 3) ? 2 : 1;                 // slabs per operand (hi, lo)
   static constexpr int BRES_BYTES = RESB ? kResK * NOP * B_BYTES : 0;
   static constexpr int STAGE_BYTES = RESB ? NOP * A_BYTES : NOP * (A_BYTES + B_BYTES);
   static constexpr int kBudget = kSmemMax - 1024 /*align*/ - 256 /*barriers*/ - BRES_BYTES;
-  static constexpr int STAGES = kBudget / STAGE_BYTES >= 4 ? 4 : kBudget / STAGE_BYTES;
+  static constexpr int STAGES = kBudget / STAGE_BYTES >= 8 ? 8 : kBudget / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BRES_BYTES + 1024 + 256;
   static_assert(STAGES >= 2, "tile too large for shared memory");
   static_assert(SMEM_BYTES <= kSmemMax, "exceeds the 227 KB of shared memory per CTA");
@@ -213,14 +212,14 @@ struct EpiTraits<E, std::void_t<typename E::Aux>> {
   static __device__ __forceinline__ void apply(const E& e, int r, int c, float4 a, const Aux& x) { e(r, c, a, x); }
 };
 // The epilogue's own global operands (stashes written passes ago: always DRAM misses) are loaded right before use.
-// Functors with `l2_prefetch(m0, n0, bn, M, et, nth)` get the chance to pull the NEXT row tile's operand lines into L2 a
-// whole tile ahead (thread et of nth epilogue threads).
-template <int ES>   // element size in bytes; [rows][ld] row-major array, tile rows [m0, m0 + 128) x columns [n0, n0 + bn)
+// Functors with `l2_prefetch(m0, n0, bn, M, et, nth)` get the chance to pull the operand lines of the consumer
+// warpgroup's NEXT row tile into L2 a whole tile ahead (thread et of nth epilogue threads).
+template <int ES>   // element size in bytes; [rows][ld] row-major array, tile rows [m0, m0 + 64) x columns [n0, n0 + bn)
 __device__ __forceinline__ void l2_prefetch_tile(const void* base, int ld, int ncols, int m0, int n0, int bn, int M,
                                                  int et, int nth) {
   constexpr int kPerLine = 128 / ES;
   const int lpr = (bn + kPerLine - 1) / kPerLine;
-  for (int i = et; i < kBM * lpr; i += nth) {
+  for (int i = et; i < kNtBM * lpr; i += nth) {
     const int row = m0 + i / lpr, col = n0 + (i % lpr) * kPerLine;
     if (row < M && col < ncols)
       asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(base) + ((size_t)row * ld + col) * ES));
@@ -242,41 +241,55 @@ struct EpiL2<E, std::void_t<decltype(&E::l2_prefetch)>> {
 // neighbouring lane (lane ^ 1) turns them into one group of 4 consecutive columns per 8-column group -- even lanes take
 // row r, odd lanes row r + 8 -- so the functors see (row, col..col+3) with col % 4 == 0, as from the fp32 engine.  A warp
 // covers 16 rows x 32 bytes per group: every global access of a functor is whole 32-byte sectors.
-template <int BN, typename Epi>
+// The functor operands (prefetch) are loaded in batches of kB groups, one batch ahead of the arithmetic: the first batch
+// before `mma_done()` (which waits for the accumulator), every later one before the previous batch's arithmetic and
+// stores, so that a memory round trip is always in flight under other work.
+template <int BN, typename Epi, typename MmaDone>
 __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[BN / 2], int row, int col0, int M, int N,
-                                            int lane) {
+                                            int lane, MmaDone&& mma_done) {
   using Tr = EpiTraits<Epi>;
   const bool odd = lane & 1;
-  constexpr int kB = 4;      // groups whose functor operands are loaded together, ahead of the arithmetic
-#pragma unroll
-  for (int j0 = 0; j0 < BN / 8; j0 += kB) {
-    float4 v[kB];
-    typename Tr::Aux aux[kB];
+  // groups per batch: two batches of operands are live beside the accumulator; with 32-byte operands (EpiChainBwd,
+  // EpiDgrad) batches of 4 need more registers than ptxas grants a 384-thread kernel and spill
+  constexpr int kB = sizeof(typename Tr::Aux) > 16 ? 2 : 4, kNB = BN / 8 / kB;
+  typename Tr::Aux aux[2][kB];
+  auto load = [&](int b) {
 #pragma unroll
     for (int u = 0; u < kB; ++u) {
-      const int j = j0 + u;
+      const int col = col0 + 8 * (kB * b + u);
+      if (row < M && col < N) aux[b & 1][u] = Tr::prefetch(epi, row, col);
+    }
+  };
+  load(0);
+  mma_done();
+#pragma unroll
+  for (int b = 0; b < kNB; ++b) {
+    if (b + 1 < kNB) load(b + 1);
+#pragma unroll
+    for (int u = 0; u < kB; ++u) {
+      const int j = kB * b + u;
       const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
       const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-      v[u] = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
+      const float4 v = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
       const int col = col0 + 8 * j;
-      if (row < M && col < N) aux[u] = Tr::prefetch(epi, row, col);
-    }
-#pragma unroll
-    for (int u = 0; u < kB; ++u) {
-      const int col = col0 + 8 * (j0 + u);
-      if (row < M && col < N) Tr::apply(epi, row, col, v[u], aux[u]);
+      if (row < M && col < N) Tr::apply(epi, row, col, v, aux[b & 1][u]);
     }
   }
 }
 
-// Persistent: gridDim.x CTAs (<= one per SM, a multiple of the number of column tiles); a CTA keeps one column tile
-// and walks the row tiles m_first, +m_stride, ...  While the consumers run the epilogue of tile i the producer already
-// fills the ring with the first k-blocks of tile i + 1.
+// Persistent ping-pong: gridDim.x CTAs (<= one per SM, a multiple of the number of column tiles); a CTA keeps one column
+// tile and walks the 64-row tiles m_first, +m_stride, ...; its j-th tile belongs to consumer warpgroup j % 2.
+//   warpgroup 0      producer: one thread issues the TMA (resident B panel, then the A ring); 40 registers
+//   warpgroups 1, 2  consumers: MMAs of a tile into a register accumulator, then its epilogue; 232 registers
+// The consumers take strict turns at issuing MMAs (named barriers kNtTurnBar + c).  A consumer passes the turn as soon as
+// its last k-block is issued, then waits for its MMAs and runs the epilogue while the other one issues: the tensor pipe
+// works under the epilogues.  Turns make the ring's consumption follow the tile order, so the k-block counter j * nk + kb
+// gives every role the stage and its parity, and each stage is released by the one warpgroup that read it.
 template <int BN, int NPROD, bool RESB, typename Epi>
-__global__ void __launch_bounds__(kTcThreads, 1)
+__global__ void __launch_bounds__(kNtThreads, 1)
 gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapBhi, const __grid_constant__ CUtensorMap mapBlo,
-                  int M, int N, int K, Epi epi, int l2pf, int b_const) {
+                  int M, int N, int K, Epi epi, int b_const) {
   using Cfg = TcCfg<BN, NPROD, RESB>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B wants 1024-B tiles
@@ -288,25 +301,27 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_n = (N + BN - 1) / BN;
-  const int tiles_m = (M + kBM - 1) / kBM;
+  const int tiles_m = (M + kNtBM - 1) / kNtBM;
   const int nk = (K + kBK - 1) / kBK;
   // A CTA owns ONE column tile (n0 fixed: its B panel can stay resident) and walks the row tiles m_first, +m_stride, ..;
   // neighbouring CTAs work on the same row tile at the same time (A is read from HBM once, from L2 after that).
   // The host makes gridDim.x a multiple of tiles_n.
   const int n0 = (int)(blockIdx.x % tiles_n) * BN;
   const int m_first = (int)(blockIdx.x / tiles_n), m_stride = (int)(gridDim.x / tiles_n);
+  const int n_tiles = m_first < tiles_m ? (tiles_m - m_first + m_stride - 1) / m_stride : 0;
 
-  if (warp == kProducerWarp && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&mapAhi); tma_prefetch_desc(&mapBhi);
     if (NPROD == 3) { tma_prefetch_desc(&mapAlo); tma_prefetch_desc(&mapBlo); }
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
     for (int kb = 0; kb < kResK; ++kb) mbar_init(bfull + 8 * kb, 1);     // one per k-block of the resident B panel
     fence_barrier_init();
   }
-  __syncthreads();
+  __syncthreads();      // the last CTA-wide barrier: after the role split only mbarriers and named barriers 1, 2
 
-  if (warp == kProducerWarp) {
-    if (lane == 0) {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       // b_const: B holds constants of the step (the packed weights, written many kernels ago): its resident panel is
       // loaded while the predecessor kernel may still be running
       if (!b_const) pdl_wait();
@@ -320,24 +335,11 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
       }
       if (b_const) pdl_wait();
       pdl_trigger();
-      // l2pf (see the launcher): pull the A boxes of the NEXT row tile into L2 while this one is loaded, so that the
-      // ring's loads see L2 latency.
-      if (l2pf && m_first < tiles_m)
-        for (int kb = 0; kb < nk; ++kb) {
-          tma_prefetch_2d(&mapAhi, kb * kBK, m_first * kBM);
-          if (NPROD == 3) tma_prefetch_2d(&mapAlo, kb * kBK, m_first * kBM);
-        }
       int it = 0;
-      AVC_PROBE_DECL(w_empty);
-      AVC_PROBE_START(t_tma0);
+      AVC_PROBE(long long w_empty = 0; const long long t_tma0 = clock64());
       for (int mt = m_first; mt < tiles_m; mt += m_stride) {
-        const int m0 = mt * kBM;
-        const bool pf = l2pf && (mt + m_stride < tiles_m);
+        const int m0 = mt * kNtBM;
         for (int kb = 0; kb < nk; ++kb, ++it) {
-          if (pf) {
-            tma_prefetch_2d(&mapAhi, kb * kBK, m0 + m_stride * kBM);
-            if (NPROD == 3) tma_prefetch_2d(&mapAlo, kb * kBK, m0 + m_stride * kBM);
-          }
           const int s = it % Cfg::STAGES;
           AVC_PROBE_WAIT(w_empty, empty0 + 8 * s, ((it / Cfg::STAGES) & 1) ^ 1);
           const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
@@ -351,57 +353,74 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
         }
       }
       AVC_PROBE_ADD(EpiProbeId<Epi>::value, 0, w_empty);
-      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 1, AVC_PROBE_NOW() - t_tma0);
+      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 1, clock64() - t_tma0);
       AVC_PROBE_ADD(EpiProbeId<Epi>::value, 7, 1);
     }
-  } else {
-    const int g = warp >> 2, wq = warp & 3;      // consumer warpgroup, warp within it
-    const bool leader = (threadIdx.x & 127) == 0;
-    const int row_in = 64 * g + 16 * wq + (lane >> 2) + 8 * (lane & 1), col_in = 4 * ((lane >> 1) & 1);
-    pdl_wait();      // the functor's operands and outputs belong to predecessor kernels
-    float acc[BN / 2];
-    int it = 0, lt = 0;
-    AVC_PROBE_DECL(w_full);
-    AVC_PROBE_START(t_mma0);
-    EpiL2<Epi>::run(epi, m_first * kBM, n0, BN, M, (int)threadIdx.x, kConsumerThreads);
-    for (int mt = m_first; mt < tiles_m; mt += m_stride, ++lt) {
-      const int m0 = mt * kBM;
-      EpiL2<Epi>::run(epi, (mt + m_stride) * kBM, n0, BN, M, (int)threadIdx.x, kConsumerThreads);   // a tile ahead
-      int prev = -1;
-      for (int kb = 0; kb < nk; ++kb, ++it) {
-        const int s = it % Cfg::STAGES;
-        if (RESB && lt == 0) mbar_wait(bfull + 8 * kb, 0);      // this k-block of the B panel has landed (first tile only)
-        AVC_PROBE_WAIT(w_full, full0 + 8 * s, (it / Cfg::STAGES) & 1);
-        const uint32_t a_hi = smem_base + s * Cfg::STAGE_BYTES + (uint32_t)g * (64 * 128);   // this warpgroup's 64 rows
-        const uint32_t b_hi = RESB ? bres_base + kb * (Cfg::NOP * Cfg::B_BYTES) : smem_base + s * Cfg::STAGE_BYTES + Cfg::NOP * Cfg::A_BYTES;
-        const uint64_t da = make_wgmma_desc(a_hi, 16, 1024), db = make_wgmma_desc(b_hi, 16, 1024);
-        constexpr uint64_t kLoA = (uint64_t)(Cfg::A_BYTES >> 4), kLoB = (uint64_t)(Cfg::B_BYTES >> 4);
-        wgmma_fence_acc(acc);
-        wgmma_fence();
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int c = (warp >> 2) - 1, wq = warp & 3;      // consumer warpgroup, warp within it
+  const int tw = threadIdx.x & 127;
+  const bool leader = tw == 0;
+  const int row_in = 16 * wq + (lane >> 2) + 8 * (lane & 1), col_in = 4 * ((lane >> 1) & 1);
+  pdl_wait();      // the functor's operands and outputs belong to predecessor kernels
+  float acc[BN / 2];
+  AVC_PROBE(long long w_full = 0, w_turn = 0, t_mma = 0, t_epi = 0; const long long t_loop0 = clock64());
+  EpiL2<Epi>::run(epi, (m_first + c * m_stride) * kNtBM, n0, BN, M, tw, 128);
+  for (int j = c; j < n_tiles; j += 2) {
+    const int m0 = (m_first + j * m_stride) * kNtBM;
+    EpiL2<Epi>::run(epi, m0 + 2 * m_stride * kNtBM, n0, BN, M, tw, 128);      // this warpgroup's next tile
+    AVC_PROBE(const long long t_turn0 = clock64());
+    if (j > 0) named_bar_sync(kNtTurnBar + c, 256);      // the other warpgroup has issued tile j - 1
+    AVC_PROBE(const long long t_mma0 = clock64(); w_turn += t_mma0 - t_turn0);
+    int prev = -1, last = 0;
+    for (int kb = 0; kb < nk; ++kb) {
+      const int it = j * nk + kb, s = it % Cfg::STAGES;
+      if (RESB && j < 2) mbar_wait(bfull + 8 * kb, 0);      // this k-block of the B panel has landed (first tile only)
+      AVC_PROBE_WAIT(w_full, full0 + 8 * s, (it / Cfg::STAGES) & 1);
+      const uint32_t a_hi = smem_base + s * Cfg::STAGE_BYTES;
+      const uint32_t b_hi = RESB ? bres_base + kb * (Cfg::NOP * Cfg::B_BYTES) : smem_base + s * Cfg::STAGE_BYTES + Cfg::NOP * Cfg::A_BYTES;
+      const uint64_t da = make_wgmma_desc(a_hi, 16, 1024), db = make_wgmma_desc(b_hi, 16, 1024);
+      constexpr uint64_t kLoA = (uint64_t)(Cfg::A_BYTES >> 4), kLoB = (uint64_t)(Cfg::B_BYTES >> 4);
+      wgmma_fence_acc(acc);
+      wgmma_fence();
 #pragma unroll
-        for (int k4 = 0; k4 < kBK / 16; ++k4) {
-          wgmma_bf16<BN, 0, 0>(acc, da + 2 * k4, db + 2 * k4, (kb | k4) ? 1u : 0u);
-          if (NPROD == 3) {
-            wgmma_bf16<BN, 0, 0>(acc, da + 2 * k4, db + kLoB + 2 * k4, 1u);
-            wgmma_bf16<BN, 0, 0>(acc, da + kLoA + 2 * k4, db + 2 * k4, 1u);
-          }
+      for (int k4 = 0; k4 < kBK / 16; ++k4) {
+        wgmma_bf16<BN, 0, 0>(acc, da + 2 * k4, db + 2 * k4, (kb | k4) ? 1u : 0u);
+        if (NPROD == 3) {
+          wgmma_bf16<BN, 0, 0>(acc, da + 2 * k4, db + kLoB + 2 * k4, 1u);
+          wgmma_bf16<BN, 0, 0>(acc, da + kLoA + 2 * k4, db + 2 * k4, 1u);
         }
-        wgmma_commit();
-        wgmma_fence_acc(acc);
+      }
+      wgmma_commit();
+      wgmma_fence_acc(acc);
+      last = s;
+      if (kb + 1 < nk) {
         wgmma_wait<1>();                      // the previous k-block's MMAs are done: its stage can be refilled
         if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
         prev = s;
       }
+    }
+    if (j + 1 < n_tiles) named_bar_arrive(kNtTurnBar + (c ^ 1), 256);      // all k-blocks issued: the other's turn
+    epilogue_nt<BN>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane, [&] {
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
-      if (leader) mbar_arrive(empty0 + 8 * prev);
-      epilogue_nt<BN>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane);
-    }
-    if (threadIdx.x == 0) {
-      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 3, w_full);
-      AVC_PROBE_ADD(EpiProbeId<Epi>::value, 4, AVC_PROBE_NOW() - t_mma0);
-    }
+      if (leader) {
+        if (prev >= 0) mbar_arrive(empty0 + 8 * prev);
+        mbar_arrive(empty0 + 8 * last);
+      }
+      AVC_PROBE(t_mma += clock64() - t_mma0);
+    });
+    AVC_PROBE(t_epi += clock64() - t_mma0);
   }
+  AVC_PROBE(if (leader) {
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 2, w_full);
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 3, w_turn);
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 4, t_mma);
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 5, t_epi - t_mma);
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 6, clock64() - t_loop0);
+  })
 }
 
 template <int BN, int NPROD, bool RESB, typename Epi>
@@ -409,10 +428,10 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
                                        const Epi& epi, bool b_const) {
   using Cfg = TcCfg<BN, NPROD, RESB>;
   CUtensorMap mAh, mAl, mBh, mBl;
-  AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kBM));
+  AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
   AVC_TRY(make_map_bf16_cached(&mBh, B.hi, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
   if (NPROD == 3) {
-    AVC_TRY(make_map_bf16_cached(&mAl, A.lo, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kBM));
+    AVC_TRY(make_map_bf16_cached(&mAl, A.lo, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
     AVC_TRY(make_map_bf16_cached(&mBl, B.lo, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
   } else {
     mAl = mAh; mBl = mBh;
@@ -430,18 +449,12 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
     AVC_CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
   }
   const int tiles_n = ceil_div(N, BN);
-  const int ntiles = ceil_div(M, kBM) * tiles_n;
+  const int ntiles = ceil_div(M, kNtBM) * tiles_n;
   int g = ntiles < num_sms ? ntiles : num_sms;         // persistent: at most one CTA per SM ...
   g = (g / tiles_n) * tiles_n;                         // ... and a whole number of CTAs per column tile
   if (g < tiles_n) return AVC_E_BADCFG;
   dim3 grid(g);
-  // TMA-prefetch of the next row tile's A boxes into L2, so that the ring's loads see L2 rather than DRAM latency.
-  // Launches whose epilogue pulls its own operands into L2 (Epi::kNoATilePrefetch) keep it off.
-  // AVC_NT_L2PF=0 / 1 forces it off / on everywhere.
-  static int l2pf_env = -2;
-  if (l2pf_env == -2) { const char* e = getenv("AVC_NT_L2PF"); l2pf_env = e ? (atoi(e) != 0 ? 1 : 0) : -1; }
-  const int l2pf = l2pf_env >= 0 ? l2pf_env : (EpiNoAPf<Epi>::value ? 0 : 1);
-  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, l2pf, b_const ? 1 : 0));
+  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kNtThreads), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, b_const ? 1 : 0));
   AVC_LAUNCH_TRY();
   return 0;
 }

@@ -585,9 +585,8 @@ extern "C" {
 
 int avc_abi_version(void) { return AVC_ABI_VERSION; }
 
-// Stall probe of the wgmma NT tiles (diagnostic builds only: -DAVC_NT_PROBE=1).  out[16][8]: per functor slot the summed
-// cycles {TMA waits empty, TMA loop, MMA waits tempty, MMA waits full, MMA loop, epilogue warp waits tfull, epilogue loop,
-// CTAs}.  Returns AVC_E_BADCFG in a regular build.
+// Stall probe of the wgmma NT tiles (diagnostic builds only: -DAVC_NT_PROBE=1).  out[16][8]: per functor the summed
+// cycles of the slots listed in avc_gemm_tc.cuh (AVC_NT_PROBE).  Returns AVC_E_BADCFG in a regular build.
 int avc_nt_probe_read(unsigned long long* host_out, int reset) {
 #ifdef AVC_NT_PROBE
   if (!host_out) return AVC_E_NULL;

@@ -31,14 +31,6 @@ __device__ __forceinline__ void split16_get4(uint2 hi, uint2 lo, float v[4]) {
 __device__ __forceinline__ float split16_get(const Split16& s, size_t row, int col) {
   return __bfloat162float(s.hi[row * s.ld + col]) + __bfloat162float(s.lo[row * s.ld + col]);
 }
-// no null check (callers test s.hi once for several groups); off = row * s.ld + col
-__device__ __forceinline__ void split16_put4_at(const Split16& s, size_t off, const float v[4]) {
-  const uint32_t h01 = bf16x2_bits(v[0], v[1]), h23 = bf16x2_bits(v[2], v[3]);
-  const float r0 = v[0] - __uint_as_float(h01 << 16), r1 = v[1] - __uint_as_float(h01 & 0xffff0000u);
-  const float r2 = v[2] - __uint_as_float(h23 << 16), r3 = v[3] - __uint_as_float(h23 & 0xffff0000u);
-  *reinterpret_cast<uint2*>(s.hi + off) = make_uint2(h01, h23);
-  *reinterpret_cast<uint2*>(s.lo + off) = make_uint2(bf16x2_bits(r0, r1), bf16x2_bits(r2, r3));
-}
 __device__ __forceinline__ void split16_put4(const Split16& s, size_t row, int col, const float v[4]) {
   if (!s.hi) return;
   const uint32_t h01 = bf16x2_bits(v[0], v[1]), h23 = bf16x2_bits(v[2], v[3]);
@@ -683,8 +675,9 @@ __global__ void k_heads_dgrad(const float* __restrict__ y6bar, const float* __re
 // =============================================================================================
 // GEMM epilogue functors.  (row, col..col+3, acc) with col % 4 == 0; N = valid output width.
 //
-// Every functor splits its work in two so that the tcgen05 epilogue can issue the global loads that do NOT depend
-// on the accumulator a whole tile ahead (the epilogue is bound by bytes in flight, not by issue slots):
+// Every functor splits its work in two so that the wgmma epilogue can issue the global loads that do NOT depend on the
+// accumulator ahead of the arithmetic, the first ones while the MMAs still run (the epilogue is bound by bytes in flight,
+// not by issue slots):
 //     Aux  prefetch(row, col)                      the stashed activations / biases this output group needs
 //     void operator()(row, col, acc, aux)          the arithmetic and the stores
 // operator()(row, col, acc) is the two back to back (what the fp32 FFMA engine calls).
@@ -712,40 +705,6 @@ struct EpiValue {
   const float* bias; float* D1; int ldz; float* OUT; int ldo; float oscale; int N; Split16 o16;
   struct Aux { float4 b; };
   __device__ __forceinline__ Aux prefetch(int, int col) const { return {load4_guarded(bias, col, N)}; }
-  __device__ __forceinline__ void prefetch4(int col, Aux (&dst)[4]) const {      // the bias depends on the column only
-    const Aux b = {col + 3 < N ? *reinterpret_cast<const float4*>(bias + col) : load4_guarded(bias, col, N)};
-    dst[0] = b; dst[1] = b; dst[2] = b; dst[3] = b;
-  }
-  // four whole groups (rows row + 8 p): branch-free math for all 16 elements, then each output's stores under ONE test
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    if (col + 3 >= N) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) (*this)(row + 8 * p, col, a[p], x[p]);
-      return;
-    }
-    float hh[4][4], dd[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      const float z[4] = {a[p].x + x[p].b.x, a[p].y + x[p].b.y, a[p].z + x[p].b.z, a[p].w + x[p].b.w};
-      softplus100_both4<FAST>(z, hh[p], dd[p]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) hh[p][i] *= oscale;
-    }
-    if (D1) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(D1 + (size_t)(row + 8 * p) * ldz + col) = make_float4(dd[p][0], dd[p][1], dd[p][2], dd[p][3]);
-    }
-    if (OUT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(OUT + (size_t)(row + 8 * p) * ldo + col) = make_float4(hh[p][0], hh[p][1], hh[p][2], hh[p][3]);
-    }
-    if (o16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(o16, (size_t)(row + 8 * p) * o16.ld + col, hh[p]);
-    }
-  }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
     const float bb[4] = {x.b.x, x.b.y, x.b.z, x.b.w};
@@ -776,27 +735,6 @@ struct EpiBias {
   const float* bias; float* OUT; int ldo; int N; Split16 o16;
   struct Aux { float4 b; };
   __device__ __forceinline__ Aux prefetch(int, int col) const { return {load4_guarded(bias, col, N)}; }
-  __device__ __forceinline__ void prefetch4(int col, Aux (&dst)[4]) const {      // the bias depends on the column only
-    const Aux b = {col + 3 < N ? *reinterpret_cast<const float4*>(bias + col) : load4_guarded(bias, col, N)};
-    dst[0] = b; dst[1] = b; dst[2] = b; dst[3] = b;
-  }
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    float v[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      v[p][0] = (col < N) ? a[p].x + x[p].b.x : 0.f; v[p][1] = (col + 1 < N) ? a[p].y + x[p].b.y : 0.f;
-      v[p][2] = (col + 2 < N) ? a[p].z + x[p].b.z : 0.f; v[p][3] = (col + 3 < N) ? a[p].w + x[p].b.w : 0.f;
-    }
-    if (OUT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(OUT + (size_t)(row + 8 * p) * ldo + col) = make_float4(v[p][0], v[p][1], v[p][2], v[p][3]);
-    }
-    if (o16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(o16, (size_t)(row + 8 * p) * o16.ld + col, v[p]);
-    }
-  }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
     const float bb[4] = {x.b.x, x.b.y, x.b.z, x.b.w};
@@ -821,28 +759,6 @@ struct EpiChain {
   }
   __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
     tc::l2_prefetch_tile<4>(D1prev, Npp, Npp, m0, n0, bn, M, et, nth);
-  }
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    if (col + 3 >= Nprev) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) (*this)(row + 8 * p, col, a[p], x[p]);
-      return;
-    }
-    float q[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      q[p][0] = x[p].d.x * a[p].x * s; q[p][1] = x[p].d.y * a[p].y * s;
-      q[p][2] = x[p].d.z * a[p].z * s; q[p][3] = x[p].d.w * a[p].w * s;
-    }
-    if (QTprev) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(QTprev + (size_t)(row + 8 * p) * Npp + col) = make_float4(q[p][0], q[p][1], q[p][2], q[p][3]);
-    }
-    if (q16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(q16, (size_t)(row + 8 * p) * q16.ld + col, q[p]);
-    }
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
@@ -873,7 +789,6 @@ struct EpiChain {
 
 // gradient chain, layer 0: ge += acc  (width E)
 struct EpiGe {
-  static constexpr bool kNoATilePrefetch = true;     // measured slower with the A-tile L2 prefetch (avc_gemm_tc.cuh launcher)
   static constexpr int kProbeId = 10;      // slot of the optional NT stall probe (avc_gemm_tc.cuh)
   float* GE; int EP; int E;
   struct Aux { float4 g; };
@@ -898,35 +813,6 @@ struct EpiColor0 {
   struct Aux { float4 c0, c1; };
   __device__ __forceinline__ Aux prefetch(int row, int) const {
     return {*reinterpret_cast<const float4*>(cin + (size_t)row * 8), *reinterpret_cast<const float4*>(cin + (size_t)row * 8 + 4)};
-  }
-  // the bias and the six Wx rows depend on the column only: loaded once for the four groups
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    const float4 b4 = *reinterpret_cast<const float4*>(bias + col);
-    float4 w[6];
-#pragma unroll
-    for (int j = 0; j < 6; ++j) w[j] = *reinterpret_cast<const float4*>(WxT + (size_t)j * ldt + col);
-    float v[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      const float cj[6] = {x[p].c0.x, x[p].c0.y, x[p].c0.z, x[p].c0.w, x[p].c1.x, x[p].c1.y};
-      v[p][0] = a[p].x + b4.x; v[p][1] = a[p].y + b4.y; v[p][2] = a[p].z + b4.z; v[p][3] = a[p].w + b4.w;
-#pragma unroll
-      for (int j = 0; j < 6; ++j) {
-        v[p][0] = fmaf(cj[j], w[j].x, v[p][0]); v[p][1] = fmaf(cj[j], w[j].y, v[p][1]);
-        v[p][2] = fmaf(cj[j], w[j].z, v[p][2]); v[p][3] = fmaf(cj[j], w[j].w, v[p][3]);
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[p][i] = fmaxf(v[p][i], 0.f);
-    }
-    if (OUT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(OUT + (size_t)(row + 8 * p) * ldo + col) = make_float4(v[p][0], v[p][1], v[p][2], v[p][3]);
-    }
-    if (o16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(o16, (size_t)(row + 8 * p) * o16.ld + col, v[p]);
-    }
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
@@ -954,27 +840,6 @@ struct EpiRelu {
   __device__ __forceinline__ Aux prefetch(int, int col) const {
     return {make_float4(bias[col], bias[col + 1], bias[col + 2], bias[col + 3])};
   }
-  __device__ __forceinline__ void prefetch4(int col, Aux (&dst)[4]) const {
-    const Aux b = {*reinterpret_cast<const float4*>(bias + col)};
-    dst[0] = b; dst[1] = b; dst[2] = b; dst[3] = b;
-  }
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    float v[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      v[p][0] = fmaxf(a[p].x + x[p].b.x, 0.f); v[p][1] = fmaxf(a[p].y + x[p].b.y, 0.f);
-      v[p][2] = fmaxf(a[p].z + x[p].b.z, 0.f); v[p][3] = fmaxf(a[p].w + x[p].b.w, 0.f);
-    }
-    if (OUT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(OUT + (size_t)(row + 8 * p) * ldo + col) = make_float4(v[p][0], v[p][1], v[p][2], v[p][3]);
-    }
-    if (o16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(o16, (size_t)(row + 8 * p) * o16.ld + col, v[p]);
-    }
-  }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
     v[0] = fmaxf(v[0] + x.b.x, 0.f); v[1] = fmaxf(v[1] + x.b.y, 0.f);
@@ -999,31 +864,6 @@ struct EpiDgradRelu {
   __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
     if (Hm) tc::l2_prefetch_tile<4>(Hm, ld, ld, m0, n0, bn, M, et, nth);
     else tc::l2_prefetch_tile<2>(Hhi, o16.ld, o16.ld, m0, n0, bn, M, et, nth);
-  }
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    float v[4][4];
-    if (Hm) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        v[p][0] = __uint_as_float(x[p].raw.x) > 0.f ? a[p].x : 0.f; v[p][1] = __uint_as_float(x[p].raw.y) > 0.f ? a[p].y : 0.f;
-        v[p][2] = __uint_as_float(x[p].raw.z) > 0.f ? a[p].z : 0.f; v[p][3] = __uint_as_float(x[p].raw.w) > 0.f ? a[p].w : 0.f;
-      }
-    } else {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        v[p][0] = (x[p].raw.x & 0x00007fffu) ? a[p].x : 0.f; v[p][1] = (x[p].raw.x & 0x7fff0000u) ? a[p].y : 0.f;
-        v[p][2] = (x[p].raw.y & 0x00007fffu) ? a[p].z : 0.f; v[p][3] = (x[p].raw.y & 0x7fff0000u) ? a[p].w : 0.f;
-      }
-    }
-    if (OUT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(OUT + (size_t)(row + 8 * p) * ld + col) = make_float4(v[p][0], v[p][1], v[p][2], v[p][3]);
-    }
-    if (o16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(o16, (size_t)(row + 8 * p) * o16.ld + col, v[p]);
-    }
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
@@ -1059,7 +899,6 @@ struct EpiStore {
 //   ubar_next[row][col] = sp'(z_l) * qbar * s_next            (col < N_l)
 //   zbar_l[row][col]    = beta (1 - sp'(z_l)) * qt_l * qbar    (= softplus'' * ua_{l+1} * qbar), padding zeroed
 struct EpiChainBwd {
-  static constexpr bool kNoATilePrefetch = true;     // measured slower with the A-tile L2 prefetch (avc_gemm_tc.cuh launcher)
   static constexpr int kProbeId = 3;      // slot of the optional NT stall probe (avc_gemm_tc.cuh)
   int N, Np; const float* D1; const float* QT; Split16 qt16; float* ZBAR; float* UNEXT; int ldu; float s_next; Split16 u16;
   // qt_l comes from its fp32 copy QT or, when QT is NULL (tcgen05 engine), from the split hi + lo
@@ -1088,46 +927,6 @@ struct EpiChainBwd {
   }
   __device__ __forceinline__ float qt_at(int row, int c) const {
     return QT ? QT[(size_t)row * Np + c] : split16_get(qt16, (size_t)row, c);
-  }
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    if (col + 3 >= Np) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) (*this)(row + 8 * p, col, a[p], x[p]);
-      return;
-    }
-    float qq[4][4];
-    if (QT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        qq[p][0] = __uint_as_float(x[p].q.x); qq[p][1] = __uint_as_float(x[p].q.y);
-        qq[p][2] = __uint_as_float(x[p].q.z); qq[p][3] = __uint_as_float(x[p].q.w);
-      }
-    } else {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_get4(make_uint2(x[p].q.x, x[p].q.y), make_uint2(x[p].q.z, x[p].q.w), qq[p]);
-    }
-    float u[4][4], zb[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      const float dd[4] = {x[p].d.x, x[p].d.y, x[p].d.z, x[p].d.w}, v[4] = {a[p].x, a[p].y, a[p].z, a[p].w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        u[p][i] = dd[i] * v[i] * s_next;
-        zb[p][i] = kBeta * (1.f - dd[i]) * qq[p][i] * v[i];
-      }
-    }
-#pragma unroll
-    for (int p = 0; p < 4; ++p)
-      *reinterpret_cast<float4*>(ZBAR + (size_t)(row + 8 * p) * Np + col) = make_float4(zb[p][0], zb[p][1], zb[p][2], zb[p][3]);
-    if (UNEXT) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(UNEXT + (size_t)(row + 8 * p) * ldu + col) = make_float4(u[p][0], u[p][1], u[p][2], u[p][3]);
-    }
-    if (u16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(u16, (size_t)(row + 8 * p) * u16.ld + col, u[p]);
-    }
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
@@ -1172,7 +971,6 @@ struct EpiChainBwd {
 // value backward dgrad into layer l-1: abar = (acc [+ sdfbar[row] * wsdf[col]]) * s ;
 //   zbar_prev[row][col] = sp'(z_prev) * abar + zbar_prev[row][col]   (col < Nprev);  D1prev = softplus'(z_prev) stash
 struct EpiDgrad {
-  static constexpr bool kNoATilePrefetch = true;     // measured slower with the A-tile L2 prefetch (avc_gemm_tc.cuh launcher)
   static constexpr int kProbeId = 4;      // slot of the optional NT stall probe (avc_gemm_tc.cuh)
   int Nprev, Npp; float s; const float* D1prev; float* ZBARprev; const float* sdfbar; const float* wsdf;
   float sdf_inv_scale; Split16 z16; int store_f32;     // store_f32 = 0: only the split of the new zbar_prev is kept
@@ -1184,42 +982,6 @@ struct EpiDgrad {
   __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
     tc::l2_prefetch_tile<4>(D1prev, Npp, Npp, m0, n0, bn, M, et, nth);
     tc::l2_prefetch_tile<4>(ZBARprev, Npp, Npp, m0, n0, bn, M, et, nth);
-  }
-  __device__ __forceinline__ void quad(int row, int col, const float4 (&a)[4], const Aux (&x)[4]) const {
-    if (col + 3 >= Npp) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) (*this)(row + 8 * p, col, a[p], x[p]);
-      return;
-    }
-    float ab[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) { ab[p][0] = a[p].x; ab[p][1] = a[p].y; ab[p][2] = a[p].z; ab[p][3] = a[p].w; }
-    if (sdfbar) {      // only the launch below the last linear: the sdf row of W_L rides along as a rank-1 term
-      const float4 w4 = *reinterpret_cast<const float4*>(wsdf + col);
-      float sb[4];
-#pragma unroll
-      for (int p = 0; p < 4; ++p) sb[p] = sdfbar[row + 8 * p] * sdf_inv_scale;
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        ab[p][0] = fmaf(sb[p], w4.x, ab[p][0]); ab[p][1] = fmaf(sb[p], w4.y, ab[p][1]);
-        ab[p][2] = fmaf(sb[p], w4.z, ab[p][2]); ab[p][3] = fmaf(sb[p], w4.w, ab[p][3]);
-      }
-    }
-    float r[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      r[p][0] = fmaf(x[p].d.x, ab[p][0] * s, x[p].zb.x); r[p][1] = fmaf(x[p].d.y, ab[p][1] * s, x[p].zb.y);
-      r[p][2] = fmaf(x[p].d.z, ab[p][2] * s, x[p].zb.z); r[p][3] = fmaf(x[p].d.w, ab[p][3] * s, x[p].zb.w);
-    }
-    if (store_f32) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-        *reinterpret_cast<float4*>(ZBARprev + (size_t)(row + 8 * p) * Npp + col) = make_float4(r[p][0], r[p][1], r[p][2], r[p][3]);
-    }
-    if (z16.hi) {
-#pragma unroll
-      for (int p = 0; p < 4; ++p) split16_put4_at(z16, (size_t)(row + 8 * p) * z16.ld + col, r[p]);
-    }
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;

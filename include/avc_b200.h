@@ -366,9 +366,9 @@ int avc_uniform_fill(uint32_t seed, int32_t n, float lo, float hi, float* out, a
  * [4] epilogue waiting for the accumulator, [5] epilogue work); this call synchronises the device and copies them. */
 int avc_chain_debug_read(long long* out8);
 /* Stall probe of the wgmma NT tiles: only in a diagnostic build (-DAVC_NT_PROBE=1, tools/nt_probe.py); a regular
- * build returns AVC_E_BADCFG.  host_out[16][8]: per epilogue functor the summed cycles {TMA warp waiting for a free
- * stage, TMA loop, MMA warp waiting for a drained accumulator, MMA warp waiting for operands, MMA loop, one epilogue
- * warp waiting for the accumulator, its loop, CTAs}; reset != 0 clears the counters. */
+ * build returns AVC_E_BADCFG.  host_out[16][8]: per epilogue functor the summed cycles {producer waiting for a free
+ * stage, producer loop, consumers waiting for operands, consumers waiting for their turn, consumers' MMAs, consumers'
+ * epilogues, consumers' loops, CTAs} (consumer slots: both consumer warpgroups); reset != 0 clears the counters. */
 int avc_nt_probe_read(unsigned long long* host_out, int reset);
 
 int avc_march_count(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, int32_t* counts,

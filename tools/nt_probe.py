@@ -3,10 +3,13 @@
     python tools/nt_probe.py --build      # here (nvcc): avatarclip_b200/libavc_b200_probe.so = product objects, with
                                           # avc_neus.cu recompiled with -DAVC_NT_PROBE=1
     python tools/nt_probe.py --run OUT    # on the GPU: a few steps of the bench workload through the probe build,
-                                          # per epilogue functor the share of its loop each warp role spent waiting
+                                          # per epilogue functor where each warp role's loop time went
 
-The probe adds a clock64 pair around every mbarrier wait of the three warp roles (TMA producer, MMA issuer, one epilogue
-warp) and sums them per functor (avc_gemm_tc.cuh, AVC_NT_PROBE)."""
+The probe takes clock64 stamps in the TMA producer and in the leading thread of each consumer warpgroup: the producer's
+waits for a free stage, the consumers' waits for operands and for their turn at the tensor pipe, and the time from a
+consumer's turn to its MMAs' completion and from there to the end of its epilogue, summed per functor
+(avc_gemm_tc.cuh, AVC_NT_PROBE).  `busy_over_wall` is the MMA and epilogue time of both consumer warpgroups over the loop
+time of one: above 1, the two worked at the same time (one's MMAs under the other's epilogue)."""
 import argparse
 import ctypes as C
 import json
@@ -65,12 +68,15 @@ def run(out_path):
         if v[7] == 0:
             continue
         ctas = v[7]
+        cons = max(v[6], 1)      # loop cycles of both consumer warpgroups
         rep[NAMES.get(i, str(i))] = {
             "ctas_per_step": ctas / steps,
-            # producer warp; consumer warpgroup 0 (its MMAs and epilogues)
-            "loop_kcycles_per_cta": {"tma": v[1] / ctas / 1e3, "consumer": v[4] / ctas / 1e3},
-            "tma_waits_free_stage": v[0] / max(v[1], 1),
-            "consumer_waits_operands": v[3] / max(v[4], 1),
+            "loop_kcycles_per_cta": {"producer": v[1] / ctas / 1e3, "consumer": v[6] / (2 * ctas) / 1e3},
+            "producer_waits_free_stage": v[0] / max(v[1], 1),
+            # shares of a consumer warpgroup's loop; the MMA share includes its operand and B-panel waits
+            "consumer": {"waits_operands": v[2] / cons, "waits_turn": v[3] / cons, "mma": v[4] / cons,
+                         "epilogue": v[5] / cons},
+            "busy_over_wall": (v[4] + v[5]) / (cons / 2),
         }
     with open(out_path, "w") as f:
         json.dump(rep, f, indent=1)
