@@ -466,9 +466,7 @@ static inline int launch_gemm_tc_nt(cudaStream_t st, int64_t M, int N, int K, co
                                     const Epi& epi, bool b_const = false) {
   if (M <= 0 || N <= 0) return 0;
   // K <= 256: the B panel stays resident in shared memory (RESB); longer reductions stream both operands.
-  static int resb = -1;       // AVC_NT_RESB=0 forces the streaming variant (tuning knob)
-  if (resb < 0) { const char* e = getenv("AVC_NT_RESB"); resb = (e && atoi(e) == 0) ? 0 : 1; }
-  if (resb && K <= kResK * kBK) {
+  if (K <= kResK * kBK) {
     if (N <= 64) return launch_gemm_tc_nt_bn<64, NPROD, true, Epi>(st, M, N, K, A, B, epi, b_const);
     return launch_gemm_tc_nt_bn<128, NPROD, true, Epi>(st, M, N, K, A, B, epi, b_const);
   }
