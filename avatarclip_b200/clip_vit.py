@@ -84,6 +84,39 @@ class _ClipFn(torch.autograd.Function):
         return None, dx, None, None
 
 
+class WeightPacker:
+    """Device copies of frozen weights for the library's weight structs: fp16 GEMM matrices (what ``clip.load`` keeps on
+    CUDA) and fp32 vectors.  ``keep`` holds the tensors alive as long as the raw pointers are in use."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        self.keep = []
+
+    def h16(self, t: torch.Tensor) -> int:
+        t = t.detach().to(self.device, torch.float16).contiguous()
+        self.keep.append(t)
+        return t.data_ptr()
+
+    def f32(self, t: torch.Tensor) -> int:
+        t = t.detach().to(self.device, torch.float32).contiguous()
+        self.keep.append(t)
+        return t.data_ptr()
+
+    def layer(self, lw: ClipLayerW, sd: Dict[str, torch.Tensor], p: str, transposed: bool):
+        """One residual block ``p`` = "transformer.resblocks.{i}." into ``lw``; the transposed copies (input-gradient
+        GEMMs) only when ``transposed``, else their pointers stay NULL."""
+        h16, f32 = self.h16, self.f32
+        lw.ln1_g, lw.ln1_b = f32(sd[p + "ln_1.weight"]), f32(sd[p + "ln_1.bias"])
+        lw.ln2_g, lw.ln2_b = f32(sd[p + "ln_2.weight"]), f32(sd[p + "ln_2.bias"])
+        for name, key in (("qkv", "attn.in_proj_weight"), ("out", "attn.out_proj.weight"),
+                          ("fc", "mlp.c_fc.weight"), ("proj", "mlp.c_proj.weight")):
+            setattr(lw, "w_" + name, h16(sd[p + key]))
+            if transposed:
+                setattr(lw, "w_" + name + "_t", h16(sd[p + key].t()))
+        lw.b_qkv, lw.b_out = f32(sd[p + "attn.in_proj_bias"]), f32(sd[p + "attn.out_proj.bias"])
+        lw.b_fc, lw.b_proj = f32(sd[p + "mlp.c_fc.bias"]), f32(sd[p + "mlp.c_proj.bias"])
+
+
 class ClipImageTower:
     def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", heads: int = None):
         L = _lib.lib()
@@ -101,19 +134,10 @@ class ClipImageTower:
         self.cfg = ClipCfg(image_size=grid * patch, patch=patch, width=width, layers=layers, heads=heads, mlp=mlp,
                            out_dim=out_dim)
         self.device = dev
-        self._keep = []
+        pk = WeightPacker(dev)
+        self._keep = pk.keep
         self.w = ClipW()
-
-        def h16(t):
-            t = t.detach().to(dev, torch.float16).contiguous()
-            self._keep.append(t)
-            return t.data_ptr()
-
-        def f32(t):
-            t = t.detach().to(dev, torch.float32).contiguous()
-            self._keep.append(t)
-            return t.data_ptr()
-
+        h16, f32 = pk.h16, pk.f32
         wp = conv.reshape(width, -1)
         self.w.w_patch, self.w.w_patch_t = h16(wp), h16(wp.t())
         self.w.cls, self.w.pos = f32(sd["class_embedding"]), f32(sd["positional_embedding"])
@@ -121,16 +145,7 @@ class ClipImageTower:
         self.w.ln_post_g, self.w.ln_post_b = f32(sd["ln_post.weight"]), f32(sd["ln_post.bias"])
         self.w.proj = f32(sd["proj"].half())     # fp16-valued (as clip.load keeps it), stored fp32
         for i in range(layers):
-            p = f"transformer.resblocks.{i}."
-            lw = self.w.layer[i]
-            lw.ln1_g, lw.ln1_b = f32(sd[p + "ln_1.weight"]), f32(sd[p + "ln_1.bias"])
-            lw.ln2_g, lw.ln2_b = f32(sd[p + "ln_2.weight"]), f32(sd[p + "ln_2.bias"])
-            for name, key in (("qkv", "attn.in_proj_weight"), ("out", "attn.out_proj.weight"),
-                              ("fc", "mlp.c_fc.weight"), ("proj", "mlp.c_proj.weight")):
-                setattr(lw, "w_" + name, h16(sd[p + key]))
-                setattr(lw, "w_" + name + "_t", h16(sd[p + key].t()))
-            lw.b_qkv, lw.b_out = f32(sd[p + "attn.in_proj_bias"]), f32(sd[p + "attn.out_proj.bias"])
-            lw.b_fc, lw.b_proj = f32(sd[p + "mlp.c_fc.bias"]), f32(sd[p + "mlp.c_proj.bias"])
+            pk.layer(self.w.layer[i], sd, f"transformer.resblocks.{i}.", transposed=True)
         self._zero_text = None
 
     def _workspace(self, B: int) -> torch.Tensor:

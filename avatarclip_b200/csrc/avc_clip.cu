@@ -1228,3 +1228,204 @@ int avc_clip_loss_bwd(const avc_clip_cfg* cfg, const avc_clip_weights* wt, int32
 }
 
 }  // extern "C"
+
+// ================================================================================================
+// CLIP text tower forward (openai/CLIP `CLIP.encode_text`, called from main.py:276,282,288).  Forward only: the text
+// weights are frozen and the reference detaches the embedding.  The same pre-LN residual blocks as the image tower,
+// built from its kernels (k_layernorm, gemm16 with EpiBiasStore / EpiResidual / EpiFc, k_head_proj) plus three new
+// ones: the token-embedding gather, causal attention over up to 128 tokens and the end-of-text row gather.  Every
+// position of the context runs (no truncation at the end-of-text token): the tower runs once per training run.
+// ================================================================================================
+namespace {
+
+constexpr int kTextMaxT = 128;     // max context
+constexpr int kTextAP = AD + 1;    // shared-memory row pitch of q / k / v: row j's element d sits in bank (j + d) % 32
+constexpr int kTextAttnThreads = 256;
+constexpr int kTextAttnSmem = (3 * kTextMaxT * kTextAP + (kTextAttnThreads / 32) * kTextMaxT) * (int)sizeof(float);
+
+// x[b,t] = token_embedding[tok[b,t]] + positional_embedding[t] (fp32).  An id outside [0, vocab) is clamped so that
+// the gather never leaves the table; the Python wrapper rejects such ids before the call.
+__global__ void k_text_embed(const int32_t* __restrict__ tok, const float* __restrict__ emb,
+                             const float* __restrict__ pos, int B, int T, int Wd, int vocab, float* __restrict__ x) {
+  pdl_enter();
+  const int bx = blockIdx.x, nt = blockDim.x, tid = threadIdx.x;
+  const int64_t i = (int64_t)bx * nt + tid;
+  if (i >= (int64_t)B * T * Wd) return;
+  const int c = (int)(i % Wd);
+  const int64_t row = i / Wd;
+  const int t = (int)(row % T);
+  const int id = min(max(tok[row], 0), vocab - 1);
+  x[i] = emb[(size_t)id * Wd + c] + pos[(size_t)t * Wd + c];
+}
+
+// Causal self-attention, one CTA per (sequence, head): T <= 128 tokens, head dim 64, scale 1/8, fp32 FFMA and softmax.
+// Query row a attends to keys 0..a (build_attention_mask: -inf above the diagonal), so no row is ever fully masked.
+// qkv: [B*T][3W] fp32 (q | k | v).  o16: [B*T][W] fp16 operand of out_proj.  Warp w owns the query rows w, w + 8, ...:
+// lanes split the keys for the scores and the head dimension for the output.
+__global__ void __launch_bounds__(kTextAttnThreads)
+k_causal_attention(const float* __restrict__ qkv, int T, int Wd, int heads, __half* __restrict__ o16) {
+  pdl_enter();
+  extern __shared__ __align__(16) unsigned char dyn_smem[];
+  const int bx = blockIdx.x, nt = blockDim.x, tid = threadIdx.x;
+  float* q = reinterpret_cast<float*>(dyn_smem);   // [T][kTextAP]
+  float* k = q + kTextMaxT * kTextAP;
+  float* v = k + kTextMaxT * kTextAP;
+  float* pw = v + kTextMaxT * kTextAP;              // [warps][kTextMaxT] probabilities of the warp's current row
+  const int b = bx / heads, h = bx % heads;
+  const float* base = qkv + (size_t)b * T * 3 * Wd + h * AD;
+  for (int i = tid; i < T * (AD / 4); i += nt) {
+    const int t = i / (AD / 4), d = (i % (AD / 4)) * 4;
+    const float* r = base + (size_t)t * 3 * Wd + d;
+    const float4 a = *reinterpret_cast<const float4*>(r);
+    const float4 c = *reinterpret_cast<const float4*>(r + Wd);
+    const float4 e = *reinterpret_cast<const float4*>(r + 2 * Wd);
+    float* qs = q + t * kTextAP + d; float* ks = k + t * kTextAP + d; float* vs = v + t * kTextAP + d;
+    qs[0] = a.x; qs[1] = a.y; qs[2] = a.z; qs[3] = a.w;
+    ks[0] = c.x; ks[1] = c.y; ks[2] = c.z; ks[3] = c.w;
+    vs[0] = e.x; vs[1] = e.y; vs[2] = e.z; vs[3] = e.w;
+  }
+  __syncthreads();
+  const int lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
+  float* p = pw + warp * kTextMaxT;
+  for (int a = warp; a < T; a += nw) {
+    const float* qa = q + a * kTextAP;
+    float mx = -INFINITY;
+    for (int j = lane; j <= a; j += 32) {
+      const float* kj = k + j * kTextAP;
+      float s = 0.f;
+#pragma unroll 16
+      for (int d = 0; d < AD; ++d) s = fmaf(qa[d], kj[d], s);
+      s *= 0.125f;
+      p[j] = s;
+      mx = fmaxf(mx, s);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    float sum = 0.f;
+    for (int j = lane; j <= a; j += 32) { const float e = expf(p[j] - mx); p[j] = e; sum += e; }
+    const float inv = 1.f / warp_sum(sum);
+    __syncwarp();
+    float o0 = 0.f, o1 = 0.f;
+    for (int j = 0; j <= a; ++j) {
+      const float pj = p[j];
+      o0 = fmaf(pj, v[j * kTextAP + lane], o0);
+      o1 = fmaf(pj, v[j * kTextAP + lane + 32], o1);
+    }
+    __half* out = o16 + ((size_t)b * T + a) * Wd + h * AD;
+    out[lane] = __float2half_rn(o0 * inv);
+    out[lane + 32] = __float2half_rn(o1 * inv);
+    __syncwarp();      // p is rewritten for the warp's next row
+  }
+}
+
+// End-of-text pooling: eot[b] = x[b, argmax_t tok[b,t]] (the first maximum, as torch.argmax; <|endoftext|> is the
+// largest id).  One CTA (one warp) per sequence.
+__global__ void k_text_eot_rows(const int32_t* __restrict__ tok, const float* __restrict__ x, int T, int Wd,
+                                float* __restrict__ eot) {
+  pdl_enter();
+  const int b = blockIdx.x, lane = threadIdx.x;
+  int best = INT_MIN, at = 0;
+  for (int t = lane; t < T; t += 32) {
+    const int v = tok[(size_t)b * T + t];
+    if (v > best) { best = v; at = t; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const int ob = __shfl_xor_sync(0xffffffffu, best, o), oa = __shfl_xor_sync(0xffffffffu, at, o);
+    if (ob > best || (ob == best && oa < at)) { best = ob; at = oa; }
+  }
+  const float* src = x + ((size_t)b * T + at) * Wd;
+  for (int c = lane; c < Wd; c += 32) eot[(size_t)b * Wd + c] = src[c];
+}
+
+struct ClipTextWs {
+  float* x;          // [M][W] residual stream
+  __half* h16;       // [M][W] LayerNorm output, operand of qkv / c_fc
+  float* qkv;        // [M][3W] (one layer)
+  __half* o16;       // [M][W] attention output, operand of out_proj
+  float* fc_pre;     // [M][mlp] c_fc pre-activation (one layer; written by EpiFc, not read)
+  __half* g16;       // [M][mlp] QuickGELU output, operand of c_proj
+  float* eot;        // [B][W] end-of-text rows
+  float* ynorm;      // [B][W] ln_final of those rows (written by k_head_proj)
+  size_t bytes;
+};
+
+int text_dims(const avc_clip_text_cfg* c) {
+  if (!c) return AVC_E_NULL;
+  if (c->context < 1 || c->context > kTextMaxT || c->vocab < 1 || c->out_dim < 1) return AVC_E_BADCFG;
+  if (c->heads <= 0 || c->width % c->heads || c->width / c->heads != AD || c->width > 32 * kLnMax) return AVC_E_BADCFG;
+  if (c->mlp < 64 || c->mlp % 64 || c->layers < 1 || c->layers > AVC_CLIP_MAX_LAYERS) return AVC_E_BADCFG;
+  return 0;
+}
+
+void carve_text(const avc_clip_text_cfg& c, int B, void* base, ClipTextWs* w) {
+  Carver cv(base);
+  const int64_t M = (int64_t)B * c.context, Wd = c.width;
+  w->x = cv.take<float>(M * Wd);
+  w->h16 = cv.take<__half>(M * Wd);
+  w->qkv = cv.take<float>(M * 3 * Wd);
+  w->o16 = cv.take<__half>(M * Wd);
+  w->fc_pre = cv.take<float>(M * c.mlp);
+  w->g16 = cv.take<__half>(M * c.mlp);
+  w->eot = cv.take<float>((int64_t)B * Wd);
+  w->ynorm = cv.take<float>((int64_t)B * Wd);
+  w->bytes = cv.used();
+}
+
+}  // namespace
+
+extern "C" {
+
+int avc_clip_text_workspace_bytes(const avc_clip_text_cfg* cfg, int32_t B, size_t* bytes) {
+  if (!cfg || !bytes) return AVC_E_NULL;
+  if (B < 1) return AVC_E_SIZE;
+  AVC_TRY(text_dims(cfg));
+  ClipTextWs w;
+  carve_text(*cfg, B, nullptr, &w);
+  *bytes = w.bytes;
+  return 0;
+}
+
+int avc_clip_encode_text(const avc_clip_text_cfg* cfg, const avc_clip_text_weights* wt, const int32_t* tokens, int32_t B,
+                         float* emb_out, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!cfg || !wt || !tokens || !emb_out || !workspace) return AVC_E_NULL;
+  if (B < 1) return AVC_E_SIZE;
+  AVC_TRY(text_dims(cfg));
+  if (((uintptr_t)workspace & 15u)) return AVC_E_ALIGN;
+  ClipTextWs w;
+  carve_text(*cfg, B, workspace, &w);
+  if (w.bytes > workspace_bytes) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Wd = cfg->width, T = cfg->context, M = B * T, mlp = cfg->mlp;
+  AVC_CUDA_TRY(cudaFuncSetAttribute(k_causal_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, kTextAttnSmem));
+
+  AVC_CUDA_TRY(launch_pdl(k_text_embed, dim3(ceil_div((int64_t)M * Wd, 256)), dim3(256), 0, st, tokens, wt->token_emb, wt->pos, B, T, Wd,
+                          cfg->vocab, w.x));
+  AVC_LAUNCH_TRY();
+  for (int l = 0; l < cfg->layers; ++l) {
+    const avc_clip_layer_weights& lw = wt->layer[l];
+    AVC_CUDA_TRY(launch_pdl(k_layernorm, dim3(ceil_div(M, 8)), dim3(256), 0, st, w.x, M, Wd, lw.ln1_g, lw.ln1_b, nullptr, w.h16, nullptr));
+    AVC_LAUNCH_TRY();
+    { EpiBiasStore e{w.qkv, 3 * Wd, lw.b_qkv};
+      AVC_TRY(gemm16(st, w.h16, Wd, (const __half*)lw.w_qkv, Wd, M, 3 * Wd, Wd, 1, e)); }
+    AVC_CUDA_TRY(launch_pdl(k_causal_attention, dim3(B * cfg->heads), dim3(kTextAttnThreads), kTextAttnSmem, st, w.qkv, T, Wd, cfg->heads,
+                            w.o16));
+    AVC_LAUNCH_TRY();
+    { EpiResidual e{w.x, Wd, lw.b_out};
+      AVC_TRY(gemm16(st, w.o16, Wd, (const __half*)lw.w_out, Wd, M, Wd, Wd, 2, e)); }
+    AVC_CUDA_TRY(launch_pdl(k_layernorm, dim3(ceil_div(M, 8)), dim3(256), 0, st, w.x, M, Wd, lw.ln2_g, lw.ln2_b, nullptr, w.h16, nullptr));
+    AVC_LAUNCH_TRY();
+    { EpiFc e{w.fc_pre, w.g16, mlp, lw.b_fc};
+      AVC_TRY(gemm16(st, w.h16, Wd, (const __half*)lw.w_fc, Wd, M, mlp, Wd, 1, e)); }
+    { EpiResidual e{w.x, Wd, lw.b_proj};
+      AVC_TRY(gemm16(st, w.g16, mlp, (const __half*)lw.w_proj, mlp, M, Wd, mlp, 4, e)); }
+  }
+  AVC_CUDA_TRY(launch_pdl(k_text_eot_rows, dim3(B), dim3(32), 0, st, tokens, w.x, T, Wd, w.eot));
+  // ln_final(eot) @ text_projection: the image tower's head with one token per sequence
+  AVC_CUDA_TRY(launch_pdl(k_head_proj, dim3(B, ceil_div(cfg->out_dim, 64)), dim3(256), (Wd + 256) * sizeof(float), st, w.eot, 1, Wd,
+                          wt->ln_final_g, wt->ln_final_b, wt->proj, cfg->out_dim, emb_out, w.ynorm));
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+}  // extern "C"

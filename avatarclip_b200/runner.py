@@ -10,8 +10,9 @@ checkpoint file layout (``sdf_network_fine`` / ``variance_network_fine`` / ``col
   + BCE) through the differentiable ``NeuSRenderer.render`` seam and ``torch.optim.Adam``, as the reference.
 * ``validate_image`` / ``validate_mesh`` / ``render_geometry_cast_light`` (main.py:634-919).
 
-Not importable here and therefore injected: ``clip`` (pass the ViT-B/32 visual state dict + encoded prompts to
-``init_clip``), ``smplx`` (pass template vertices / faces, or the SMPL tensors, to ``init_smpl``).
+Without the ``clip`` package, ``init_clip`` encodes the conf's prompts itself from openai's ``ViT-B-32.pt`` and BPE
+merges file (``clip_tokenizer`` / ``clip_text``).  Not importable here and therefore injected: ``smplx`` (pass template
+vertices / faces, or the SMPL tensors, to ``init_smpl``).
 """
 from __future__ import annotations
 
@@ -30,6 +31,14 @@ from .dataset import SMPL_Dataset
 from .fields import RenderingNetwork, SDFNetwork, SingleVarianceNetwork
 from .renderer import NeuSRenderer
 from .sampling import StepSampler, lookat, sphere_coord
+
+
+def _clip_importable() -> bool:
+    try:
+        import clip  # noqa: F401 (optional dependency)
+    except ImportError:
+        return False
+    return True
 
 
 def to8b(x):
@@ -170,10 +179,19 @@ class Runner:
             return _NullWriter()
 
     # ------------------------------------------------------------------ CLIP / SMPL seams
-    def init_clip(self, visual_state_dict=None, encoded_text=None, encoded_face_text=None, encoded_back_text=None):
-        """main.py:258-288.  With the ``clip`` package importable this does what the reference does; otherwise pass the
-        ViT-B/32 visual state dict and the encoded prompt [1,512] (+ face / back prompts when the conf enables them)."""
+    def init_clip(self, visual_state_dict=None, encoded_text=None, encoded_face_text=None, encoded_back_text=None,
+                  clip_model_path=None, bpe_path=None):
+        """main.py:258-288.  Either pass the ViT-B/32 visual state dict and the encoded prompt [1,512] (+ face / back
+        prompts when the conf enables them), or let init_clip encode the conf's prompts itself:
+
+        * with ``clip_model_path`` given, or without the ``clip`` package: on the GPU from openai's ``ViT-B-32.pt``
+          (``clip_model_path``, else ``$AVC_CLIP_MODEL``, else ``~/.cache/clip/ViT-B-32.pt`` where ``clip.load`` saves
+          it) and the BPE merges ``bpe_simple_vocab_16e6.txt.gz`` (``bpe_path``, else next to the model file);
+        * otherwise through the ``clip`` package, as the reference does."""
         from .clip_vit import ClipImageTower
+        if visual_state_dict is None and (clip_model_path is not None or not _clip_importable()):
+            visual_state_dict, encoded_text, encoded_face_text, encoded_back_text = \
+                self._encode_prompts(clip_model_path, bpe_path)
         if visual_state_dict is None:
             import clip                                                   # noqa: F401 (optional dependency)
             model, _ = clip.load("ViT-B/32", jit=False)
@@ -193,6 +211,32 @@ class Runner:
         prep = lambda t: None if t is None else t.detach().float().reshape(1, -1).to(self.device)
         self.encoded_text, self.encoded_face_text, self.encoded_back_text = \
             prep(encoded_text), prep(encoded_face_text), prep(encoded_back_text)
+
+    def _encode_prompts(self, clip_model_path=None, bpe_path=None):
+        """The ``clip``-free half of init_clip: read ViT-B-32.pt, tokenize the prompt (+ face / back prompts) and encode
+        them in one batch on the GPU.  Returns (visual state dict, prompt, face prompt, back prompt) with [1,512]
+        embeddings (None for a prompt the conf does not use).  The text tower is dropped afterwards."""
+        from .clip_text import ClipTextTower, load_clip_model
+        from .clip_tokenizer import ClipTokenizer
+        model_path = clip_model_path or os.environ.get("AVC_CLIP_MODEL") or \
+            os.path.join(os.path.expanduser("~"), ".cache", "clip", "ViT-B-32.pt")
+        if not os.path.isfile(model_path):
+            raise FileNotFoundError(f"init_clip: the CLIP ViT-B/32 model file {model_path} does not exist (pass "
+                                    "clip_model_path or set AVC_CLIP_MODEL to openai's ViT-B-32.pt)")
+        bpe_path = bpe_path or os.path.join(os.path.dirname(model_path), "bpe_simple_vocab_16e6.txt.gz")
+        if not os.path.isfile(bpe_path):
+            raise FileNotFoundError(f"init_clip: the CLIP BPE merges file {bpe_path} does not exist (pass bpe_path; "
+                                    "openai ships bpe_simple_vocab_16e6.txt.gz inside the clip package)")
+        keys = ["clip.prompt"] + ["clip.face_prompt"] * self.use_face_prompt + ["clip.back_prompt"] * self.use_back_prompt
+        prompts = [self.conf.get_string(k) for k in keys]
+        for k, text in zip(keys, prompts):
+            logging.info("%s: %s", k, text)
+        visual, text_sd = load_clip_model(model_path)
+        tower = ClipTextTower(text_sd, device=self.device)
+        tokens = ClipTokenizer(bpe_path).tokenize(prompts, context_length=tower.context)
+        emb = dict(zip(keys, tower.encode_text(tokens).split(1)))
+        del tower, text_sd
+        return visual, emb["clip.prompt"], emb.get("clip.face_prompt"), emb.get("clip.back_prompt")
 
     def init_smpl(self, v=None, f=None, smpl=None, v_shaped=None, pose=None):
         """main.py:290-335: the posed template ``self.v`` [1,V,3] / ``self.f`` [F,3] the silhouette rasteriser draws.

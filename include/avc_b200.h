@@ -219,6 +219,41 @@ int avc_clip_loss_bwd(const avc_clip_cfg* cfg, const avc_clip_weights* w, int32_
                       float* d_canvases, void* workspace, size_t workspace_bytes, avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * CLIP ViT-B/32 text tower (openai/CLIP `CLIP.encode_text`, the prompt embeddings of main.py:276,282,288; the
+ * weights are the non-`visual.*` half of ViT-B-32.pt).  Forward only: the weights are frozen and the reference
+ * detaches the embedding.  token_embedding + positional_embedding, `layers` pre-LN residual blocks with causal
+ * self-attention (scale 1/sqrt(64), fp32 softmax) and QuickGELU MLP, ln_final on the row of each sequence's first
+ * maximal token id (<|endoftext|>), @ text_projection.  Same precision scheme as the image tower: fp16 GEMM operands,
+ * fp32 accumulation, residual stream, LayerNorm and softmax.  Supported: width / heads == 64, width <= 1024,
+ * context <= 128, mlp % 64 == 0, 1 <= layers <= AVC_CLIP_MAX_LAYERS; anything else is AVC_E_BADCFG.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct avc_clip_text_cfg {
+  int32_t context;    /* 77    */
+  int32_t vocab;      /* 49408 */
+  int32_t width;      /* 512   */
+  int32_t layers;     /* 12    */
+  int32_t heads;      /* 8     */
+  int32_t mlp;        /* 2048  */
+  int32_t out_dim;    /* 512   */
+} avc_clip_text_cfg;
+
+typedef struct avc_clip_text_weights {
+  const float* token_emb;          /* [vocab, W]  token_embedding.weight (fp16 values stored as fp32) */
+  const float* pos;                /* [context, W] positional_embedding (fp16 values stored as fp32) */
+  const float *ln_final_g, *ln_final_b;
+  const float* proj;               /* fp32 [W, out_dim] text_projection */
+  /* transformer.resblocks.{i}.*: the forward reads w_qkv / w_out / w_fc / w_proj, the biases and the LayerNorms;
+   * the transposed copies (*_t) are unused and may be NULL */
+  avc_clip_layer_weights layer[AVC_CLIP_MAX_LAYERS];
+} avc_clip_text_weights;
+
+int avc_clip_text_workspace_bytes(const avc_clip_text_cfg* cfg, int32_t B, size_t* bytes);
+/* tokens: DEVICE int32 [B][context] (clip.tokenize); ids must lie in [0, vocab) -- an id outside is clamped, never read
+ * out of bounds.  emb_out[B][out_dim] = encode_text(tokens). */
+int avc_clip_encode_text(const avc_clip_text_cfg* cfg, const avc_clip_text_weights* w, const int32_t* tokens, int32_t B,
+                         float* emb_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Shading + canvas scatter + non-CLIP losses of Runner.train_clip (main.py:417-497, 528-534) with
  * use_silhouettes = True (every shipped train_clip conf).  The two switches the shipped confs vary
  * (the 18 confs/ablation files ending in _0 / _1 / _2) are the last two fields: zero-initialised = add_no_texture = texture_cast_light =
