@@ -346,6 +346,51 @@ int avc_lbs_fwd(const float* v_shaped, const float* pose, int32_t pose2rot, cons
                 size_t workspace_bytes, avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Mesh animation: AvatarGen/AppearanceGen/drive.py (generate_animation :308-361), the step after validate_mesh that
+ * rigs the exported mesh with SMPL skin weights and skins it through a motion.  Indices are int32, points fp32.
+ *
+ * avc_nearest_vertex replaces find_nearest_ind (drive.py:235-240): nearest[i] = argmin_j ((ref[j] - query[i])**2).sum()
+ * in fp64 -- each operand promoted exactly, the sum taken as (dx*dx + dy*dy) + dz*dz without fused multiply-adds, as
+ * numpy does -- ties to the smallest j.  query [N][3], ref [M][3], nearest [N].
+ * ------------------------------------------------------------------------------------------ */
+int avc_nearest_vertex(const float* query, int32_t N, const float* ref, int32_t M, int32_t* nearest,
+                       avc_stream_t stream);
+
+/* Replaces the island search of cleanup_mesh (drive.py:172-203; the removal :204-209 is the caller's gather).
+ * Components of the graph whose edges are the triangle edges; a vertex in no triangle is a component of its own.
+ * faces [F][3] (F may be 0; a triangle with an index outside [0, V) is ignored).  labels [V]: the smallest vertex
+ * index of each vertex's component.  kept [2] (DEVICE): {label, size} of the largest component; among equal sizes the
+ * one with the smallest label, i.e. the first the reference's scan in vertex order finds.  Nothing is read back to the
+ * host.  Workspace: avc_mesh_components_workspace_bytes(V). */
+int avc_mesh_components_workspace_bytes(int32_t V, size_t* bytes);
+int avc_mesh_components(const int32_t* faces, int32_t F, int32_t V, int32_t* labels, int32_t* kept, void* workspace,
+                        size_t workspace_bytes, avc_stream_t stream);
+
+/* The joint transforms of inv_lbs / lbs (drive.py:243-245, 256-258) with beta = 0, for n_frames poses at once:
+ * joints_out [n_joints][3] = J_regressor . v_template (vertices2joints, :51-68); A_out [n_frames][n_joints][3][4] =
+ * the top three rows of batch_rigid_transform's rel_transforms (:93-148; the bottom row is [0 0 0 1]).  pose:
+ * [n_frames][n_joints][3] axis-angle when pose2rot != 0 (batch_rodrigues, :13-49), else [n_frames][n_joints][3][3]
+ * rotation matrices.  v_template [V][3], J_regressor [n_joints][V], parents [n_joints] (parents[0] = -1, a parent
+ * before its child).  1 <= n_joints <= 32. */
+int avc_lbs_rel_transforms(const float* v_template, const float* J_regressor, const int32_t* parents, int32_t V,
+                           int32_t n_joints, const float* pose, int32_t pose2rot, int32_t n_frames, float* joints_out,
+                           float* A_out, avc_stream_t stream);
+
+/* inv_lbs (drive.py:242-253): per vertex T = sum_j W[v][j] A_j as a 4x4 whose bottom row is [0 0 0 s], s = sum_j
+ * W[v][j]; tpose_out[v] = rows 0-2 of T^-1 . [verts[v]; 1] = M^-1 (p - t / s) for T's top block [M | t], in fp64.
+ * W[v] = lbs_weights[nearest[v]] (the gather of drive.py:338-339), or lbs_weights[v] when nearest is NULL (then
+ * M >= N).  verts [N][3], lbs_weights [M][n_joints], A [n_joints][3][4] (one frame of avc_lbs_rel_transforms). */
+int avc_inv_lbs(const float* verts, const int32_t* nearest, int32_t N, const float* lbs_weights, int32_t M,
+                int32_t n_joints, const float* A, float* tpose_out, avc_stream_t stream);
+
+/* lbs (drive.py:255-265, no pose blend shapes) over frames [frame_begin, frame_begin + frame_count) of A
+ * [n_frames][n_joints][3][4]: out[f - frame_begin][v] = (sum_j W[v][j] A[f]_j) . [tpose[v]; 1], i.e. the float32
+ * payload of write_pc2 (:295-305) for those frames.  W as in avc_inv_lbs. */
+int avc_lbs_frames(const float* tpose, const int32_t* nearest, int32_t N, const float* lbs_weights, int32_t M,
+                   int32_t n_joints, const float* A, int32_t n_frames, int32_t frame_begin, int32_t frame_count,
+                   float* out, avc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self-test of the wgmma GEMM tiles (engine 1): C[M][N] = A[M][K] . B[N][K]^T, fp32 in/out, operands
  * split into bf16 (hi, lo) pairs; nprod = 1 (hi*hi only) or 3 (hi*hi + hi*lo + lo*hi).
  * workspace >= 4 * (M + N) * round_up(K, 8) + 1024 bytes.
