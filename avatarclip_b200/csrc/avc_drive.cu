@@ -1,7 +1,8 @@
 // avc_drive.cu -- the animation step after the exported mesh: AvatarGen/AppearanceGen/drive.py's cleanup_mesh (:172-210),
 // find_nearest_ind (:235-240), inv_lbs (:242-253) and lbs (:255-265) over a motion sequence.
-//   k_nearest_vertex    exact fp64 argmin of the squared distance to a reference point set; reference points staged
-//                       through shared memory in tiles, NN_QPT query points per thread held in registers
+//   k_nearest_vertex    exact argmin of the squared distance to a reference point set, in fp64 (drive.py) or fp32
+//                       (Avatar2FBX's find_nearest_ind); reference points staged through shared memory in tiles,
+//                       NN_QPT query points per thread held in registers
 //   k_cc_*              connected components of the triangle-edge graph: lock-free union-find (hook the larger root
 //                       under the smaller by CAS, path halving), flatten + atomicAdd sizes, one 64-bit atomicMax picks
 //                       the largest component (ties: smallest minimum vertex index, the reference's discovery order)
@@ -20,36 +21,55 @@ constexpr int NJ_MAX = 32;
 // ---------------------------------------------------------------- nearest vertex (drive.py:235-240)
 constexpr int NN_THREADS = 128, NN_QPT = 4, NN_TILE = 256;
 
+// The distance arithmetic of numpy's ((tv - v) ** 2).sum(-1) in the precision T of its operands: every op rounded on
+// its own (no contraction into FMAs).  double: drive.py (float32 template minus float64 points); float: Avatar2FBX's
+// ply_utils.py:84-89 (both operands float32).
+template <typename T> struct NnOps;
+template <> struct NnOps<double> {
+  static __device__ __forceinline__ double inf() { return __longlong_as_double(0x7ff0000000000000ll); }
+  static __device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
+  static __device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
+  static __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
+};
+template <> struct NnOps<float> {
+  static __device__ __forceinline__ float inf() { return __int_as_float(0x7f800000); }
+  static __device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b); }
+  static __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
+  static __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
+};
+
+template <typename T>
 __global__ void __launch_bounds__(NN_THREADS)
 k_nearest_vertex(const float* __restrict__ query, int N, const float* __restrict__ ref, int M,
                  int32_t* __restrict__ nearest) {
-  __shared__ double sR[NN_TILE * 3];
-  double qx[NN_QPT], qy[NN_QPT], qz[NN_QPT], best[NN_QPT];
+  using O = NnOps<T>;
+  __shared__ T sR[NN_TILE * 3];
+  T qx[NN_QPT], qy[NN_QPT], qz[NN_QPT], best[NN_QPT];
   int bi[NN_QPT];
   const int base = blockIdx.x * (NN_THREADS * NN_QPT) + threadIdx.x;
 #pragma unroll
   for (int k = 0; k < NN_QPT; ++k) {
     const int i = base + k * NN_THREADS;
     const bool ok = i < N;
-    qx[k] = ok ? (double)query[(size_t)i * 3 + 0] : 0.0;
-    qy[k] = ok ? (double)query[(size_t)i * 3 + 1] : 0.0;
-    qz[k] = ok ? (double)query[(size_t)i * 3 + 2] : 0.0;
-    best[k] = __longlong_as_double(0x7ff0000000000000ll);   // +inf
+    qx[k] = ok ? (T)query[(size_t)i * 3 + 0] : (T)0;
+    qy[k] = ok ? (T)query[(size_t)i * 3 + 1] : (T)0;
+    qz[k] = ok ? (T)query[(size_t)i * 3 + 2] : (T)0;
+    best[k] = O::inf();
     bi[k] = 0;
   }
   for (int t0 = 0; t0 < M; t0 += NN_TILE) {
     const int n = min(NN_TILE, M - t0);
     __syncthreads();
-    for (int i = threadIdx.x; i < n * 3; i += NN_THREADS) sR[i] = (double)ref[(size_t)t0 * 3 + i];
+    for (int i = threadIdx.x; i < n * 3; i += NN_THREADS) sR[i] = (T)ref[(size_t)t0 * 3 + i];
     __syncthreads();
 #pragma unroll 2
     for (int j = 0; j < n; ++j) {
-      const double rx = sR[j * 3], ry = sR[j * 3 + 1], rz = sR[j * 3 + 2];
+      const T rx = sR[j * 3], ry = sR[j * 3 + 1], rz = sR[j * 3 + 2];
 #pragma unroll
       for (int k = 0; k < NN_QPT; ++k) {
-        // numpy: ((tv - v) ** 2).sum(-1) in float64 = (dx*dx + dy*dy) + dz*dz, each op rounded (no FMA)
-        const double dx = __dsub_rn(rx, qx[k]), dy = __dsub_rn(ry, qy[k]), dz = __dsub_rn(rz, qz[k]);
-        const double d = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+        // numpy: ((tv - v) ** 2).sum(-1) = (dx*dx + dy*dy) + dz*dz, each op rounded (no FMA)
+        const T dx = O::sub(rx, qx[k]), dy = O::sub(ry, qy[k]), dz = O::sub(rz, qz[k]);
+        const T d = O::add(O::add(O::mul(dx, dx), O::mul(dy, dy)), O::mul(dz, dz));
         if (d < best[k]) { best[k] = d; bi[k] = t0 + j; }      // strict <, increasing index: ties keep the first
       }
     }
@@ -102,10 +122,18 @@ __global__ void k_cc_hook(const int32_t* __restrict__ faces, int F, int V, int* 
   cc_union(labels, b, c);
 }
 
+// No path halving here: a halving write parent[prev] = next could land after prev's own thread stored its root, leaving
+// prev labelled with an inner node of its tree.  Every write of this pass stores a root, so the walk always ends there.
+__device__ __forceinline__ int cc_find(const volatile int* parent, int v) {
+  int cur = v, next;
+  while ((next = parent[cur]) != cur) cur = next;
+  return cur;
+}
+
 __global__ void k_cc_flatten(int V, int* labels, int* __restrict__ sizes) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= V) return;
-  const int r = cc_root(labels, v);
+  const int r = cc_find(labels, v);
   labels[v] = r;
   atomicAdd(sizes + r, 1);
 }
@@ -310,7 +338,18 @@ extern "C" {
 int avc_nearest_vertex(const float* query, int32_t N, const float* ref, int32_t M, int32_t* nearest, avc_stream_t stream) {
   if (!query || !ref || !nearest) return AVC_E_NULL;
   if (N < 1 || M < 1) return AVC_E_SIZE;
-  k_nearest_vertex<<<blocks(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M, nearest);
+  k_nearest_vertex<double><<<blocks(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M,
+                                                                                                     nearest);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_nearest_vertex_f32(const float* query, int32_t N, const float* ref, int32_t M, int32_t* nearest,
+                           avc_stream_t stream) {
+  if (!query || !ref || !nearest) return AVC_E_NULL;
+  if (N < 1 || M < 1) return AVC_E_SIZE;
+  k_nearest_vertex<float><<<blocks(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M,
+                                                                                                    nearest);
   AVC_LAUNCH_TRY();
   return 0;
 }

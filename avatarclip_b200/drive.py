@@ -219,8 +219,9 @@ def find_nearest_ind(new_vertices, template_object) -> torch.Tensor:
     return _nearest(_f32(new_vertices, device).reshape(-1, 3), _f32(tv, device).reshape(-1, 3)).long()
 
 
-def _rel_transforms(s: dict, pose: torch.Tensor, pose2rot: bool) -> torch.Tensor:
-    """A [frames, nj, 12] for beta = 0 (drive.py:243-245)."""
+def _rel_transforms(s: dict, pose: torch.Tensor, pose2rot: bool, return_joints: bool = False):
+    """A [frames, nj, 12] for beta = 0 (drive.py:243-245); with ``return_joints``, (A, J [nj, 3] = J_regressor .
+    v_template)."""
     nj, V = s["J_regressor"].shape
     frames = pose.shape[0]
     A = torch.empty(frames, nj, 12, dtype=torch.float32, device=pose.device)
@@ -228,7 +229,7 @@ def _rel_transforms(s: dict, pose: torch.Tensor, pose2rot: bool) -> torch.Tensor
     _lib.check(_L().avc_lbs_rel_transforms(_lib.ptr(s["v_template"]), _lib.ptr(s["J_regressor"]), _lib.ptr(s["parents"]),
                                            V, nj, _lib.ptr(pose), 1 if pose2rot else 0, frames, _lib.ptr(joints),
                                            _lib.ptr(A), _lib.stream_ptr()), "avc_lbs_rel_transforms")
-    return A
+    return (A, joints) if return_joints else A
 
 
 def _zero_beta(beta):

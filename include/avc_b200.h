@@ -391,6 +391,43 @@ int avc_lbs_frames(const float* tpose, const int32_t* nearest, int32_t N, const 
                    float* out, avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Avatar export: Avatar2FBX/export_fbx.py (:44-118), which rigs the exported mesh to SMPL's skeleton.
+ *
+ * avc_nearest_vertex_f32 is Avatar2FBX's find_nearest_ind (utils/ply_utils.py:84-89), where both operands are float32:
+ * nearest[i] = argmin_j of the float32 (dx*dx + dy*dy) + dz*dz, d = ref[j] - query[i], every operation rounded on its
+ * own (no fused multiply-adds), ties to the smallest j.  Near-equidistant reference points may give another index than
+ * avc_nearest_vertex's fp64 distance.  Shapes and errors as avc_nearest_vertex.
+ * ------------------------------------------------------------------------------------------ */
+int avc_nearest_vertex_f32(const float* query, int32_t N, const float* ref, int32_t M, int32_t* nearest,
+                           avc_stream_t stream);
+
+/* open3d's TriangleMesh::simplify_vertex_clustering(voxel, SimplificationContraction.Average) with Avatar2FBX's voxel
+ * (utils/ply_utils.py:16-19): voxel = max over axes of (max - min) / resolution (resolution 256 there).
+ *   - Voxel of a vertex: idx = floor((v - (min - voxel / 2)) / voxel) per axis, in fp64 with each operation rounded on
+ *     its own, so a vertex exactly on a voxel boundary lands where numpy / Eigen put it.  If every vertex is the same
+ *     point (voxel 0) they share one voxel.
+ *   - Output vertex k is the k-th distinct voxel in order of its first vertex, scanning the input in index order.
+ *     Vertices in no triangle are clustered too.
+ *   - Its position is the fp64 mean of the voxel's positions, rounded to float32; its colour (when colors is not NULL)
+ *     the fp64 mean of c / 255, rounded to float32.  The sums are taken by atomics in no fixed order.  They are exact,
+ *     so the means do not depend on that order, whenever the sum of a voxel's coordinates fits in 53 bits: its values
+ *     lie on one power-of-two grid no finer than about 2^-29 of their magnitude (true of the avatar meshes measured; a
+ *     coordinate of 1e-16 beside one of 1e-2 is not, and such a voxel may change in its last bit between runs).
+ *     Colours are summed as integers and may differ from a sequential fp64 mean of c / 255 by one float32 ulp.
+ *   - Triangles are remapped in input order.  A triangle with two corners in one voxel is dropped, and so is one that
+ *     is a rotation (a,b,c), (b,c,a) or (c,a,b) of an earlier kept triangle; a reversed triangle (a,c,b) is kept.  A
+ *     kept triangle keeps the rotation it first appeared in.  A triangle with an index outside [0, V) is dropped.
+ * verts [V][3], colors [V][3] uint8 or NULL, tris [F][3] (F may be 0).  Outputs sized by the inputs: verts_out [V][3],
+ * colors_out [V][3] (required when colors is given), tris_out [F][3].  counts [2] (DEVICE): {output vertices, output
+ * triangles}; the rows beyond them are left unwritten.  Nothing is read back to the host.  1 <= resolution <=
+ * 2^21 - 2 (the voxel key packs 21 bits per axis), else AVC_E_BADCFG.  1 <= V <= 2^30, 0 <= F <= 2^30.
+ * Workspace: avc_mesh_cluster_workspace_bytes(V, F). */
+int avc_mesh_cluster_workspace_bytes(int32_t V, int32_t F, size_t* bytes);
+int avc_mesh_cluster(const float* verts, const uint8_t* colors, int32_t V, const int32_t* tris, int32_t F,
+                     int32_t resolution, float* verts_out, float* colors_out, int32_t* tris_out, int32_t* counts,
+                     void* workspace, size_t workspace_bytes, avc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self-test of the wgmma GEMM tiles (engine 1): C[M][N] = A[M][K] . B[N][K]^T, fp32 in/out, operands
  * split into bf16 (hi, lo) pairs; nprod = 1 (hi*hi only) or 3 (hi*hi + hi*lo + lo*hi).
  * workspace >= 4 * (M + N) * round_up(K, 8) + 1024 bytes.
