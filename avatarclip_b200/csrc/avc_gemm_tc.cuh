@@ -58,9 +58,11 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 // CTAs of every launch, per epilogue functor (Epi::kProbeId), in the slots
 //   0 producer waits for a free stage   1 producer loop          2 consumers wait for operands   3 consumers wait for turn
 //   4 consumers' MMAs (turn to done)    5 consumers' epilogues   6 consumers' loops              7 CTAs
+//   8 consumers wait for staged epilogue operands
 // (the consumer slots add up both consumer warpgroups).  AVC_PROBE(...) code only exists in the probe build.
+constexpr int kNtProbeSlots = 9;
 #ifdef AVC_NT_PROBE
-static __device__ unsigned long long g_nt_probe[16][8];
+static __device__ unsigned long long g_nt_probe[16][kNtProbeSlots];
 #define AVC_PROBE(...) __VA_ARGS__
 #define AVC_PROBE_WAIT(acc, bar, par) do { long long t__ = clock64(); mbar_wait(bar, par); (acc) += clock64() - t__; } while (0)
 #define AVC_PROBE_ADD(id, slot, v) atomicAdd(&g_nt_probe[id][slot], (unsigned long long)(v))
@@ -162,6 +164,37 @@ static inline int make_map_bf16(CUtensorMap* m, const void* base, uint64_t rows,
   return r == CUDA_SUCCESS ? 0 : AVC_E_BADCFG;
 }
 
+// 2-D fp32 (es = 4) or bf16 (es = 2) tensor [rows][cols], row pitch ld elements, box = box_cols x box_rows; the swizzle
+// spans one box row (box_cols * es = 32, 64 or 128 bytes).  Columns >= cols and rows >= rows of a box read as zero.
+// Cached like make_map_bf16_cached.
+static inline int make_map_rows_cached(CUtensorMap* m, int es, const void* base, uint64_t rows, uint64_t cols,
+                                       uint64_t ld, uint32_t box_cols, uint32_t box_rows) {
+  static thread_local MapCacheEntry cache[64];
+  const uint64_t h = ((uintptr_t)base >> 8) * 0x9E3779B97F4A7C15ull ^ (rows * 31 + cols * 131 + ld * 7 + box_cols + 3 * box_rows + es);
+  MapCacheEntry& e = cache[(h >> 32) & 63];
+  const uint32_t bc = box_cols | ((uint32_t)es << 16);      // the element size is part of the key
+  if (e.base == base && e.rows == rows && e.cols == cols && e.ld == ld && e.bc == bc && e.br == box_rows) {
+    *m = e.map;
+    return 0;
+  }
+  PFN_encodeTiled fn = get_encode_fn();
+  if (!fn) return AVC_E_BADCFG;
+  if (((uintptr_t)base & 15u) || (ld * es) % 16) return AVC_E_ALIGN;
+  const uint32_t span = box_cols * es;
+  const CUtensorMapSwizzle sw = span == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : span == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                                                     : CU_TENSOR_MAP_SWIZZLE_32B;
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {ld * es};
+  cuuint32_t box[2] = {box_cols, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(m, es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base),
+                  dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return AVC_E_BADCFG;
+  e.base = base; e.rows = rows; e.cols = cols; e.ld = ld; e.bc = bc; e.br = box_rows; e.map = *m;
+  return 0;
+}
+
 struct SplitPtr {            // two-term bf16 split of an fp32 matrix, both [rows][ld]
   const __nv_bfloat16* hi;
   const __nv_bfloat16* lo;
@@ -182,17 +215,28 @@ constexpr int kNtTurnBar = 1;     // named barrier kNtTurnBar + c: consumer warp
 // RESB: the CTA keeps its whole B panel (BN rows x up to kResK k-blocks, hi and lo) resident in shared memory and only
 // streams A: re-fetched for every row tile, the B panel would multiply the L2 -> SM operand traffic of a tile.
 constexpr int kResK = 4;          // k-blocks (of 64) a resident panel holds: K <= 256
-template <int BN, int NPROD, bool RESB = false>
+// Functors with staged epilogue operands (EpiStage below) give the A ring kEpiAStages stages and the rest of the shared
+// memory to the epilogue rings, at most kEpiSlotsMax slots per consumer warpgroup.
+constexpr int kEpiAStages = 3, kEpiSlotsMax = 8;
+// EPI_SLOT: bytes of one epilogue ring slot (0: the functor stages nothing, no rings)
+template <int BN, int NPROD, bool RESB = false, int EPI_SLOT = 0>
 struct TcCfg {
   static constexpr int A_BYTES = kNtBM * kBK * 2;                  // one (hi or lo) A slab: 8 KB
   static constexpr int B_BYTES = BN * kBK * 2;
   static constexpr int NOP = (NPROD == 3) ? 2 : 1;                 // slabs per operand (hi, lo)
   static constexpr int BRES_BYTES = RESB ? kResK * NOP * B_BYTES : 0;
   static constexpr int STAGE_BYTES = RESB ? NOP * A_BYTES : NOP * (A_BYTES + B_BYTES);
-  static constexpr int kBudget = kSmemMax - 1024 /*align*/ - 256 /*barriers*/ - BRES_BYTES;
-  static constexpr int STAGES = kBudget / STAGE_BYTES >= 8 ? 8 : kBudget / STAGE_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BRES_BYTES + 1024 + 256;
+  static constexpr int BAR_BYTES = EPI_SLOT ? 512 : 256;
+  static constexpr int kBudget = kSmemMax - 1024 /*align*/ - BAR_BYTES - BRES_BYTES;
+  static constexpr int STAGES = EPI_SLOT ? kEpiAStages : kBudget / STAGE_BYTES >= 8 ? 8 : kBudget / STAGE_BYTES;
+  static constexpr int kEpiFit = EPI_SLOT ? (kBudget - STAGES * STAGE_BYTES) / (2 * EPI_SLOT) : 0;
+  static constexpr int EPI_SLOTS = kEpiFit > kEpiSlotsMax ? kEpiSlotsMax : kEpiFit;      // per consumer warpgroup
+  static constexpr int SLOT_BYTES = EPI_SLOT;
+  static constexpr int EPI_BYTES = 2 * EPI_SLOTS * EPI_SLOT;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BRES_BYTES + EPI_BYTES + 1024 + BAR_BYTES;
   static_assert(STAGES >= 2, "tile too large for shared memory");
+  static_assert(!EPI_SLOT || EPI_SLOTS >= 2, "no room for two epilogue slots per consumer");
+  static_assert(8 * (2 * STAGES + kResK + 4 * EPI_SLOTS) <= BAR_BYTES, "mbarriers overflow their area");
   static_assert(SMEM_BYTES <= kSmemMax, "exceeds the 227 KB of shared memory per CTA");
 };
 
@@ -211,6 +255,57 @@ struct EpiTraits<E, std::void_t<typename E::Aux>> {
   static __device__ __forceinline__ Aux prefetch(const E& e, int r, int c) { return e.prefetch(r, c); }
   static __device__ __forceinline__ void apply(const E& e, int r, int c, float4 a, const Aux& x) { e(r, c, a, x); }
 };
+// groups of 8 columns per epilogue batch: two batches of global operands are live beside the accumulator; with 32-byte
+// operands (EpiChainBwd, EpiDgrad) batches of 4 need more registers than ptxas grants a 384-thread kernel and spill
+template <typename E>
+struct EpiBatch {
+  static constexpr int kB = sizeof(typename EpiTraits<E>::Aux) > 16 ? 2 : 4;
+  static constexpr int kCols = 8 * kB;
+};
+
+// Staged epilogue operands.  A functor with a nested `using Stage = tc::Staged<ES0[, ES1[, ES2]]>` (element sizes in bytes:
+// 4 fp32, 2 bf16) has the per-tile global operands of its epilogue loaded by TMA into shared memory ahead of the tile:
+//   tc::StageOp stage_op(int i) const                 (host) operand i: [rows][ld] array, column extent = padded width
+//   static Aux from_stage(const uint4 (&raw)[kN])      4 consecutive elements of each operand (bf16: raw.x, raw.y) -> Aux
+// A ring slot holds one batch (EpiBatch::kCols columns x 64 rows) of every operand.  Columns past the extent and rows past
+// M read as zero (TMA out-of-bounds fill).
+template <int E0, int E1 = 0, int E2 = 0>
+struct Staged {
+  static constexpr int kN = 1 + (E1 > 0) + (E2 > 0);
+  static constexpr int kColBytes = E0 + E1 + E2;
+  __host__ __device__ static constexpr int es(int i) { return i == 0 ? E0 : i == 1 ? E1 : E2; }
+  __host__ __device__ static constexpr int before(int i) { return i == 0 ? 0 : i == 1 ? E0 : E0 + E1; }
+};
+struct StageOp { const void* base; int ld; int cols; };
+template <typename E, typename = void>
+struct EpiStage {
+  static constexpr int kN = 0, kSlotBytes = 0;
+};
+template <typename E>
+struct EpiStage<E, std::void_t<typename E::Stage>> {
+  using S = typename E::Stage;
+  static constexpr int kN = S::kN, kSlotBytes = kNtBM * EpiBatch<E>::kCols * S::kColBytes;
+};
+template <int N>
+struct EpiMaps { CUtensorMap m[N]; };
+template <>
+struct EpiMaps<0> {};
+// 4 elements at (r, c) of a [64][cols] box as TMA wrote it: rows of span = cols * ES bytes, swizzled over the span
+// (16-byte unit bits 4.. ^= address bits 7..)
+// (volatile: stays behind the slot's full-barrier wait)
+template <int ES, int COLS>
+__device__ __forceinline__ uint4 stage_read(uint32_t slab, int r, int c) {
+  constexpr int kSpan = COLS * ES;
+  static_assert(kSpan == 32 || kSpan == 64 || kSpan == 128, "swizzle span");
+  const uint32_t lin = (uint32_t)(r * kSpan + c * ES);
+  const uint32_t addr = slab + (lin ^ (((lin >> 7) & (kSpan / 16 - 1)) << 4));
+  uint4 v = make_uint4(0u, 0u, 0u, 0u);
+  if constexpr (ES == 4)
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+  else
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+  return v;
+}
 // The epilogue's own global operands (stashes written passes ago: always DRAM misses) are loaded right before use.
 // Functors with `l2_prefetch(m0, n0, bn, M, et, nth)` get the chance to pull the operand lines of the consumer
 // warpgroup's NEXT row tile into L2 a whole tile ahead (thread et of nth epilogue threads).
@@ -244,35 +339,79 @@ struct EpiL2<E, std::void_t<decltype(&E::l2_prefetch)>> {
 // The functor operands (prefetch) are loaded in batches of kB groups, one batch ahead of the arithmetic: the first batch
 // before `mma_done()` (which waits for the accumulator), every later one before the previous batch's arithmetic and
 // stores, so that a memory round trip is always in flight under other work.
-template <int BN, typename Epi, typename MmaDone>
+// Staged functors (EpiStage) read their operands from the consumer's epilogue ring instead: batch b is chunk q0 + b of the
+// ring (one slot per batch), waited for on its full barrier and released to the loader after the batch's arithmetic.
+struct EpiRing {
+  uint32_t base;               // slot 0 of this consumer's ring (shared-memory address)
+  uint32_t full0, empty0;      // mbarriers of slot 0 (8 bytes apart)
+  int q0;                      // ring chunk counter of the tile's first batch
+  int r, c;                    // this thread's row / first column inside a chunk
+};
+template <int BN, int SLOTS, typename Epi, typename MmaDone>
 __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[BN / 2], int row, int col0, int M, int N,
-                                            int lane, MmaDone&& mma_done) {
+                                            int lane, MmaDone&& mma_done, const EpiRing& ring, long long& w_stage) {
   using Tr = EpiTraits<Epi>;
   const bool odd = lane & 1;
-  // groups per batch: two batches of operands are live beside the accumulator; with 32-byte operands (EpiChainBwd,
-  // EpiDgrad) batches of 4 need more registers than ptxas grants a 384-thread kernel and spill
-  constexpr int kB = sizeof(typename Tr::Aux) > 16 ? 2 : 4, kNB = BN / 8 / kB;
-  typename Tr::Aux aux[2][kB];
-  auto load = [&](int b) {
-#pragma unroll
-    for (int u = 0; u < kB; ++u) {
-      const int col = col0 + 8 * (kB * b + u);
-      if (row < M && col < N) aux[b & 1][u] = Tr::prefetch(epi, row, col);
-    }
+  constexpr int kB = EpiBatch<Epi>::kB, kNB = BN / 8 / kB;
+  auto group = [&](int j) {      // the 4-column group j of this thread's row (one exchange with lane ^ 1)
+    const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+    const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+    return odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
   };
-  load(0);
-  mma_done();
+  if constexpr (EpiStage<Epi>::kN > 0) {
+    using St = typename Epi::Stage;
+    constexpr int kCols = EpiBatch<Epi>::kCols, kSlot = EpiStage<Epi>::kSlotBytes;
+    mma_done();
 #pragma unroll
-  for (int b = 0; b < kNB; ++b) {
-    if (b + 1 < kNB) load(b + 1);
+    for (int b = 0; b < kNB; ++b) {
+      const int q = ring.q0 + b, s = q % SLOTS;
+      AVC_PROBE_WAIT(w_stage, ring.full0 + 8 * s, (q / SLOTS) & 1);
+      const uint32_t slot = ring.base + s * kSlot;
+      typename Tr::Aux aux[kB];
 #pragma unroll
-    for (int u = 0; u < kB; ++u) {
-      const int j = kB * b + u;
-      const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
-      const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
-      const float4 v = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
-      const int col = col0 + 8 * j;
-      if (row < M && col < N) Tr::apply(epi, row, col, v, aux[b & 1][u]);
+      for (int u = 0; u < kB; ++u) {
+        uint4 raw[St::kN];
+#pragma unroll
+        for (int i = 0; i < St::kN; ++i) {
+          const uint32_t slab = slot + kNtBM * kCols * St::before(i);
+          raw[i] = St::es(i) == 4 ? stage_read<4, kCols>(slab, ring.r, ring.c + 8 * u)
+                                  : stage_read<2, kCols>(slab, ring.r, ring.c + 8 * u);
+        }
+        aux[u] = Epi::from_stage(raw);
+      }
+#pragma unroll
+      for (int u = 0; u < kB; ++u) {
+        const int j = kB * b + u;
+        const float4 v = group(j);
+        const int col = col0 + 8 * j;
+        if (row < M && col < N) Tr::apply(epi, row, col, v, aux[u]);
+      }
+      __syncwarp();
+      if ((lane & 31) == 0) mbar_arrive(ring.empty0 + 8 * s);      // one arrival per warp: the slot may be refilled
+    }
+  } else {
+    typename Tr::Aux aux[2][kB];
+    auto load = [&](int b) {
+#pragma unroll
+      for (int u = 0; u < kB; ++u) {
+        const int col = col0 + 8 * (kB * b + u);
+        if (row < M && col < N) aux[b & 1][u] = Tr::prefetch(epi, row, col);
+      }
+    };
+    load(0);
+    mma_done();
+#pragma unroll
+    for (int b = 0; b < kNB; ++b) {
+      if (b + 1 < kNB) load(b + 1);
+#pragma unroll
+      for (int u = 0; u < kB; ++u) {
+        const int j = kB * b + u;
+        const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+        const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+        const float4 v = odd ? make_float4(r0, r1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], r0, r1);
+        const int col = col0 + 8 * j;
+        if (row < M && col < N) Tr::apply(epi, row, col, v, aux[b & 1][u]);
+      }
     }
   }
 }
@@ -285,19 +424,30 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
 // its last k-block is issued, then waits for its MMAs and runs the epilogue while the other one issues: the tensor pipe
 // works under the epilogues.  Turns make the ring's consumption follow the tile order, so the k-block counter j * nk + kb
 // gives every role the stage and its parity, and each stage is released by the one warpgroup that read it.
+// Staged functors (EpiStage): threads 32 and 64 of the producer warpgroup are the epilogue operand loaders of consumer
+// warpgroups 0 and 1.  Each walks its consumer's tiles and issues, batch by batch, one chunk of every staged operand
+// (TMA, box kCols x 64) into the consumer's epilogue ring (EPI_SLOTS slots, full / empty mbarriers), so that the
+// operands of a tile land while its MMAs run.  The ring chunk counter (tile j: (j / 2) * batches + b) gives both sides the
+// slot and its parity.
 template <int BN, int NPROD, bool RESB, typename Epi>
 __global__ void __launch_bounds__(kNtThreads, 1)
 gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapBhi, const __grid_constant__ CUtensorMap mapBlo,
-                  int M, int N, int K, Epi epi, int b_const) {
-  using Cfg = TcCfg<BN, NPROD, RESB>;
+                  int M, int N, int K, Epi epi, int b_const, const __grid_constant__ EpiMaps<EpiStage<Epi>::kN> emaps) {
+  using Cfg = TcCfg<BN, NPROD, RESB, EpiStage<Epi>::kSlotBytes>;
+  constexpr int kStaged = EpiStage<Epi>::kN;
+  constexpr int kEpiCols = EpiBatch<Epi>::kCols, kEpiNB = BN / kEpiCols;      // ring chunks per tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B wants 1024-B tiles
-  constexpr int kOpBytes = Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BRES_BYTES;     // stages, then the resident B panel
+  // stages, then the resident B panel, then the two epilogue rings
+  constexpr int kOpBytes = Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BRES_BYTES + Cfg::EPI_BYTES;
   uint64_t* bars = (uint64_t*)(smem + kOpBytes);
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bres_base = smem_base + Cfg::STAGES * Cfg::STAGE_BYTES;
   const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * Cfg::STAGES, bfull = empty0 + 8 * Cfg::STAGES;
+  // epilogue ring of consumer c: slots at epi_off + c * EPI_SLOTS * EPI_SLOT, barriers efull0 / eempty0 + 8 * (c * EPI_SLOTS + s)
+  constexpr int kEpiOff = Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BRES_BYTES;
+  const uint32_t efull0 = bfull + 8 * kResK, eempty0 = efull0 + 16 * Cfg::EPI_SLOTS;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_n = (N + BN - 1) / BN;
@@ -315,12 +465,37 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
     if (NPROD == 3) { tma_prefetch_desc(&mapAlo); tma_prefetch_desc(&mapBlo); }
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
     for (int kb = 0; kb < kResK; ++kb) mbar_init(bfull + 8 * kb, 1);     // one per k-block of the resident B panel
+    if constexpr (kStaged > 0) {
+      for (int i = 0; i < kStaged; ++i) tma_prefetch_desc(&emaps.m[i]);
+      for (int s = 0; s < 2 * Cfg::EPI_SLOTS; ++s) { mbar_init(efull0 + 8 * s, 1); mbar_init(eempty0 + 8 * s, 4); }
+    }
     fence_barrier_init();
   }
   __syncthreads();      // the last CTA-wide barrier: after the role split only mbarriers and named barriers 1, 2
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if constexpr (kStaged > 0) {
+      if (threadIdx.x == 32 || threadIdx.x == 64) {      // epilogue operand loader of consumer warpgroup c
+        const int c = warp - 1;
+        pdl_wait();      // the stashes belong to predecessor kernels
+        int q = 0;
+        for (int j = c; j < n_tiles; j += 2) {
+          const int m0 = (m_first + j * m_stride) * kNtBM;
+#pragma unroll 1
+          for (int b = 0; b < kEpiNB; ++b, ++q) {      // rolled: this warpgroup runs on 40 registers
+            const int s = c * Cfg::EPI_SLOTS + q % Cfg::EPI_SLOTS;
+            mbar_wait(eempty0 + 8 * s, ((q / Cfg::EPI_SLOTS) & 1) ^ 1);
+            const uint32_t dst = smem_base + kEpiOff + s * Cfg::SLOT_BYTES;
+            mbar_expect_tx(efull0 + 8 * s, (uint32_t)Cfg::SLOT_BYTES);     // out-of-bounds fill counts as well
+#pragma unroll
+            for (int i = 0; i < kStaged; ++i)
+              tma_load_2d(dst + kNtBM * kEpiCols * Epi::Stage::before(i), &emaps.m[i], n0 + b * kEpiCols, m0, efull0 + 8 * s);
+          }
+        }
+        return;
+      }
+    }
     if (threadIdx.x == 0) {
       // b_const: B holds constants of the step (the packed weights, written many kernels ago): its resident panel is
       // loaded while the predecessor kernel may still be running
@@ -366,6 +541,9 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   const int row_in = 16 * wq + (lane >> 2) + 8 * (lane & 1), col_in = 4 * ((lane >> 1) & 1);
   pdl_wait();      // the functor's operands and outputs belong to predecessor kernels
   float acc[BN / 2];
+  long long w_stage = 0;      // (probe build) waits on the epilogue ring
+  EpiRing ring{smem_base + kEpiOff + c * Cfg::EPI_SLOTS * Cfg::SLOT_BYTES, efull0 + 8 * c * Cfg::EPI_SLOTS,
+               eempty0 + 8 * c * Cfg::EPI_SLOTS, 0, row_in, col_in};
   AVC_PROBE(long long w_full = 0, w_turn = 0, t_mma = 0, t_epi = 0; const long long t_loop0 = clock64());
   EpiL2<Epi>::run(epi, (m_first + c * m_stride) * kNtBM, n0, BN, M, tw, 128);
   for (int j = c; j < n_tiles; j += 2) {
@@ -403,7 +581,8 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
       }
     }
     if (j + 1 < n_tiles) named_bar_arrive(kNtTurnBar + (c ^ 1), 256);      // all k-blocks issued: the other's turn
-    epilogue_nt<BN>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane, [&] {
+    ring.q0 = (j >> 1) * kEpiNB;
+    epilogue_nt<BN, Cfg::EPI_SLOTS>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane, [&] {
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       if (leader) {
@@ -411,10 +590,12 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
         mbar_arrive(empty0 + 8 * last);
       }
       AVC_PROBE(t_mma += clock64() - t_mma0);
-    });
+    }, ring, w_stage);
     AVC_PROBE(t_epi += clock64() - t_mma0);
   }
+  (void)w_stage;
   AVC_PROBE(if (leader) {
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 8, w_stage);
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 2, w_full);
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 3, w_turn);
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 4, t_mma);
@@ -426,7 +607,16 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
 template <int BN, int NPROD, bool RESB, typename Epi>
 static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K, const SplitPtr& A, const SplitPtr& B,
                                        const Epi& epi, bool b_const) {
-  using Cfg = TcCfg<BN, NPROD, RESB>;
+  using Cfg = TcCfg<BN, NPROD, RESB, EpiStage<Epi>::kSlotBytes>;
+  EpiMaps<EpiStage<Epi>::kN> emaps;
+  if constexpr (EpiStage<Epi>::kN > 0) {
+    for (int i = 0; i < EpiStage<Epi>::kN; ++i) {
+      const StageOp op = epi.stage_op(i);
+      if (!op.base) return AVC_E_BADCFG;
+      AVC_TRY(make_map_rows_cached(&emaps.m[i], Epi::Stage::es(i), op.base, (uint64_t)M, (uint64_t)op.cols,
+                                   (uint64_t)op.ld, EpiBatch<Epi>::kCols, kNtBM));
+    }
+  }
   CUtensorMap mAh, mAl, mBh, mBl;
   AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
   AVC_TRY(make_map_bf16_cached(&mBh, B.hi, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
@@ -454,7 +644,7 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
   g = (g / tiles_n) * tiles_n;                         // ... and a whole number of CTAs per column tile
   if (g < tiles_n) return AVC_E_BADCFG;
   dim3 grid(g);
-  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kNtThreads), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, b_const ? 1 : 0));
+  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kNtThreads), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, b_const ? 1 : 0, emaps));
   AVC_LAUNCH_TRY();
   return 0;
 }

@@ -585,15 +585,15 @@ extern "C" {
 
 int avc_abi_version(void) { return AVC_ABI_VERSION; }
 
-// Stall probe of the wgmma NT tiles (diagnostic builds only: -DAVC_NT_PROBE=1).  out[16][8]: per functor the summed
+// Stall probe of the wgmma NT tiles (diagnostic builds only: -DAVC_NT_PROBE=1).  out[16][9]: per functor the summed
 // cycles of the slots listed in avc_gemm_tc.cuh (AVC_NT_PROBE).  Returns AVC_E_BADCFG in a regular build.
 int avc_nt_probe_read(unsigned long long* host_out, int reset) {
 #ifdef AVC_NT_PROBE
   if (!host_out) return AVC_E_NULL;
   AVC_CUDA_TRY(cudaDeviceSynchronize());
-  AVC_CUDA_TRY(cudaMemcpyFromSymbol(host_out, tc::g_nt_probe, sizeof(unsigned long long) * 16 * 8));
+  AVC_CUDA_TRY(cudaMemcpyFromSymbol(host_out, tc::g_nt_probe, sizeof(unsigned long long) * 16 * tc::kNtProbeSlots));
   if (reset) {
-    static unsigned long long zeros[16 * 8];
+    static unsigned long long zeros[16 * tc::kNtProbeSlots];
     AVC_CUDA_TRY(cudaMemcpyToSymbol(tc::g_nt_probe, zeros, sizeof(zeros)));
   }
   return 0;
@@ -603,6 +603,70 @@ int avc_nt_probe_read(unsigned long long* host_out, int reset) {
 #endif
 }
 const char* avc_build_arch(void) { return "sm_90a"; }
+
+// Self-test of the backward epilogue functors through the wgmma NT tiles (tests/test_nt_epilogue_gpu.py):
+// acc = A[M][K] . B[N][K]^T on the two-term split, then
+//   kind 0  EpiChainBwd  D1 = X, qt = split of Y (both [M][ldx]), s_next = s -> ZBAR = OUT [M][ldx], ubar = OUT2 [M][ld2]
+//   kind 1  EpiDgrad     D1prev = X, zbar_prev = Y (updated in place, fp32), s
+//   kind 2  EpiDgrad     as 1 with the sdf term: sdfbar = v1 [M], wsdf = v2 [ldx], sdf_inv_scale = s2
+//   kind 3  EpiChain     Nprev = Nv, D1prev = X, s -> qt_prev = OUT [M][ldx]; ge = OUT2 [M][ld2] += the columns >= Nv
+//   kind 4  EpiDgradRelu mask from the bf16 hi half of X -> OUT [M][ldx]
+//   kind 5  EpiGe        ge = OUT2 [M][ld2] += acc
+// workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes.
+int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
+                    const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
+                    float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!A || !B || !X || !workspace) return AVC_E_NULL;
+  if (M <= 0 || N <= 0 || K <= 0 || ldx % 8 || ld2 % 8) return AVC_E_SIZE;
+  const int ld = (int)round_up(K, 8);
+  Carver cv(workspace);
+  __nv_bfloat16* ah = cv.take<__nv_bfloat16>(M * ld);
+  __nv_bfloat16* al = cv.take<__nv_bfloat16>(M * ld);
+  __nv_bfloat16* bh = cv.take<__nv_bfloat16>((int64_t)N * ld);
+  __nv_bfloat16* bl = cv.take<__nv_bfloat16>((int64_t)N * ld);
+  __nv_bfloat16* xh = cv.take<__nv_bfloat16>(M * ldx);
+  __nv_bfloat16* xl = cv.take<__nv_bfloat16>(M * ldx);
+  if (cv.used() > workspace_bytes) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  tc::k_split_bf16<<<blocks_for(M * ld, 256), 256, 0, st>>>(A, M, K, K, ah, al, ld);
+  tc::k_split_bf16<<<blocks_for((int64_t)N * ld, 256), 256, 0, st>>>(B, N, K, K, bh, bl, ld);
+  const float* xs = kind == 0 ? Y : X;      // the operand that is read as a bf16 pair
+  if (kind == 0 || kind == 4) tc::k_split_bf16<<<blocks_for(M * ldx, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldx);
+  AVC_LAUNCH_TRY();
+  const tc::SplitPtr a{ah, al, ld}, b{bh, bl, ld};
+  const Split16 none{nullptr, nullptr, ldx};
+  switch (kind) {
+    case 0: {
+      EpiChainBwd e;
+      e.N = N; e.Np = ldx; e.D1 = X; e.QT = nullptr; e.qt16 = Split16{xh, xl, ldx}; e.ZBAR = OUT; e.UNEXT = OUT2;
+      e.ldu = ld2; e.s_next = s; e.u16 = Split16{nullptr, nullptr, ld2};
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    case 1:
+    case 2: {
+      EpiDgrad e;
+      e.Nprev = N; e.Npp = ldx; e.s = s; e.D1prev = X; e.ZBARprev = Y;
+      e.sdfbar = kind == 2 ? v1 : nullptr; e.wsdf = kind == 2 ? v2 : nullptr; e.sdf_inv_scale = s2;
+      e.z16 = none; e.store_f32 = 1;
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    case 3: {
+      EpiChain e;
+      e.Nprev = Nv; e.Npp = ldx; e.s = s; e.D1prev = X; e.QTprev = OUT; e.GE = OUT2; e.EP = ld2; e.E = N - Nv;
+      e.q16 = none;
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    case 4: {
+      EpiDgradRelu e{nullptr, xh, OUT, ldx, none};
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    case 5: {
+      EpiGe e{OUT2, ld2, N};
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+  }
+  return AVC_E_BADCFG;
+}
 
 int avc_neus_param_count(const avc_neus_cfg* cfg, int64_t* n_params) {
   if (!cfg || !n_params) return AVC_E_NULL;

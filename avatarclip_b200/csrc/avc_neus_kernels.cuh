@@ -754,11 +754,13 @@ struct EpiChain {
   int Nprev, Npp; float s; const float* D1prev; float* QTprev; float* GE; int EP; int E; Split16 q16;
   struct Aux { float4 d; };
   __device__ __forceinline__ Aux prefetch(int row, int col) const {
-    const int c = clamp_group(col, Nprev);    // always a valid address; the value is only used when col + 3 < Nprev
+    const int c = clamp_group(col, Npp);      // always a valid address; the value is only used where col + i < Nprev
     return {*reinterpret_cast<const float4*>(D1prev + (size_t)row * Npp + c)};
   }
-  __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
-    tc::l2_prefetch_tile<4>(D1prev, Npp, Npp, m0, n0, bn, M, et, nth);
+  using Stage = tc::Staged<4>;                // the NT tiles stage D1prev in shared memory
+  tc::StageOp stage_op(int) const { return {D1prev, Npp, Npp}; }
+  static __device__ __forceinline__ Aux from_stage(const uint4 (&r)[1]) {
+    return {make_float4(__uint_as_float(r[0].x), __uint_as_float(r[0].y), __uint_as_float(r[0].z), __uint_as_float(r[0].w))};
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
@@ -769,11 +771,12 @@ struct EpiChain {
       split16_put4(q16, (size_t)row, col, q);
       return;
     }
+    const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w};      // D1prev[row][col + i] where col + i < Nprev <= Npp
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       int c = col + i;
       if (c < Nprev) {
-        float qv = D1prev[(size_t)row * Npp + c] * v[i] * s;
+        float qv = dd[i] * v[i] * s;
         if (QTprev) QTprev[(size_t)row * Npp + c] = qv;
         split16_put(q16, (size_t)row, c, qv);
       } else {
@@ -916,54 +919,35 @@ struct EpiChainBwd {
     }
     return x;
   }
-  __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
-    tc::l2_prefetch_tile<4>(D1, Np, Np, m0, n0, bn, M, et, nth);
-    if (QT) {
-      tc::l2_prefetch_tile<4>(QT, Np, Np, m0, n0, bn, M, et, nth);
-    } else {
-      tc::l2_prefetch_tile<2>(qt16.hi, qt16.ld, Np, m0, n0, bn, M, et, nth);
-      tc::l2_prefetch_tile<2>(qt16.lo, qt16.ld, Np, m0, n0, bn, M, et, nth);
-    }
+  // the NT tiles stage D1 and the split of qt in shared memory (they never get the fp32 copy QT)
+  using Stage = tc::Staged<4, 2, 2>;
+  tc::StageOp stage_op(int i) const {
+    if (QT || Np % 4 || N > Np) return {nullptr, 0, 0};
+    return i == 0 ? tc::StageOp{D1, Np, Np} : tc::StageOp{i == 1 ? qt16.hi : qt16.lo, qt16.ld, Np};
   }
-  __device__ __forceinline__ float qt_at(int row, int c) const {
-    return QT ? QT[(size_t)row * Np + c] : split16_get(qt16, (size_t)row, c);
+  static __device__ __forceinline__ Aux from_stage(const uint4 (&r)[3]) {
+    return {make_float4(__uint_as_float(r[0].x), __uint_as_float(r[0].y), __uint_as_float(r[0].z), __uint_as_float(r[0].w)),
+            make_uint4(r[1].x, r[1].y, r[2].x, r[2].y)};
   }
+  // Both engines call with col < N and col % 4 == 0, and Np (a multiple of 8) >= N: every group lies inside the PADDED
+  // width.  The padding of the sp' stash and of qt is zero (EpiValue / EpiChain), so the padding columns of a group get
+  // the zeros the padding of ubar / zbar must hold.
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
-    // whole group inside the PADDED width: the padding of the sp' stash and of qt is zero (EpiValue / EpiChain), so the
-    // vector path yields the zeros the padding of ubar / zbar must hold
-    if (col + 3 < Np) {
-      const size_t o = (size_t)row * Np + col;
-      const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w};
-      float qq[4];
-      if (QT) { qq[0] = __uint_as_float(x.q.x); qq[1] = __uint_as_float(x.q.y); qq[2] = __uint_as_float(x.q.z); qq[3] = __uint_as_float(x.q.w); }
-      else split16_get4(make_uint2(x.q.x, x.q.y), make_uint2(x.q.z, x.q.w), qq);
-      float u[4], zb[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        u[i] = dd[i] * v[i] * s_next;
-        zb[i] = kBeta * (1.f - dd[i]) * qq[i] * v[i];
-      }
-      if (UNEXT) *reinterpret_cast<float4*>(UNEXT + (size_t)row * ldu + col) = make_float4(u[0], u[1], u[2], u[3]);
-      split16_put4(u16, (size_t)row, col, u);
-      *reinterpret_cast<float4*>(ZBAR + o) = make_float4(zb[0], zb[1], zb[2], zb[3]);
-      return;
-    }
-    float zb[4];
+    const size_t o = (size_t)row * Np + col;
+    const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w};
+    float qq[4];
+    if (QT) { qq[0] = __uint_as_float(x.q.x); qq[1] = __uint_as_float(x.q.y); qq[2] = __uint_as_float(x.q.z); qq[3] = __uint_as_float(x.q.w); }
+    else split16_get4(make_uint2(x.q.x, x.q.y), make_uint2(x.q.z, x.q.w), qq);
+    float u[4], zb[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      int c = col + i;
-      if (c < N) {
-        float s1 = D1[(size_t)row * Np + c];
-        float uv = s1 * v[i] * s_next;
-        if (UNEXT) UNEXT[(size_t)row * ldu + c] = uv;
-        split16_put(u16, (size_t)row, c, uv);
-        zb[i] = kBeta * (1.f - s1) * qt_at(row, c) * v[i];
-      } else {
-        zb[i] = 0.f;
-      }
+      u[i] = dd[i] * v[i] * s_next;
+      zb[i] = kBeta * (1.f - dd[i]) * qq[i] * v[i];
     }
-    *reinterpret_cast<float4*>(ZBAR + (size_t)row * Np + col) = make_float4(zb[0], zb[1], zb[2], zb[3]);
+    if (UNEXT) *reinterpret_cast<float4*>(UNEXT + (size_t)row * ldu + col) = make_float4(u[0], u[1], u[2], u[3]);
+    split16_put4(u16, (size_t)row, col, u);
+    *reinterpret_cast<float4*>(ZBAR + o) = make_float4(zb[0], zb[1], zb[2], zb[3]);
   }
   AVC_EPI_DIRECT
 };
@@ -979,39 +963,31 @@ struct EpiDgrad {
     const size_t o = (size_t)row * Npp + clamp_group(col, Npp);
     return {*reinterpret_cast<const float4*>(D1prev + o), *reinterpret_cast<const float4*>(ZBARprev + o)};
   }
-  __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
-    tc::l2_prefetch_tile<4>(D1prev, Npp, Npp, m0, n0, bn, M, et, nth);
-    tc::l2_prefetch_tile<4>(ZBARprev, Npp, Npp, m0, n0, bn, M, et, nth);
+  using Stage = tc::Staged<4, 4>;             // the NT tiles stage D1prev and ZBARprev in shared memory
+  tc::StageOp stage_op(int i) const {
+    if (Npp % 4 || Nprev > Npp) return {nullptr, 0, 0};
+    return {i == 0 ? D1prev : ZBARprev, Npp, Npp};
   }
+  static __device__ __forceinline__ Aux from_stage(const uint4 (&r)[2]) {
+    return {make_float4(__uint_as_float(r[0].x), __uint_as_float(r[0].y), __uint_as_float(r[0].z), __uint_as_float(r[0].w)),
+            make_float4(__uint_as_float(r[1].x), __uint_as_float(r[1].y), __uint_as_float(r[1].z), __uint_as_float(r[1].w))};
+  }
+  // Both engines call with col < Nprev and col % 4 == 0, and Npp (a multiple of 8) >= Nprev: every group lies inside the
+  // padded width, where the sp' stash and the zbar padding are zero, and so is the result.
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
     AVC_EPI_UNPACK;
     float sb = sdfbar ? sdfbar[row] * sdf_inv_scale : 0.f;
-    if (col + 3 < Npp) {      // padded width: sp' stash and zbar padding are zero, so is the result there
-      const size_t o = (size_t)row * Npp + col;
-      const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w}, zo[4] = {x.zb.x, x.zb.y, x.zb.z, x.zb.w};
-      float r[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float ab = v[i];
-        if (sdfbar) ab = fmaf(sb, wsdf[col + i], ab);
-        r[i] = fmaf(dd[i], ab * s, zo[i]);
-      }
-      if (store_f32) *reinterpret_cast<float4*>(ZBARprev + o) = make_float4(r[0], r[1], r[2], r[3]);
-      split16_put4(z16, (size_t)row, col, r);
-      return;
-    }
+    const size_t o = (size_t)row * Npp + col;
+    const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w}, zo[4] = {x.zb.x, x.zb.y, x.zb.z, x.zb.w};
+    float r[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      int c = col + i;
-      if (c < Nprev) {
-        float ab = v[i];
-        if (sdfbar) ab = fmaf(sb, wsdf[c], ab);
-        size_t o = (size_t)row * Npp + c;
-        float zv = fmaf(D1prev[o], ab * s, ZBARprev[o]);
-        if (store_f32) ZBARprev[o] = zv;
-        split16_put(z16, (size_t)row, c, zv);
-      }
+      float ab = v[i];
+      if (sdfbar) ab = fmaf(sb, wsdf[col + i], ab);
+      r[i] = fmaf(dd[i], ab * s, zo[i]);
     }
+    if (store_f32) *reinterpret_cast<float4*>(ZBARprev + o) = make_float4(r[0], r[1], r[2], r[3]);
+    split16_put4(z16, (size_t)row, col, r);
   }
   AVC_EPI_DIRECT
 };

@@ -439,6 +439,12 @@ int avc_tc_gemm_nt_test(const float* A, const float* B, int64_t M, int32_t N, in
  * workspace >= 4 * P * (round_up(N1,8) + round_up(N2,8)) + 2048 bytes. */
 int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, int32_t N2, int32_t nprod,
                         float* C, float* colsum, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+/* The backward epilogue functors of the NeuS path through the NT tiles on caller data: kind 0 second-order sweep,
+ * 1 / 2 value backward without / with the sdf term, 3 gradient chain, 4 ReLU-mask dgrad, 5 encoding-gradient
+ * accumulation (argument roles in avc_neus.cu).  workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes. */
+int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
+                    const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
+                    float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Per-step view preparation of Runner.train_clip (SURVEY.md 8f rank 1), all on the device.
@@ -483,9 +489,10 @@ int avc_uniform_fill(uint32_t seed, int32_t n, float lo, float hi, float* out, a
  * [4] epilogue waiting for the accumulator, [5] epilogue work); this call synchronises the device and copies them. */
 int avc_chain_debug_read(long long* out8);
 /* Stall probe of the wgmma NT tiles: only in a diagnostic build (-DAVC_NT_PROBE=1, tools/nt_probe.py); a regular
- * build returns AVC_E_BADCFG.  host_out[16][8]: per epilogue functor the summed cycles {producer waiting for a free
+ * build returns AVC_E_BADCFG.  host_out[16][9]: per epilogue functor the summed cycles {producer waiting for a free
  * stage, producer loop, consumers waiting for operands, consumers waiting for their turn, consumers' MMAs, consumers'
- * epilogues, consumers' loops, CTAs} (consumer slots: both consumer warpgroups); reset != 0 clears the counters. */
+ * epilogues, consumers' loops, CTAs, consumers waiting for staged epilogue operands} (consumer slots: both consumer
+ * warpgroups); reset != 0 clears the counters. */
 int avc_nt_probe_read(unsigned long long* host_out, int reset);
 
 int avc_march_count(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, int32_t* counts,

@@ -4,11 +4,14 @@
                                           # avc_neus.cu recompiled with -DAVC_NT_PROBE=1
     python tools/nt_probe.py --run OUT    # on the GPU: a few steps of the bench workload through the probe build,
                                           # per epilogue functor where each warp role's loop time went
+    python tools/nt_probe.py --run OUT --lib OTHER.so --slots 8    # another probe build (8 slots: before the
+                                          # epilogue-ring slot existed)
 
 The probe takes clock64 stamps in the TMA producer and in the leading thread of each consumer warpgroup: the producer's
 waits for a free stage, the consumers' waits for operands and for their turn at the tensor pipe, and the time from a
 consumer's turn to its MMAs' completion and from there to the end of its epilogue, summed per functor
-(avc_gemm_tc.cuh, AVC_NT_PROBE).  `busy_over_wall` is the MMA and epilogue time of both consumer warpgroups over the loop
+(avc_gemm_tc.cuh, AVC_NT_PROBE), and the consumers' waits for the epilogue operands staged in shared memory
+(`waits_staged`, functors with a `Stage`).  `busy_over_wall` is the MMA and epilogue time of both consumer warpgroups over the loop
 time of one: above 1, the two worked at the same time (one's MMAs under the other's epilogue)."""
 import argparse
 import ctypes as C
@@ -38,8 +41,8 @@ def build():
     print("built", PROBE_LIB)
 
 
-def run(out_path):
-    os.environ["AVC_B200_LIB"] = PROBE_LIB
+def run(out_path, lib=PROBE_LIB, slots=9):
+    os.environ["AVC_B200_LIB"] = lib
     sys.path.insert(0, ROOT)
     import torch
     from avatarclip_b200 import _lib, workload as WL
@@ -48,7 +51,7 @@ def run(out_path):
     dev = torch.device("cuda", 0)
     L = _lib.lib()
     L.avc_nt_probe_read.argtypes = [C.POINTER(C.c_ulonglong), C.c_int]
-    buf = (C.c_ulonglong * 128)()
+    buf = (C.c_ulonglong * (16 * slots))()
     sp, cp = WL.synth_states(WL.B2_SDF_KW, WL.B2_COL_KW, seed=0)
     _, _, _, ren = WL.build_networks(WL.B2_SDF_KW, WL.B2_COL_KW, WL.B2_REN_KW, sp, cp, 0.3, dev, engine=1)
     tower = ClipImageTower(WL.random_vit_state(seed=0), device=dev)
@@ -64,7 +67,7 @@ def run(out_path):
     assert L.avc_nt_probe_read(buf, 1) == 0
     rep = {}
     for i in range(16):
-        v = [buf[i * 8 + j] for j in range(8)]
+        v = [buf[i * slots + j] for j in range(slots)] + [0] * (9 - slots)
         if v[7] == 0:
             continue
         ctas = v[7]
@@ -75,7 +78,7 @@ def run(out_path):
             "producer_waits_free_stage": v[0] / max(v[1], 1),
             # shares of a consumer warpgroup's loop; the MMA share includes its operand and B-panel waits
             "consumer": {"waits_operands": v[2] / cons, "waits_turn": v[3] / cons, "mma": v[4] / cons,
-                         "epilogue": v[5] / cons},
+                         "epilogue": v[5] / cons, "waits_staged": v[8] / cons},
             "busy_over_wall": (v[4] + v[5]) / (cons / 2),
         }
     with open(out_path, "w") as f:
@@ -87,8 +90,10 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--build", action="store_true")
     ap.add_argument("--run", metavar="OUT")
+    ap.add_argument("--lib", default=PROBE_LIB, help="probe build to load (default: the one --build makes)")
+    ap.add_argument("--slots", type=int, default=9, help="counters per functor of that build")
     a = ap.parse_args()
     if a.build:
         build()
     if a.run:
-        run(a.run)
+        run(a.run, a.lib, a.slots)
