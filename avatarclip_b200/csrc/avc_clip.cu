@@ -1428,4 +1428,124 @@ int avc_clip_encode_text(const avc_clip_text_cfg* cfg, const avc_clip_text_weigh
   return 0;
 }
 
+// One CLIP kernel on caller buffers, launched the way the towers launch it (argument roles in include/avc_b200.h).
+int avc_clip_kernel_test(int32_t kind, const int32_t* d, const void* const* in, void* const* out, avc_stream_t stream) {
+  if (!d || !in || !out) return AVC_E_NULL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const auto H16 = [](const void* p) { return (const __half*)p; };
+  const auto F32 = [](const void* p) { return (const float*)p; };
+  if (kind >= 0 && kind <= 6) {
+    const int M = d[0], N = d[1], K = d[2], ks = d[3];
+    if (M < 1 || N < 1 || K < 1 || ks < 1) return AVC_E_SIZE;
+    const __half *A = H16(in[0]), *W = H16(in[1]);
+    switch (kind) {
+      case 0: return gemm16(st, A, K, W, K, M, N, K, ks, EpiBiasStore{(float*)out[0], N, F32(in[2])});
+      case 1: return gemm16(st, A, K, W, K, M, N, K, ks, EpiResidual{(float*)out[0], N, F32(in[2])});
+      case 2: return gemm16(st, A, K, W, K, M, N, K, ks, EpiFc{(float*)out[0], (__half*)out[1], N, F32(in[2])});
+      case 3: return gemm16(st, A, K, W, K, M, N, K, ks, EpiDfc{F32(in[2]), (__half*)out[1], N});
+      case 4: return gemm16(st, A, K, W, K, M, N, K, ks, EpiAccumUnscale{(float*)out[0], N, F32(in[2])});
+      case 5: return gemm16(st, A, K, W, K, M, N, K, ks, EpiStoreUnscale{(float*)out[0], N, F32(in[2])});
+      default: {
+        const int np = d[4];
+        if (np < 1) return AVC_E_SIZE;
+        return gemm16(st, A, K, W, K, M, N, K, ks, EpiPatch{(float*)out[0], np + 1, N, np});
+      }
+    }
+  }
+  switch (kind) {
+    case 7: {       // k_layernorm
+      const int M = d[0], Wd = d[1];
+      if (M < 1 || Wd < 1 || Wd > 32 * kLnMax) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_layernorm, dim3(ceil_div(M, 8)), dim3(256), 0, st, F32(in[0]), M, Wd, F32(in[1]), F32(in[2]),
+                              (float*)out[0], (__half*)out[1], (float*)out[2]));
+      break;
+    }
+    case 8: {       // k_layernorm_bwd
+      const int M = d[0], Wd = d[1];
+      if (M < 1 || Wd < 1 || Wd > 32 * kLnMax) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_layernorm_bwd, dim3(ceil_div(M, 8)), dim3(256), 0, st, F32(in[0]), (float*)out[0], M, Wd, F32(in[1]),
+                              (float*)out[1], d[2], Wd, Wd, Wd, (__half*)out[2], (float*)out[3], d[3]));
+      break;
+    }
+    case 9: {       // k_to_half_rowscaled
+      const int M = d[0], N = d[1];
+      if (M < 1 || N < 1 || d[2] < N) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_to_half_rowscaled, dim3(ceil_div(M, 8)), dim3(256), 0, st, F32(in[0]), M, N, d[2], (__half*)out[0],
+                              (float*)out[1], (const int*)in[1]));
+      break;
+    }
+    case 10:        // k_attention
+    case 11: {      // k_attention_bwd
+      const int B = d[0], T = d[1], Wd = d[2], heads = d[3];
+      if (B < 1 || T < 1 || T > AT || heads < 1 || Wd != heads * AD) return AVC_E_SIZE;
+      AVC_TRY(set_attn_smem());
+      if (kind == 10)
+        AVC_CUDA_TRY(launch_pdl(k_attention, dim3(B * heads), dim3(512), kAttnFwdSmem, st, F32(in[0]), T, Wd, heads, (__half*)out[0]));
+      else
+        AVC_CUDA_TRY(launch_pdl(k_attention_bwd, dim3(B * heads), dim3(512), kAttnBwdSmem, st, F32(in[0]), F32(in[1]), T, Wd, heads,
+                                (float*)out[0]));
+      break;
+    }
+    case 12: {      // k_causal_attention
+      const int B = d[0], T = d[1], Wd = d[2], heads = d[3];
+      if (B < 1 || T < 1 || T > kTextMaxT || heads < 1 || Wd != heads * AD) return AVC_E_SIZE;
+      AVC_CUDA_TRY(cudaFuncSetAttribute(k_causal_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, kTextAttnSmem));
+      AVC_CUDA_TRY(launch_pdl(k_causal_attention, dim3(B * heads), dim3(kTextAttnThreads), kTextAttnSmem, st, F32(in[0]), T, Wd, heads,
+                              (__half*)out[0]));
+      break;
+    }
+    case 13:        // k_preprocess
+    case 14: {      // k_preprocess_bwd (d canvas is overwritten, as avc_clip_loss_bwd does)
+      const int H = d[0], W = d[1], B = d[2], IS = d[3], P = d[4], mode = d[5];
+      if (H < 1 || W < 1 || B < 1 || P < 1 || IS < P || IS % P || (mode != 0 && mode != 1)) return AVC_E_SIZE;
+      if (mode == 1 && (H != IS || W != IS)) return AVC_E_SIZE;
+      const int64_t npx = (int64_t)B * 3 * IS * IS;
+      if (kind == 13) {
+        AVC_CUDA_TRY(launch_pdl(k_preprocess, dim3((int)((npx + 255) / 256)), dim3(256), 0, st, F32(in[0]), H, W, B, IS, P,
+                                (__half*)out[0], mode));
+      } else {
+        AVC_CUDA_TRY(cudaMemsetAsync(out[0], 0, sizeof(float) * (size_t)B * H * W * 3, st));
+        AVC_CUDA_TRY(launch_pdl(k_preprocess_bwd, dim3((int)((npx + 255) / 256)), dim3(256), 0, st, F32(in[0]), H, W, B, IS, P,
+                                (float*)out[0], mode));
+      }
+      break;
+    }
+    case 15: {      // k_head_proj
+      const int B = d[0], T = d[1], Wd = d[2], OD = d[3];
+      if (B < 1 || T < 1 || Wd < 4 || Wd % 4 || OD < 1) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_head_proj, dim3(B, ceil_div(OD, 64)), dim3(256), (Wd + 256) * sizeof(float), st, F32(in[0]), T, Wd,
+                              F32(in[1]), F32(in[2]), F32(in[3]), OD, (float*)out[0], (float*)out[1]));
+      break;
+    }
+    case 16: {      // k_cosine
+      const int B = d[0], OD = d[1];
+      if (B < 1 || OD < 1) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_cosine, dim3(B), dim3(256), 0, st, F32(in[0]), F32(in[1]), OD, (float*)out[0]));
+      break;
+    }
+    case 17: {      // k_head_bwd_dy
+      const int B = d[0], Wd = d[1], OD = d[2], rows = 96;
+      if (B < 1 || Wd < 1 || OD < 1 || (!in[3] && !in[4])) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_head_bwd_dy, dim3(B, ceil_div(Wd, rows)), dim3(256), OD * sizeof(float), st, Wd, F32(in[0]), OD,
+                              F32(in[1]), F32(in[2]), F32(in[3]), F32(in[4]), (float*)out[0], rows));
+      break;
+    }
+    case 18: {      // k_head_bwd_ln
+      const int B = d[0], T = d[1], Wd = d[2];
+      if (B < 1 || T < 1 || Wd < 1) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_head_bwd_ln, dim3(B), dim3(256), 0, st, F32(in[0]), T, Wd, F32(in[1]), F32(in[2]), (float*)out[0]));
+      break;
+    }
+    case 19: {      // k_text_eot_rows
+      const int B = d[0], T = d[1], Wd = d[2];
+      if (B < 1 || T < 1 || Wd < 1) return AVC_E_SIZE;
+      AVC_CUDA_TRY(launch_pdl(k_text_eot_rows, dim3(B), dim3(32), 0, st, (const int32_t*)in[0], F32(in[1]), T, Wd, (float*)out[0]));
+      break;
+    }
+    default: return AVC_E_BADCFG;
+  }
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
 }  // extern "C"

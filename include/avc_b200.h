@@ -445,6 +445,33 @@ int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, i
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
                     float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+/* One kernel of the CLIP towers (avc_clip.cu) on caller buffers, launched by the host code the towers use (the GEMMs
+ * through the same M <= 128 wgmma / M > 128 mma.sync dispatch and split-K recomputation).  dims is a HOST int array,
+ * in / out are HOST arrays of DEVICE pointers; "h" marks fp16, "i" int32, everything else is fp32.  Outputs are
+ * written in place (x, dst, dy, dx are read as well when the kernel accumulates).  Nothing else is touched.
+ *   0..6 GEMM  acc[M][N] = A[M][K] . Wt[N][K]^T, dims {M, N, K, ksplit (, np)}; in {A h, Wt h, aux}:
+ *        0 out[0][M][N]  = acc + bias(aux[N])                          (EpiBiasStore)
+ *        1 out[0][M][N] += acc + bias(aux[N]) once over the splits      (EpiResidual)
+ *        2 out[0][M][N]  = pre = acc + bias(aux[N]), out[1] h = QuickGELU(pre)     (EpiFc)
+ *        3 out[1] h[M][N] = acc * QuickGELU'(pre), pre = aux[M][N]                 (EpiDfc)
+ *        4 out[0][M][N] += acc / aux[M]                                 (EpiAccumUnscale)
+ *        5 out[0][M][N]  = acc / aux[M]                                 (EpiStoreUnscale)
+ *        6 out[0][b*(np+1) + 1 + p][N] += acc[b*np + p]                 (EpiPatch; aux unused)
+ *   7  k_layernorm      dims {M, Wd};  in {x, g, b};  out {y32, y16 h, save_x}, any may be NULL
+ *   8  k_layernorm_bwd  dims {M, Wd, accumulate, zero_dy};  in {x, g};  out {dy, dx, dx16 h or NULL, dx_scale[M]}
+ *   9  k_to_half_rowscaled  dims {M, N, ld_src};  in {src, row_map i[M] or NULL};  out {dst h[M][N], scale[M]}
+ *   10 k_attention      dims {B, T, Wd, heads};  in {qkv[B*T][3Wd]};  out {o16 h[B*T][Wd]}
+ *   11 k_attention_bwd  dims {B, T, Wd, heads};  in {qkv, dO[B*T][Wd]};  out {dqkv[B*T][3Wd]}
+ *   12 k_causal_attention  dims {B, T, Wd, heads};  in {qkv};  out {o16 h}
+ *   13 k_preprocess     dims {H, W, B, IS, P, mode};  in {canvas};  out {a0 h[B*(IS/P)^2][3P^2]}
+ *   14 k_preprocess_bwd dims as 13;  in {dpatch};  out {dcanvas} (zeroed first)
+ *   15 k_head_proj      dims {B, T, Wd, OD};  in {x[B*T][Wd], g, b, proj[Wd][OD]};  out {emb[B][OD], ynorm[B][Wd]}
+ *   16 k_cosine         dims {B, OD};  in {emb, text};  out {cos[B]}
+ *   17 k_head_bwd_dy    dims {B, Wd, OD};  in {proj, text, emb, g_cos[B] or NULL, g_emb[B][OD] or NULL};  out {dy[B][Wd]}
+ *   18 k_head_bwd_ln    dims {B, T, Wd};  in {x[B*T][Wd], g, dy[B][Wd]};  out {dx[B*T][Wd]}
+ *   19 k_text_eot_rows  dims {B, T, Wd};  in {tok i[B][T], x[B*T][Wd]};  out {eot[B][Wd]} */
+int avc_clip_kernel_test(int32_t kind, const int32_t* dims, const void* const* in, void* const* out,
+                         avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Per-step view preparation of Runner.train_clip (SURVEY.md 8f rank 1), all on the device.

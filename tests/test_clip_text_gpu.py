@@ -118,3 +118,20 @@ def test_unsupported_shapes_and_token_ids_are_rejected():
         t[0, 2] = bad_id
         with pytest.raises(_lib.AvcError, match="token ids"):
             tower.encode_text(t.cuda())
+
+
+@pytest.mark.parametrize("context", [1, 2, 128])
+def test_encode_text_context_lengths(context):
+    """Contexts of 1 and 128 tokens (the causal attention's limit) on a two-layer tower."""
+    from avatarclip_b200.clip_text import ClipTextTower
+    conf = ot.TextConf(context=context, vocab=1000, layers=2)
+    sd = ot.random_text_state(conf, seed=context)
+    g = torch.Generator().manual_seed(context)
+    tok = torch.randint(1, 999, (3, context), generator=g, dtype=torch.int32)
+    tok[0, -1] = 999
+    tok[1, context // 2] = 999
+    want = ot.encode_text(sd, tok, conf)
+    got = ClipTextTower(sd, device="cuda").encode_text(tok.cuda()).cpu()
+    err = U.rel_to_max(got, want)
+    U.log_parity("clip_text_context", {"context": context, "emb_rel_to_max": err})
+    assert err < 1.7e-3         # measured <= 4.39e-4 on an H100 (400 W)
