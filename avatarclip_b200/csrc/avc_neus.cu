@@ -277,14 +277,35 @@ int gradient_chain(const NeusPlan& pl, const NeusWs& w, int64_t P, float* grad_o
 }
 
 // -------------------------------------------------------------------------------- placement
+// The per-kernel launches are shared by the render and the kernel self-test (avc_neus_kernel_test).
+int coarse_z(const float* near, const float* far, const float* jitter, int n, int pitch, int Rc, float* z,
+             cudaStream_t st) {
+  k_coarse_z<<<blocks_for((int64_t)Rc * n, 256), 256, 0, st>>>(near, far, jitter, n, pitch, Rc, z);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int upsample(const float* rays_o, const float* rays_d, const float* z, const float* sdf, int n, int pitch, int Rc,
+             float inv_s, int per, float* newz, cudaStream_t st) {
+  k_upsample<<<blocks_for(Rc, 8), 256, 0, st>>>(rays_o, rays_d, z, sdf, n, pitch, Rc, inv_s, per, newz);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int merge(const float* z, const float* sdf, int n, int pitch, const float* newz, const float* news, int per, int Rc,
+          float* zo, float* so, int pitch_o, cudaStream_t st) {
+  k_merge<<<blocks_for(Rc, 8), 256, 0, st>>>(z, sdf, n, pitch, newz, news, per, Rc, zo, so, pitch_o);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
 int place_samples(const NeusPlan& pl, const NeusWs& w, const float* rays_o, const float* rays_d, const float* near,
                   const float* far, const float* jitter, int Rc, float* z_out_raymajor, cudaStream_t st) {
   // ray-major buffers [Rc][S]; one warp per ray in the per-ray kernels
   const int S = pl.S;
   if (S > kPlaceMaxN || pl.per > kPlaceMaxNew) return AVC_E_BADCFG;
   float* z0 = (pl.cfg.n_importance == 0) ? z_out_raymajor : w.zA;
-  k_coarse_z<<<blocks_for((int64_t)Rc * pl.n0, 256), 256, 0, st>>>(near, far, jitter, pl.n0, S, Rc, z0);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(coarse_z(near, far, jitter, pl.n0, S, Rc, z0, st));
   if (pl.cfg.n_importance == 0) return 0;
   EncodeTargets t = make_targets(pl, w);
   int64_t Pn = (int64_t)pl.n0 * Rc;
@@ -297,8 +318,7 @@ int place_samples(const NeusPlan& pl, const NeusWs& w, const float* rays_o, cons
   for (int i = 0; i < pl.steps; ++i) {
     const bool last = (i + 1 == pl.steps);
     float inv_s = 64.0f * (float)(1 << i);                                     // renderer.py:346
-    k_upsample<<<blocks_for(Rc, 8), 256, 0, st>>>(rays_o, rays_d, zc, sc, n, S, Rc, inv_s, pl.per, w.newZ);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(upsample(rays_o, rays_d, zc, sc, n, S, Rc, inv_s, pl.per, w.newZ, st));
     if (!last) {
       Pn = (int64_t)pl.per * Rc;
       k_encode_samples<<<blocks_for(Pn * 8, 256), 256, 0, st>>>(rays_o, rays_d, w.newZ, pl.per, pl.per, Rc,
@@ -307,9 +327,7 @@ int place_samples(const NeusPlan& pl, const NeusWs& w, const float* rays_o, cons
       AVC_TRY(value_chain(pl, w, Pn, false, false, w.newS, st, 0, 0));   // newS is [Rc][per]: identity mapping
     }
     // the last round writes the merged depths straight into the caller's z_vals [Rc][S]
-    k_merge<<<blocks_for(Rc, 8), 256, 0, st>>>(zc, sc, n, S, w.newZ, last ? nullptr : w.newS, pl.per, Rc,
-                                               last ? z_out_raymajor : zn, sn, S);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(merge(zc, sc, n, S, w.newZ, last ? nullptr : w.newS, pl.per, Rc, last ? z_out_raymajor : zn, sn, S, st));
     float* tz = zc; zc = zn; zn = tz;
     float* ts = sc; sc = sn; sn = ts;
     n += pl.per;
@@ -333,6 +351,55 @@ CompositeArgs make_composite_args(const NeusPlan& pl, const NeusWs& w, const Chu
   A.sample_dist = 2.0f / (float)pl.n0;                                         // renderer.py:304
   A.S = pl.S; A.Rc = io.Rc;
   return A;
+}
+
+// Compositing forward of one chunk; adds the chunk's eikonal sums into ctx.  Only the per-ray outputs of `out` are used.
+int composite_forward(const CompositeArgs& A, const avc_neus_outputs& out, float* ray_part, float* ctx,
+                      cudaStream_t st) {
+  k_composite_fwd<<<blocks_for(A.Rc, 8), 256, 0, st>>>(A, out.color_fine, out.extra_color_fine, out.s_val, out.cdf_fine,
+                                                       out.weight_sum, out.weight_max, out.weights, ray_part);
+  AVC_LAUNCH_TRY();
+  k_reduce_ray_part<<<1, 1024, 0, st>>>(ray_part, A.Rc, 0, ctx + CTX_EIK_NUM);
+  k_reduce_ray_part<<<1, 1024, 0, st>>>(ray_part, A.Rc, 1, ctx + CTX_EIK_DEN);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// Compositing backward of one chunk; adds the chunk's inv_s adjoint into ctx.
+int composite_backward(const CompositeArgs& A, const CompositeBwdArgs& G, float* ctx, cudaStream_t st) {
+  k_composite_bwd<<<blocks_for(A.Rc, 8), 256, 0, st>>>(A, G);
+  AVC_LAUNCH_TRY();
+  k_reduce_ray_part<<<1, 1024, 0, st>>>(G.ray_part, A.Rc, 2, ctx + CTX_INVS_BAR);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// Eikonal normaliser of one chunk, added into ctx (k_relax_count writes ray_part[r][1]).
+int relax_count(const float* rays_o, const float* rays_d, const float* z_vals, int S, int64_t Rc, float sample_dist,
+                float* ray_part, float* ctx, cudaStream_t st) {
+  k_relax_count<<<blocks_for(Rc, 8), 256, 0, st>>>(rays_o, rays_d, z_vals, S, Rc, sample_dist, ray_part);
+  k_reduce_ray_part<<<1, 1024, 0, st>>>(ray_part, Rc, 1, ctx + CTX_EIK_DEN);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int ctx_init(const float* params, int64_t off_var, float* ctx, int zero_sums, cudaStream_t st) {
+  k_ctx_init<<<1, 32, 0, st>>>(params, off_var, ctx, zero_sums);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int finalize_fwd(const float* ctx, float* gerr_out, cudaStream_t st) {
+  k_finalize_fwd<<<1, 32, 0, st>>>(ctx, gerr_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int variance_grad(const float* params, int64_t off_var, const float* ctx, const float* g_sval, int64_t R,
+                  float* grad_var, cudaStream_t st) {
+  k_variance_grad<<<1, 256, 0, st>>>(params, off_var, ctx, g_sval, R, grad_var);
+  AVC_LAUNCH_TRY();
+  return 0;
 }
 
 // Runs the fine pass on io.out.z_vals; with write_outputs=false only the stash is (re)built.
@@ -368,16 +435,7 @@ int fine_forward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, bool wr
                                                              pack + pl.pk_b6, P, oh);
     AVC_LAUNCH_TRY();
   }
-  if (write_outputs) {
-    CompositeArgs A = make_composite_args(pl, w, io);
-    k_composite_fwd<<<blocks_for(io.Rc, 8), 256, 0, st>>>(A, io.out.color_fine, io.out.extra_color_fine, io.out.s_val,
-                                                          io.out.cdf_fine, io.out.weight_sum, io.out.weight_max,
-                                                          io.out.weights, w.ray_part);
-    AVC_LAUNCH_TRY();
-    k_reduce_ray_part<<<1, 1024, 0, st>>>(w.ray_part, io.Rc, 0, w.ctx + CTX_EIK_NUM);
-    k_reduce_ray_part<<<1, 1024, 0, st>>>(w.ray_part, io.Rc, 1, w.ctx + CTX_EIK_DEN);
-    AVC_LAUNCH_TRY();
-  }
+  if (write_outputs) AVC_TRY(composite_forward(make_composite_args(pl, w, io), io.out, w.ray_part, w.ctx, st));
   return 0;
 }
 
@@ -416,10 +474,7 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
   G.g_w = cot.weights; G.g_cdf = cot.cdf_fine; G.g_n = cot.gradients; G.g_gerr = cot.gradient_error;
   G.weights = io.out.weights;
   G.y6bar = w.y6bar; G.sdfbar = w.sdfbar; G.nbar = w.nbar; G.ray_part = w.ray_part;
-  k_composite_bwd<<<blocks_for(io.Rc, 8), 256, 0, st>>>(A, G);
-  AVC_LAUNCH_TRY();
-  k_reduce_ray_part<<<1, 1024, 0, st>>>(w.ray_part, io.Rc, 2, w.ctx + CTX_INVS_BAR);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(composite_backward(A, G, w.ctx, st));
 
   // ---- colour heads: lin{Lc} <- y6bar[:,0:3], extra_lin <- y6bar[:,3:6]   (models/fields.py:172-181)
   {
@@ -668,6 +723,71 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
   return AVC_E_BADCFG;
 }
 
+// One compositing, scalar or placement kernel of the NeuS path on caller buffers, launched by the render's own host
+// helpers (argument roles in include/avc_b200.h).
+int avc_neus_kernel_test(int32_t kind, const int64_t* d, const float* fs, const void* const* in, void* const* out,
+                         avc_stream_t stream) {
+  if (!d || !fs || !in || !out) return AVC_E_NULL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const auto F32 = [](const void* p) { return (const float*)p; };
+  const auto O32 = [](void* p) { return (float*)p; };
+  switch (kind) {
+    case 0: return ctx_init(F32(in[0]), d[0], O32(out[0]), (int)d[1], st);
+    case 1:
+    case 2: {
+      const int S = (int)d[0], bg_kind = (int)d[2];
+      const int64_t Rc = d[1];
+      if (S < 1 || S > 256 || Rc < 1) return AVC_E_SIZE;
+      if (bg_kind < 0 || bg_kind > 2 || (bg_kind != 0 && !in[5])) return AVC_E_BADCFG;
+      CompositeArgs A;
+      A.rays_d = F32(in[0]); A.z_vals = F32(in[1]); A.sdf = F32(in[2]); A.cin = F32(in[3]); A.rgb6 = F32(in[4]);
+      A.background = F32(in[5]); A.bg_kind = bg_kind; A.cos_anneal = fs[0]; A.sample_dist = fs[1]; A.S = S; A.Rc = Rc;
+      if (kind == 1) {
+        float* ctx = O32(out[8]);
+        A.ctx = ctx;
+        avc_neus_outputs o;
+        memset(&o, 0, sizeof(o));
+        o.color_fine = O32(out[0]); o.extra_color_fine = O32(out[1]); o.s_val = O32(out[2]); o.cdf_fine = O32(out[3]);
+        o.weight_sum = O32(out[4]); o.weight_max = O32(out[5]); o.weights = O32(out[6]);
+        return composite_forward(A, o, O32(out[7]), ctx, st);
+      }
+      float* ctx = O32(out[4]);
+      A.ctx = ctx;
+      CompositeBwdArgs G;
+      G.g_color = F32(in[6]); G.g_extra = F32(in[7]); G.g_wsum = F32(in[8]); G.g_wmax = F32(in[9]);
+      G.g_w = F32(in[10]); G.g_cdf = F32(in[11]); G.g_n = F32(in[12]); G.g_gerr = F32(in[13]); G.weights = F32(in[14]);
+      if (G.g_wmax && !G.weights) return AVC_E_NULL;
+      G.y6bar = O32(out[0]); G.sdfbar = O32(out[1]); G.nbar = O32(out[2]); G.ray_part = O32(out[3]);
+      return composite_backward(A, G, ctx, st);
+    }
+    case 3: {
+      if (d[0] < 1 || d[1] < 1) return AVC_E_SIZE;
+      return relax_count(F32(in[0]), F32(in[1]), F32(in[2]), (int)d[0], d[1], fs[0], O32(out[0]), O32(out[1]), st);
+    }
+    case 4: return finalize_fwd(F32(in[0]), O32(out[0]), st);
+    case 5: return variance_grad(F32(in[0]), d[0], F32(in[1]), F32(in[2]), d[1], O32(out[0]), st);
+    case 6: {
+      const int n = (int)d[0], pitch = (int)d[1], Rc = (int)d[2];
+      if (n < 1 || pitch < n || Rc < 1) return AVC_E_SIZE;
+      return coarse_z(F32(in[0]), F32(in[1]), F32(in[2]), n, pitch, Rc, O32(out[0]), st);
+    }
+    case 7: {
+      const int n = (int)d[0], pitch = (int)d[1], Rc = (int)d[2], per = (int)d[3];
+      if (n < 2 || n > kPlaceMaxN || pitch < n || Rc < 1 || per < 1 || per > kPlaceMaxNew) return AVC_E_SIZE;
+      return upsample(F32(in[0]), F32(in[1]), F32(in[2]), F32(in[3]), n, pitch, Rc, fs[0], per, O32(out[0]), st);
+    }
+    case 8: {
+      const int n = (int)d[0], pitch = (int)d[1], Rc = (int)d[2], per = (int)d[3], pitch_o = (int)d[4];
+      if (n < 1 || n > kPlaceMaxN || pitch < n || Rc < 1 || per < 1 || per > kPlaceMaxNew || pitch_o < n + per)
+        return AVC_E_SIZE;
+      if (in[3] && !out[1]) return AVC_E_NULL;
+      return merge(F32(in[0]), F32(in[1]), n, pitch, F32(in[2]), F32(in[3]), per, Rc, O32(out[0]), O32(out[1]), pitch_o,
+                   st);
+    }
+  }
+  return AVC_E_BADCFG;
+}
+
 int avc_neus_param_count(const avc_neus_cfg* cfg, int64_t* n_params) {
   if (!cfg || !n_params) return AVC_E_NULL;
   NeusPlan pl;
@@ -727,8 +847,7 @@ int avc_neus_render_fwd(const avc_neus_cfg* cfg, const float* params, const floa
   cudaStream_t st = (cudaStream_t)stream;
 
   AVC_TRY(prepare_weights(pl, w, params, st));
-  k_ctx_init<<<1, 32, 0, st>>>(params, pl.off_var, w.ctx, 1);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(ctx_init(params, pl.off_var, w.ctx, 1, st));
 
   for (int64_t r0 = 0; r0 < R; r0 += Rc_max) {
     const int64_t Rc = (R - r0) < Rc_max ? (R - r0) : Rc_max;
@@ -748,9 +867,7 @@ int avc_neus_render_fwd(const avc_neus_cfg* cfg, const float* params, const floa
     }
     AVC_TRY(fine_forward(pl, w, io, true, st));
   }
-  k_finalize_fwd<<<1, 32, 0, st>>>(w.ctx, out->gradient_error);
-  AVC_LAUNCH_TRY();
-  return 0;
+  return finalize_fwd(w.ctx, out->gradient_error, st);
 }
 
 int avc_neus_render_bwd(const avc_neus_cfg* cfg, const float* params, const float* rays_o, const float* rays_d,
@@ -775,14 +892,11 @@ int avc_neus_render_bwd(const avc_neus_cfg* cfg, const float* params, const floa
   // The workspace still holds pack / ctx sums / (single chunk) the stash of the matching forward.
   // Multi-chunk calls rebuild the stash per chunk from the saved depths.
   AVC_CUDA_TRY(cudaMemsetAsync(w.wbar, 0, sizeof(float) * (size_t)pl.n_params, st));
-  k_ctx_init<<<1, 32, 0, st>>>(params, pl.off_var, w.ctx, 1);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(ctx_init(params, pl.off_var, w.ctx, 1, st));
   for (int64_t r0 = 0; r0 < R; r0 += Rc_max) {   // eikonal normaliser over ALL rays of the call
     const int64_t Rc = (R - r0) < Rc_max ? (R - r0) : Rc_max;
-    k_relax_count<<<blocks_for(Rc, 8), 256, 0, st>>>(rays_o + r0 * 3, rays_d + r0 * 3, fwd_out->z_vals + r0 * pl.S,
-                                                       pl.S, Rc, 2.0f / (float)pl.n0, w.ray_part);
-    k_reduce_ray_part<<<1, 1024, 0, st>>>(w.ray_part, Rc, 1, w.ctx + CTX_EIK_DEN);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(relax_count(rays_o + r0 * 3, rays_d + r0 * 3, fwd_out->z_vals + r0 * pl.S, pl.S, Rc, 2.0f / (float)pl.n0,
+                        w.ray_part, w.ctx, st));
   }
   if (!single) AVC_TRY(prepare_weights(pl, w, params, st));
   for (int64_t r0 = 0; r0 < R; r0 += Rc_max) {
@@ -797,9 +911,7 @@ int avc_neus_render_bwd(const avc_neus_cfg* cfg, const float* params, const floa
     AVC_TRY(fine_backward(pl, w, io, c, st));
   }
   AVC_TRY(weight_norm_backward_all(pl, params, w.wbar, grad_params, st));
-  k_variance_grad<<<1, 256, 0, st>>>(params, pl.off_var, w.ctx, cot->s_val, R, grad_params + pl.off_var);
-  AVC_LAUNCH_TRY();
-  return 0;
+  return variance_grad(params, pl.off_var, w.ctx, cot->s_val, R, grad_params + pl.off_var, st);
 }
 
 int avc_neus_sdf_query(const avc_neus_cfg* cfg, const float* params, const float* pts, int64_t P, float* sdf_out,

@@ -240,10 +240,11 @@ __global__ void k_encode_fine(const float* __restrict__ rays_o, const float* __r
 // Discontinuous decisions (bin search, radius < 1) use separately rounded mul/add like torch eager.
 // =============================================================================================
 __device__ __forceinline__ float torch_linspace(float start, float end, int n, int j) {
-  // at::linspace (float): step = (end-start)/(n-1); first half start + step*j, second half end - step*(n-1-j)
+  // at::linspace's CUDA kernel (float): step = (end-start)/(n-1); first half start + step*j, second half
+  // end - step*(n-1-j), each contracted into one FMA as torch's build compiles it
   if (n == 1) return start;
   float step = (end - start) / (float)(n - 1);
-  return (j < n / 2) ? __fadd_rn(start, __fmul_rn(step, (float)j)) : __fsub_rn(end, __fmul_rn(step, (float)(n - 1 - j)));
+  return (j < n / 2) ? __fmaf_rn(step, (float)j, start) : __fmaf_rn(-step, (float)(n - 1 - j), end);
 }
 
 // Placement buffers are RAY-MAJOR [ray][pitch]; one warp per ray.
@@ -255,7 +256,8 @@ __global__ void k_coarse_z(const float* __restrict__ near, const float* __restri
   float nr = near[r], fr = far[r];
   float span = __fsub_rn(fr, nr);
   float zz = __fadd_rn(nr, __fmul_rn(span, torch_linspace(0.f, 1.f, n, j)));   // renderer.py:305-306
-  if (jitter) zz = __fadd_rn(zz, __fdiv_rn(__fmul_rn(jitter[r], 2.0f), (float)n));   // renderer.py:319
+  // renderer.py:319; torch divides a CUDA tensor by a scalar as a product with the scalar's fp32 reciprocal
+  if (jitter) zz = __fadd_rn(zz, __fmul_rn(__fmul_rn(jitter[r], 2.0f), __frcp_rn((float)n)));
   z[(size_t)r * pitch + j] = zz;
 }
 

@@ -445,6 +445,28 @@ int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, i
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
                     float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+/* One compositing, scalar or placement kernel of the NeuS path (avc_neus_kernels.cuh) on caller buffers, launched by the
+ * host helpers the render uses.  dims is a HOST int64 array, fscal a HOST float array, in / out HOST arrays of DEVICE
+ * pointers (all fp32).  An input marked "or NULL" may be NULL exactly where the render passes NULL.  ctx is the [4+]
+ * scalar block {inv_s, eik_num, eik_den, invs_bar}; the kinds add into its sums as the render does.
+ *   0 k_ctx_init       dims {off_var, zero_sums};  in {params};  out {ctx}
+ *   1 k_composite_fwd + k_reduce_ray_part (eik_num, eik_den)   dims {S <= 256, Rc, bg_kind};  fscal {cos_anneal,
+ *     sample_dist};  in {rays_d[Rc][3], z[Rc][S], sdf[P], cin[P][8], rgb6[P][8], background ([3] | [Rc] | NULL)};
+ *     out {color[Rc][3], extra[Rc][3], s_val[Rc], cdf[P], wsum[Rc], wmax[Rc], weights[P], ray_part[Rc][4], ctx}
+ *   2 k_composite_bwd + k_reduce_ray_part (invs_bar)   dims, fscal as 1;  in {as 1, then the cotangents g_color[Rc][3],
+ *     g_extra[Rc][3], g_wsum[Rc], g_wmax[Rc], g_w[P], g_cdf[P], g_n[P][3], g_gerr[1] (each or NULL), weights[P] (or NULL
+ *     when g_wmax is)};  out {y6bar[P][8], sdfbar[P], nbar[P][4], ray_part[Rc][4], ctx}
+ *   3 k_relax_count + k_reduce_ray_part (eik_den)   dims {S, Rc};  fscal {sample_dist};  in {rays_o, rays_d, z[Rc][S]};
+ *     out {ray_part[Rc][4], ctx}
+ *   4 k_finalize_fwd   in {ctx};  out {gradient_error[1]}
+ *   5 k_variance_grad  dims {off_var, R};  in {params, ctx, g_sval[R] or NULL};  out {grad_var[1]}
+ *   6 k_coarse_z       dims {n, pitch, Rc};  in {near[Rc], far[Rc], jitter[Rc] or NULL};  out {z[Rc][pitch]}
+ *   7 k_upsample       dims {n (2..256), pitch, Rc, per (1..64)};  fscal {inv_s};  in {rays_o, rays_d, z[Rc][pitch],
+ *     sdf[Rc][pitch]};  out {newz[Rc][per]}
+ *   8 k_merge          dims {n (<= 256), pitch, Rc, per (<= 64), pitch_o >= n + per};  in {z[Rc][pitch], sdf[Rc][pitch],
+ *     newz[Rc][per], news[Rc][per] or NULL};  out {zo[Rc][pitch_o], so[Rc][pitch_o] (unused when news is NULL)} */
+int avc_neus_kernel_test(int32_t kind, const int64_t* dims, const float* fscal, const void* const* in, void* const* out,
+                         avc_stream_t stream);
 /* One kernel of the CLIP towers (avc_clip.cu) on caller buffers, launched by the host code the towers use (the GEMMs
  * through the same M <= 128 wgmma / M > 128 mma.sync dispatch and split-K recomputation).  dims is a HOST int array,
  * in / out are HOST arrays of DEVICE pointers; "h" marks fp16, "i" int32, everything else is fp32.  Outputs are

@@ -341,6 +341,22 @@ def render_core(sdf_p, col_p, variance, sconf: SDFConf, cconf: ColorConf, rconf:
         sampled, extra_sampled = raw.reshape(R, S, 3), None
 
     inv_s = inv_s_from_variance(variance).reshape(1, 1).expand(R * S, 1)
+    c = composite(sdf, grads, pts, sampled, extra_sampled, dists, inv_s, dirs, background_rgb, cos_anneal_ratio)
+    return {
+        "color": c["color"], "extra_color": c["extra_color"], "sdf": sdf, "dists": dists,
+        "gradients": grads.reshape(R, S, 3), "s_val": 1.0 / inv_s, "mid_z_vals": mid_z,
+        "weights": c["weights"], "cdf": c["cdf"], "gradient_error": c["gradient_error"],
+        "inside_sphere": c["inside"],
+    }
+
+
+def composite(sdf, grads, pts, sampled, extra_sampled, dists, inv_s, dirs, background_rgb=None,
+              cos_anneal_ratio: float = 0.0, relax_total=None):
+    """The compositing of render_core, models/renderer.py:234-286, on per-sample tensors: sdf [P,1], grads / pts /
+    dirs [P,3] (P = R*S, ray-major), sampled / extra_sampled [R,S,3] (extra_sampled None without extra_color), dists
+    [R,S], inv_s broadcastable to [P,1].  ``relax_total`` replaces the eikonal normaliser relax.sum() (the product sums
+    it over every chunk of a call).  Also returns the per-ray ``relax`` mask and the per-sample ``alpha``."""
+    R, S = dists.shape
     true_cos = (dirs * grads).sum(-1, keepdim=True)
     iter_cos = -(F.relu(-true_cos * 0.5 + 0.5) * (1.0 - cos_anneal_ratio)
                  + F.relu(-true_cos) * cos_anneal_ratio)
@@ -354,28 +370,26 @@ def render_core(sdf_p, col_p, variance, sconf: SDFConf, cconf: ColorConf, rconf:
     alpha = ((pp + 1e-5) / (cc + 1e-5)).reshape(R, S).clip(0.0, 1.0)
 
     pts_norm = torch.linalg.norm(pts, ord=2, dim=-1, keepdim=True).reshape(R, S)
-    inside = (pts_norm < 1.0).to(z_vals.dtype).detach()
-    relax = (pts_norm < 1.2).to(z_vals.dtype).detach()
+    inside = (pts_norm < 1.0).to(dists.dtype).detach()
+    relax = (pts_norm < 1.2).to(dists.dtype).detach()
 
-    trans = torch.cumprod(torch.cat([torch.ones(R, 1, dtype=z_vals.dtype), 1.0 - alpha + 1e-7], -1), -1)[:, :-1]
+    ones = torch.ones(R, 1, dtype=dists.dtype, device=dists.device)
+    trans = torch.cumprod(torch.cat([ones, 1.0 - alpha + 1e-7], -1), -1)[:, :-1]
     weights = alpha * trans
     wsum = weights.sum(-1, keepdim=True)
     color = (sampled * weights[..., None]).sum(1)
-    extra_color = (extra_sampled * weights[..., None]).sum(1) if rconf.extra_color else None
+    extra_color = (extra_sampled * weights[..., None]).sum(1) if extra_sampled is not None else None
     if background_rgb is not None:
-        if rconf.extra_color:
+        if extra_sampled is not None:
             extra_color = extra_color + background_rgb * (1.0 - wsum)
         else:
             color = color + background_rgb * (1.0 - wsum)
 
     gnorm = torch.linalg.norm(grads.reshape(R, S, 3), ord=2, dim=-1)
-    gerr = (relax * (gnorm - 1.0) ** 2).sum() / (relax.sum() + 1e-5)
-    return {
-        "color": color, "extra_color": extra_color, "sdf": sdf, "dists": dists,
-        "gradients": grads.reshape(R, S, 3), "s_val": 1.0 / inv_s, "mid_z_vals": mid_z,
-        "weights": weights, "cdf": cc.reshape(R, S), "gradient_error": gerr,
-        "inside_sphere": inside,
-    }
+    den = relax.sum() if relax_total is None else relax_total
+    gerr = (relax * (gnorm - 1.0) ** 2).sum() / (den + 1e-5)
+    return {"color": color, "extra_color": extra_color, "weights": weights, "cdf": cc.reshape(R, S),
+            "gradient_error": gerr, "inside": inside, "relax": relax, "alpha": alpha}
 
 
 def render(sdf_p, col_p, variance, sconf: SDFConf, cconf: ColorConf, rconf: RenderConf,

@@ -6,8 +6,9 @@ Why it exists: the reference obtains its second-order terms from
 the formulas down.  The CUDA path must.  This file states them once, in the exact
 step order the kernels of ``avatarclip_b200/csrc`` execute (the step names below are
 the kernel names), and ``tests/test_oracle_manual.py`` proves them against
-``oracle.neus`` autograd in fp64.  GPU tests then compare each CUDA stage with the
-matching stage here.
+``oracle.neus`` autograd in fp64.  The GPU tests compare the whole render with this
+oracle; tests/test_neus_kernels_gpu.py checks the compositing, scalar and placement
+kernels alone against fp64 autograd of oracle.neus (oracle/neus_kernels.py).
 
 Symbols (per sample point; P = rays x samples):
   y = scale * x, e = enc(y) [E];  in_l: input of linear l (after the optional skip
