@@ -58,9 +58,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 // CTAs of every launch, per epilogue functor (Epi::kProbeId), in the slots
 //   0 producer waits for a free stage   1 producer loop          2 consumers wait for operands   3 consumers wait for turn
 //   4 consumers' MMAs (turn to done)    5 consumers' epilogues   6 consumers' loops              7 CTAs
-//   8 consumers wait for staged epilogue operands
+//   8 consumers wait for staged epilogue operands     9 consumers wait for their TMA stores to release a ring slot
 // (the consumer slots add up both consumer warpgroups).  AVC_PROBE(...) code only exists in the probe build.
-constexpr int kNtProbeSlots = 9;
+constexpr int kNtProbeSlots = 10;
 #ifdef AVC_NT_PROBE
 static __device__ unsigned long long g_nt_probe[16][kNtProbeSlots];
 #define AVC_PROBE(...) __VA_ARGS__
@@ -114,6 +114,17 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
+// TMA bulk store of a box from shared memory; elements outside the map's extents are not written
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int x, int y) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"((uint64_t)map), "r"(src), "r"(x), "r"(y) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// all of this thread's bulk groups have completed their writes
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------ host: tensor maps
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -169,9 +180,9 @@ static inline int make_map_bf16(CUtensorMap* m, const void* base, uint64_t rows,
 // Cached like make_map_bf16_cached.
 static inline int make_map_rows_cached(CUtensorMap* m, int es, const void* base, uint64_t rows, uint64_t cols,
                                        uint64_t ld, uint32_t box_cols, uint32_t box_rows) {
-  static thread_local MapCacheEntry cache[64];
+  static thread_local MapCacheEntry cache[256];
   const uint64_t h = ((uintptr_t)base >> 8) * 0x9E3779B97F4A7C15ull ^ (rows * 31 + cols * 131 + ld * 7 + box_cols + 3 * box_rows + es);
-  MapCacheEntry& e = cache[(h >> 32) & 63];
+  MapCacheEntry& e = cache[(h >> 32) & 255];
   const uint32_t bc = box_cols | ((uint32_t)es << 16);      // the element size is part of the key
   if (e.base == base && e.rows == rows && e.cols == cols && e.ld == ld && e.bc == bc && e.br == box_rows) {
     *m = e.map;
@@ -215,8 +226,8 @@ constexpr int kNtTurnBar = 1;     // named barrier kNtTurnBar + c: consumer warp
 // RESB: the CTA keeps its whole B panel (BN rows x up to kResK k-blocks, hi and lo) resident in shared memory and only
 // streams A: re-fetched for every row tile, the B panel would multiply the L2 -> SM operand traffic of a tile.
 constexpr int kResK = 4;          // k-blocks (of 64) a resident panel holds: K <= 256
-// Functors with staged epilogue operands (EpiStage below) give the A ring kEpiAStages stages and the rest of the shared
-// memory to the epilogue rings, at most kEpiSlotsMax slots per consumer warpgroup.
+// Functors with epilogue rings (staged operands, EpiStage, or ring-stored outputs, EpiOut, below) give the A ring
+// kEpiAStages stages and the rest of the shared memory to the rings, at most kEpiSlotsMax slots per consumer warpgroup.
 constexpr int kEpiAStages = 3, kEpiSlotsMax = 8;
 // EPI_SLOT: bytes of one epilogue ring slot (0: the functor stages nothing, no rings)
 template <int BN, int NPROD, bool RESB = false, int EPI_SLOT = 0>
@@ -248,18 +259,24 @@ struct EpiTraits {
   using Aux = NoAux;
   static __device__ __forceinline__ Aux prefetch(const E&, int, int) { return {}; }
   static __device__ __forceinline__ void apply(const E& e, int r, int c, float4 a, const Aux&) { e(r, c, a); }
+  template <typename S>
+  static __device__ __forceinline__ void ring(const E& e, int r, int c, float4 a, const Aux&, const S& s) { e.ring(r, c, a, s); }
 };
 template <typename E>
 struct EpiTraits<E, std::void_t<typename E::Aux>> {
   using Aux = typename E::Aux;
   static __device__ __forceinline__ Aux prefetch(const E& e, int r, int c) { return e.prefetch(r, c); }
   static __device__ __forceinline__ void apply(const E& e, int r, int c, float4 a, const Aux& x) { e(r, c, a, x); }
+  template <typename S>
+  static __device__ __forceinline__ void ring(const E& e, int r, int c, float4 a, const Aux& x, const S& s) { e.ring(r, c, a, x, s); }
 };
 // groups of 8 columns per epilogue batch: two batches of global operands are live beside the accumulator; with 32-byte
 // operands (EpiChainBwd, EpiDgrad) batches of 4 need more registers than ptxas grants a 384-thread kernel and spill
-template <typename E>
+// (RING: outputs stored through the epilogue ring, EpiOut below: batches of 2, so that two slots per consumer fit beside
+// the B panel)
+template <typename E, bool RING = false>
 struct EpiBatch {
-  static constexpr int kB = sizeof(typename EpiTraits<E>::Aux) > 16 ? 2 : 4;
+  static constexpr int kB = (RING || sizeof(typename EpiTraits<E>::Aux) > 16) ? 2 : 4;
   static constexpr int kCols = 8 * kB;
 };
 
@@ -290,15 +307,20 @@ template <int N>
 struct EpiMaps { CUtensorMap m[N]; };
 template <>
 struct EpiMaps<0> {};
-// 4 elements at (r, c) of a [64][cols] box as TMA wrote it: rows of span = cols * ES bytes, swizzled over the span
-// (16-byte unit bits 4.. ^= address bits 7..)
-// (volatile: stays behind the slot's full-barrier wait)
+// Address of the 4 elements at (r, c) of a [rows][COLS] box as TMA reads and writes it: rows of span = COLS * ES bytes,
+// swizzled over the span (16-byte unit bits 4.. ^= address bits 7..; the box starts at a multiple of 8 rows' bytes)
 template <int ES, int COLS>
-__device__ __forceinline__ uint4 stage_read(uint32_t slab, int r, int c) {
+__device__ __forceinline__ uint32_t box_addr(uint32_t slab, int r, int c) {
   constexpr int kSpan = COLS * ES;
   static_assert(kSpan == 32 || kSpan == 64 || kSpan == 128, "swizzle span");
   const uint32_t lin = (uint32_t)(r * kSpan + c * ES);
-  const uint32_t addr = slab + (lin ^ (((lin >> 7) & (kSpan / 16 - 1)) << 4));
+  return slab + (lin ^ (((lin >> 7) & (kSpan / 16 - 1)) << 4));
+}
+// 4 elements at (r, c) of a [64][cols] box as TMA wrote it
+// (volatile: stays behind the slot's full-barrier wait)
+template <int ES, int COLS>
+__device__ __forceinline__ uint4 stage_read(uint32_t slab, int r, int c) {
+  const uint32_t addr = box_addr<ES, COLS>(slab, r, c);
   uint4 v = make_uint4(0u, 0u, 0u, 0u);
   if constexpr (ES == 4)
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
@@ -306,28 +328,75 @@ __device__ __forceinline__ uint4 stage_read(uint32_t slab, int r, int c) {
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
   return v;
 }
-// The epilogue's own global operands (stashes written passes ago: always DRAM misses) are loaded right before use.
-// Functors with `l2_prefetch(m0, n0, bn, M, et, nth)` get the chance to pull the operand lines of the consumer
-// warpgroup's NEXT row tile into L2 a whole tile ahead (thread et of nth epilogue threads).
-template <int ES>   // element size in bytes; [rows][ld] row-major array, tile rows [m0, m0 + 64) x columns [n0, n0 + bn)
-__device__ __forceinline__ void l2_prefetch_tile(const void* base, int ld, int ncols, int m0, int n0, int bn, int M,
-                                                 int et, int nth) {
-  constexpr int kPerLine = 128 / ES;
-  const int lpr = (bn + kPerLine - 1) / kPerLine;
-  for (int i = et; i < kNtBM * lpr; i += nth) {
-    const int row = m0 + i / lpr, col = n0 + (i % lpr) * kPerLine;
-    if (row < M && col < ncols)
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(base) + ((size_t)row * ld + col) * ES));
-  }
-}
+
+// Ring-stored epilogue outputs.  A functor with a nested `using Out = tc::Outs<ES0, ES1, ...>` (element sizes in bytes: 4
+// fp32, 2 bf16) has the NT tiles send its outputs through the consumer's epilogue ring and TMA bulk stores instead of
+// register stores:
+//   tc::OutOp out_op(int i, int N) const       (host) output i of a GEMM N columns wide: [rows][ld] array and column
+//                                              extent; base nullptr: not stored
+//   void ring(row, col, acc[, aux], const S& s) const    operator()'s arithmetic, handing the values of the 4 columns
+//                                              to s.f32(i, v) or s.split(i, v) (bf16 hi to output i, lo to output i + 1)
+// Each warp owns 16 rows of the 64-row tile and its own part of every slot, [output][16 rows][kCols], and stores it
+// with boxes of 16 rows x kCols.  Rows >= M and columns past an output's extent are not written (TMA bounds), so the
+// extents restate which columns the functor's global path writes.  Columns < N go through ring(), groups wholly at
+// columns >= N are zeros.
+template <int... ES>
+struct Outs {
+  static constexpr int kN = sizeof...(ES);
+  static constexpr int kColBytes = (ES + ...);
+  __host__ __device__ static constexpr int es(int i) { int k = 0, r = 0; ((r = (k++ == i ? ES : r)), ...); return r; }
+  __host__ __device__ static constexpr int before(int i) { int k = 0, r = 0; ((r += (k++ < i ? ES : 0)), ...); return r; }
+};
+struct OutOp { const void* base; int ld; int cols; };
 template <typename E, typename = void>
-struct EpiL2 {
-  static __device__ __forceinline__ void run(const E&, int, int, int, int, int, int) {}
+struct EpiOut {
+  static constexpr int kN = 0, kSlotBytes = 0;
 };
 template <typename E>
-struct EpiL2<E, std::void_t<decltype(&E::l2_prefetch)>> {
-  static __device__ __forceinline__ void run(const E& e, int m0, int n0, int bn, int M, int et, int nth) {
-    if (m0 < M) e.l2_prefetch(m0, n0, bn, M, et, nth);
+struct EpiOut<E, std::void_t<typename E::Out>> {
+  using O = typename E::Out;
+  static_assert(EpiStage<E>::kN == 0, "a functor stages its operands or ring-stores its outputs, not both");
+  static constexpr int kN = O::kN, kSlotBytes = kNtBM * EpiBatch<E, true>::kCols * O::kColBytes;
+};
+// TMA bounds the columns of a store in whole 16-byte units (it writes past an extent up to the next 16 bytes), so a
+// launch whose stored outputs do not all end on 16 bytes keeps the functor's register stores (RING = false).
+// (measured on an H100: with an extent of 217 bf16 columns, a store box wrote through column 223, and with 217 fp32
+// columns through column 219)
+template <int N>
+struct EpiOutMaps { CUtensorMap m[N]; };      // per output: its tensor map (box 16 rows x kCols)
+template <>
+struct EpiOutMaps<0> {};
+// A thread's view of its warp's part of a ring slot: row r (0..15) of the warp's box, columns c..c+3 of the batch.
+// Outputs whose bit in `mask` is clear are not stored, so they are not written here either.
+template <typename O, int COLS>
+struct RingSink {
+  uint32_t box; int r, c; uint32_t mask;
+  __device__ __forceinline__ uint32_t at(int i) const {
+    const uint32_t slab = box + 16 * COLS * O::before(i);
+    return O::es(i) == 4 ? box_addr<4, COLS>(slab, r, c) : box_addr<2, COLS>(slab, r, c);
+  }
+  __device__ __forceinline__ void f32(int i, const float v[4]) const {
+    if (!((mask >> i) & 1u)) return;
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(at(i)), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
+  }
+  // the two-term bf16 split of v, rounded as split16_put4 rounds it
+  __device__ __forceinline__ void split(int i, const float v[4]) const {
+    if (!((mask >> i) & 3u)) return;
+    const uint32_t h01 = bf16x2_bits(v[0], v[1]), h23 = bf16x2_bits(v[2], v[3]);
+    const float r0 = v[0] - __uint_as_float(h01 << 16), r1 = v[1] - __uint_as_float(h01 & 0xffff0000u);
+    const float r2 = v[2] - __uint_as_float(h23 << 16), r3 = v[3] - __uint_as_float(h23 & 0xffff0000u);
+    if ((mask >> i) & 1u) asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(at(i)), "r"(h01), "r"(h23) : "memory");
+    if ((mask >> (i + 1)) & 1u)
+      asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(at(i + 1)), "r"(bf16x2_bits(r0, r1)), "r"(bf16x2_bits(r2, r3)) : "memory");
+  }
+  // a group wholly at columns >= N: zeros (they land only where an extent reaches past N, in a stash's padding)
+  __device__ __forceinline__ void zero() const {
+#pragma unroll
+    for (int i = 0; i < O::kN; ++i) {
+      if (!((mask >> i) & 1u)) continue;
+      if (O::es(i) == 4) asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(at(i)), "r"(0u) : "memory");
+      else asm volatile("st.shared.v2.u32 [%0], {%1, %1};" ::"r"(at(i)), "r"(0u) : "memory");
+    }
   }
 };
 
@@ -341,18 +410,24 @@ struct EpiL2<E, std::void_t<decltype(&E::l2_prefetch)>> {
 // stores, so that a memory round trip is always in flight under other work.
 // Staged functors (EpiStage) read their operands from the consumer's epilogue ring instead: batch b is chunk q0 + b of the
 // ring (one slot per batch), waited for on its full barrier and released to the loader after the batch's arithmetic.
+// Functors with ring-stored outputs (EpiOut) write batch b into chunk q0 + b of the ring, and each warp sends its part
+// of the slot out with TMA bulk stores (one bulk group per batch).  Before a warp rewrites a slot, its lane 0 waits
+// until the stores issued from that slot SLOTS batches ago have read it (`wait_group.read SLOTS - 1`): no barrier.
 struct EpiRing {
   uint32_t base;               // slot 0 of this consumer's ring (shared-memory address)
   uint32_t full0, empty0;      // mbarriers of slot 0 (8 bytes apart)
   int q0;                      // ring chunk counter of the tile's first batch
   int r, c;                    // this thread's row / first column inside a chunk
+  int m0, n0, wq;              // the tile's origin, the warp within the consumer warpgroup
+  uint32_t omask;              // ring-stored outputs that are stored (bit i: output i)
 };
-template <int BN, int SLOTS, typename Epi, typename MmaDone>
+template <int BN, int SLOTS, bool RING, typename Epi, typename OMaps, typename MmaDone>
 __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[BN / 2], int row, int col0, int M, int N,
-                                            int lane, MmaDone&& mma_done, const EpiRing& ring, long long& w_stage) {
+                                            int lane, MmaDone&& mma_done, const EpiRing& ring, const OMaps& omaps,
+                                            long long& w_stage, long long& w_drain) {
   using Tr = EpiTraits<Epi>;
   const bool odd = lane & 1;
-  constexpr int kB = EpiBatch<Epi>::kB, kNB = BN / 8 / kB;
+  constexpr int kB = EpiBatch<Epi, RING>::kB, kNB = BN / 8 / kB;
   auto group = [&](int j) {      // the 4-column group j of this thread's row (one exchange with lane ^ 1)
     const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
     const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
@@ -388,6 +463,50 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
       }
       __syncwarp();
       if ((lane & 31) == 0) mbar_arrive(ring.empty0 + 8 * s);      // one arrival per warp: the slot may be refilled
+    }
+  } else if constexpr (RING) {
+    using O = typename Epi::Out;
+    constexpr int kCols = EpiBatch<Epi, true>::kCols, kSlot = EpiOut<Epi>::kSlotBytes, kWarpBytes = 16 * kCols * O::kColBytes;
+    typename Tr::Aux aux[2][kB];
+    auto load = [&](int b) {
+#pragma unroll
+      for (int u = 0; u < kB; ++u) {
+        const int col = col0 + 8 * (kB * b + u);
+        if (row < M && col < N) aux[b & 1][u] = Tr::prefetch(epi, row, col);
+      }
+    };
+    load(0);
+    mma_done();
+#pragma unroll
+    for (int b = 0; b < kNB; ++b) {
+      if (b + 1 < kNB) load(b + 1);
+      const uint32_t box = ring.base + ((ring.q0 + b) % SLOTS) * kSlot + ring.wq * kWarpBytes;
+      if (lane == 0) {
+        AVC_PROBE(const long long t0 = clock64());
+        bulk_wait_read<SLOTS - 1>();
+        AVC_PROBE(w_drain += clock64() - t0);
+      }
+      __syncwarp();
+#pragma unroll
+      for (int u = 0; u < kB; ++u) {
+        const int j = kB * b + u;
+        const float4 v = group(j);
+        const int col = col0 + 8 * j;
+        const RingSink<O, kCols> sink{box, ring.r - 16 * ring.wq, ring.c + 8 * u, ring.omask};
+        if (row < M) {
+          if (col < N) Tr::ring(epi, row, col, v, aux[b & 1][u], sink);
+          else sink.zero();
+        }
+      }
+      fence_proxy_async();      // the generic-proxy writes above, before the async proxy reads them
+      __syncwarp();
+      if (lane == 0) {
+#pragma unroll
+        for (int i = 0; i < O::kN; ++i)
+          if ((ring.omask >> i) & 1u)
+            tma_store_2d(&omaps.m[i], box + 16 * kCols * O::before(i), ring.n0 + b * kCols, ring.m0 + 16 * ring.wq);
+        bulk_commit();
+      }
     }
   } else {
     typename Tr::Aux aux[2][kB];
@@ -429,14 +548,18 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
 // (TMA, box kCols x 64) into the consumer's epilogue ring (EPI_SLOTS slots, full / empty mbarriers), so that the
 // operands of a tile land while its MMAs run.  The ring chunk counter (tile j: (j / 2) * batches + b) gives both sides the
 // slot and its parity.
-template <int BN, int NPROD, bool RESB, typename Epi>
+// Functors with ring-stored outputs (EpiOut) use the same rings, without loaders or mbarriers: the consumers' warps write
+// their outputs into them and store them with TMA (omaps: one tensor map per output, omask: the outputs stored).
+template <int BN, int NPROD, bool RESB, typename Epi, bool RING = false>
 __global__ void __launch_bounds__(kNtThreads, 1)
 gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapBhi, const __grid_constant__ CUtensorMap mapBlo,
-                  int M, int N, int K, Epi epi, int b_const, const __grid_constant__ EpiMaps<EpiStage<Epi>::kN> emaps) {
-  using Cfg = TcCfg<BN, NPROD, RESB, EpiStage<Epi>::kSlotBytes>;
+                  int M, int N, int K, Epi epi, int b_const, const __grid_constant__ EpiMaps<EpiStage<Epi>::kN> emaps,
+                  const __grid_constant__ EpiOutMaps<EpiOut<Epi>::kN> omaps, uint32_t omask) {
+  static_assert(!RING || EpiOut<Epi>::kN > 0, "only functors with an Out ring-store");
+  using Cfg = TcCfg<BN, NPROD, RESB, RING ? EpiOut<Epi>::kSlotBytes : EpiStage<Epi>::kSlotBytes>;
   constexpr int kStaged = EpiStage<Epi>::kN;
-  constexpr int kEpiCols = EpiBatch<Epi>::kCols, kEpiNB = BN / kEpiCols;      // ring chunks per tile
+  constexpr int kEpiCols = EpiBatch<Epi, RING>::kCols, kEpiNB = BN / kEpiCols;      // ring chunks per tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B wants 1024-B tiles
   // stages, then the resident B panel, then the two epilogue rings
@@ -468,6 +591,10 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
     if constexpr (kStaged > 0) {
       for (int i = 0; i < kStaged; ++i) tma_prefetch_desc(&emaps.m[i]);
       for (int s = 0; s < 2 * Cfg::EPI_SLOTS; ++s) { mbar_init(efull0 + 8 * s, 1); mbar_init(eempty0 + 8 * s, 4); }
+    }
+    if constexpr (RING) {
+      for (int i = 0; i < EpiOut<Epi>::kN; ++i)
+        if ((omask >> i) & 1u) tma_prefetch_desc(&omaps.m[i]);
     }
     fence_barrier_init();
   }
@@ -541,14 +668,12 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   const int row_in = 16 * wq + (lane >> 2) + 8 * (lane & 1), col_in = 4 * ((lane >> 1) & 1);
   pdl_wait();      // the functor's operands and outputs belong to predecessor kernels
   float acc[BN / 2];
-  long long w_stage = 0;      // (probe build) waits on the epilogue ring
+  long long w_stage = 0, w_drain = 0;      // (probe build) waits on the epilogue ring, on the TMA stores' reads
   EpiRing ring{smem_base + kEpiOff + c * Cfg::EPI_SLOTS * Cfg::SLOT_BYTES, efull0 + 8 * c * Cfg::EPI_SLOTS,
-               eempty0 + 8 * c * Cfg::EPI_SLOTS, 0, row_in, col_in};
+               eempty0 + 8 * c * Cfg::EPI_SLOTS, 0, row_in, col_in, 0, n0, wq, omask};
   AVC_PROBE(long long w_full = 0, w_turn = 0, t_mma = 0, t_epi = 0; const long long t_loop0 = clock64());
-  EpiL2<Epi>::run(epi, (m_first + c * m_stride) * kNtBM, n0, BN, M, tw, 128);
   for (int j = c; j < n_tiles; j += 2) {
     const int m0 = (m_first + j * m_stride) * kNtBM;
-    EpiL2<Epi>::run(epi, m0 + 2 * m_stride * kNtBM, n0, BN, M, tw, 128);      // this warpgroup's next tile
     AVC_PROBE(const long long t_turn0 = clock64());
     if (j > 0) named_bar_sync(kNtTurnBar + c, 256);      // the other warpgroup has issued tile j - 1
     AVC_PROBE(const long long t_mma0 = clock64(); w_turn += t_mma0 - t_turn0);
@@ -582,7 +707,8 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
     }
     if (j + 1 < n_tiles) named_bar_arrive(kNtTurnBar + (c ^ 1), 256);      // all k-blocks issued: the other's turn
     ring.q0 = (j >> 1) * kEpiNB;
-    epilogue_nt<BN, Cfg::EPI_SLOTS>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane, [&] {
+    ring.m0 = m0;
+    epilogue_nt<BN, Cfg::EPI_SLOTS, RING>(epi, acc, m0 + row_in, n0 + col_in, M, N, lane, [&] {
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       if (leader) {
@@ -590,12 +716,16 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
         mbar_arrive(empty0 + 8 * last);
       }
       AVC_PROBE(t_mma += clock64() - t_mma0);
-    }, ring, w_stage);
+    }, ring, omaps, w_stage, w_drain);
     AVC_PROBE(t_epi += clock64() - t_mma0);
   }
-  (void)w_stage;
+  if constexpr (RING) {
+    if (lane == 0) bulk_wait_all();      // the outputs are written before the CTA exits (and its shared memory goes)
+  }
+  (void)w_stage; (void)w_drain;
   AVC_PROBE(if (leader) {
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 8, w_stage);
+    AVC_PROBE_ADD(EpiProbeId<Epi>::value, 9, w_drain);
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 2, w_full);
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 3, w_turn);
     AVC_PROBE_ADD(EpiProbeId<Epi>::value, 4, t_mma);
@@ -604,29 +734,12 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   })
 }
 
-template <int BN, int NPROD, bool RESB, typename Epi>
-static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K, const SplitPtr& A, const SplitPtr& B,
-                                       const Epi& epi, bool b_const) {
-  using Cfg = TcCfg<BN, NPROD, RESB, EpiStage<Epi>::kSlotBytes>;
-  EpiMaps<EpiStage<Epi>::kN> emaps;
-  if constexpr (EpiStage<Epi>::kN > 0) {
-    for (int i = 0; i < EpiStage<Epi>::kN; ++i) {
-      const StageOp op = epi.stage_op(i);
-      if (!op.base) return AVC_E_BADCFG;
-      AVC_TRY(make_map_rows_cached(&emaps.m[i], Epi::Stage::es(i), op.base, (uint64_t)M, (uint64_t)op.cols,
-                                   (uint64_t)op.ld, EpiBatch<Epi>::kCols, kNtBM));
-    }
-  }
-  CUtensorMap mAh, mAl, mBh, mBl;
-  AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
-  AVC_TRY(make_map_bf16_cached(&mBh, B.hi, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
-  if (NPROD == 3) {
-    AVC_TRY(make_map_bf16_cached(&mAl, A.lo, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
-    AVC_TRY(make_map_bf16_cached(&mBl, B.lo, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
-  } else {
-    mAl = mAh; mBl = mBh;
-  }
-  auto kern = gemm_tc_nt_kernel<BN, NPROD, RESB, Epi>;
+template <int BN, int NPROD, bool RESB, typename Epi, bool RING>
+static inline int launch_gemm_tc_nt_kern(cudaStream_t st, int64_t M, int N, int K, const CUtensorMap (&mab)[4],
+                                         const Epi& epi, bool b_const, const EpiMaps<EpiStage<Epi>::kN>& emaps,
+                                         const EpiOutMaps<EpiOut<Epi>::kN>& omaps, uint32_t omask) {
+  using Cfg = TcCfg<BN, NPROD, RESB, RING ? EpiOut<Epi>::kSlotBytes : EpiStage<Epi>::kSlotBytes>;
+  auto kern = gemm_tc_nt_kernel<BN, NPROD, RESB, Epi, RING>;
   static thread_local bool attr_set = false;    // per template instantiation and host thread (= device)
   if (!attr_set) {
     AVC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -644,9 +757,56 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
   g = (g / tiles_n) * tiles_n;                         // ... and a whole number of CTAs per column tile
   if (g < tiles_n) return AVC_E_BADCFG;
   dim3 grid(g);
-  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kNtThreads), (size_t)Cfg::SMEM_BYTES, st, mAh, mAl, mBh, mBl, (int)M, N, K, epi, b_const ? 1 : 0, emaps));
+  AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kNtThreads), (size_t)Cfg::SMEM_BYTES, st, mab[0], mab[1], mab[2], mab[3],
+                          (int)M, N, K, epi, b_const ? 1 : 0, emaps, omaps, omask));
   AVC_LAUNCH_TRY();
   return 0;
+}
+
+// 1: the last NT launch of this host thread stored its outputs through the ring, 0: from registers (read by the tests)
+inline thread_local int g_nt_last_ring = -1;
+
+template <int BN, int NPROD, bool RESB, typename Epi>
+static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K, const SplitPtr& A, const SplitPtr& B,
+                                       const Epi& epi, bool b_const) {
+  EpiMaps<EpiStage<Epi>::kN> emaps;
+  if constexpr (EpiStage<Epi>::kN > 0) {
+    for (int i = 0; i < EpiStage<Epi>::kN; ++i) {
+      const StageOp op = epi.stage_op(i);
+      if (!op.base) return AVC_E_BADCFG;
+      AVC_TRY(make_map_rows_cached(&emaps.m[i], Epi::Stage::es(i), op.base, (uint64_t)M, (uint64_t)op.cols,
+                                   (uint64_t)op.ld, EpiBatch<Epi>::kCols, kNtBM));
+    }
+  }
+  EpiOutMaps<EpiOut<Epi>::kN> omaps{};
+  uint32_t omask = 0;
+  bool ring = false;
+  if constexpr (EpiOut<Epi>::kN > 0) {
+    ring = true;
+    for (int i = 0; i < EpiOut<Epi>::kN; ++i) {
+      const OutOp op = epi.out_op(i, N);
+      if (!op.base) continue;
+      const int es = Epi::Out::es(i);      // TMA addresses whole 16 bytes: base, row pitch and extent
+      if (((uintptr_t)op.base & 15u) || (op.ld * es) % 16 || (op.cols * es) % 16) { ring = false; break; }
+      AVC_TRY(make_map_rows_cached(&omaps.m[i], Epi::Out::es(i), op.base, (uint64_t)M, (uint64_t)op.cols,
+                                   (uint64_t)op.ld, EpiBatch<Epi, true>::kCols, 16));      // one warp's box
+      omask |= 1u << i;
+    }
+  }
+  CUtensorMap mab[4];
+  AVC_TRY(make_map_bf16_cached(&mab[0], A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
+  AVC_TRY(make_map_bf16_cached(&mab[2], B.hi, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
+  if (NPROD == 3) {
+    AVC_TRY(make_map_bf16_cached(&mab[1], A.lo, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
+    AVC_TRY(make_map_bf16_cached(&mab[3], B.lo, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
+  } else {
+    mab[1] = mab[0]; mab[3] = mab[2];
+  }
+  g_nt_last_ring = ring ? 1 : 0;
+  if constexpr (EpiOut<Epi>::kN > 0) {
+    if (ring) return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, true>(st, M, N, K, mab, epi, b_const, emaps, omaps, omask);
+  }
+  return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, false>(st, M, N, K, mab, epi, b_const, emaps, omaps, 0);
 }
 
 // N <= 64 -> one 64-wide tile, else 128-wide tiles (a 65536-row GEMM then has 1024 tiles = 7.8 waves over 132

@@ -667,7 +667,16 @@ const char* avc_build_arch(void) { return "sm_90a"; }
 //   kind 3  EpiChain     Nprev = Nv, D1prev = X, s -> qt_prev = OUT [M][ldx]; ge = OUT2 [M][ld2] += the columns >= Nv
 //   kind 4  EpiDgradRelu mask from the bf16 hi half of X -> OUT [M][ldx]
 //   kind 5  EpiGe        ge = OUT2 [M][ld2] += acc
-// workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes.
+// The functors below write an fp32 copy to OUT [M][ldx] and the bf16 split of it into OUT2, read as a bf16 array
+// [M][2 ld2]: hi in columns [0, ld2), lo in columns [ld2, 2 ld2) of each row.
+//   kind 6  EpiValue<true>  bias = v1 [N], oscale = s -> sp' stash D1 = Y [M][ldx] (padding written), OUT, split
+//   kind 7  EpiBias         bias = v1 -> OUT, split
+//   kind 8  EpiColor0       bias = v1, cin = X [M][8], WxT = v2 [6][ldx] -> OUT, split
+//   kind 9  EpiRelu         bias = v1 -> OUT, split
+//   kind 10 EpiStore        -> OUT, split
+//   kind 11 EpiDgradRelu    as kind 4, and the split (the mask is read at the split's pitch, 2 ld2)
+//   kinds 108..111          kinds 8..11 with one bf16 product on the hi halves (NPROD = 1)
+// workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes (kind 11: + 8 * M * ld2 instead of 4 * M * ldx).
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
                     float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
@@ -679,14 +688,15 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
   __nv_bfloat16* al = cv.take<__nv_bfloat16>(M * ld);
   __nv_bfloat16* bh = cv.take<__nv_bfloat16>((int64_t)N * ld);
   __nv_bfloat16* bl = cv.take<__nv_bfloat16>((int64_t)N * ld);
-  __nv_bfloat16* xh = cv.take<__nv_bfloat16>(M * ldx);
-  __nv_bfloat16* xl = cv.take<__nv_bfloat16>(M * ldx);
+  const int ldm = kind % 100 == 11 ? 2 * ld2 : ldx;      // EpiDgradRelu reads its mask at the pitch of its split output
+  __nv_bfloat16* xh = cv.take<__nv_bfloat16>(M * ldm);
+  __nv_bfloat16* xl = cv.take<__nv_bfloat16>(M * ldm);
   if (cv.used() > workspace_bytes) return AVC_E_SIZE;
   cudaStream_t st = (cudaStream_t)stream;
   tc::k_split_bf16<<<blocks_for(M * ld, 256), 256, 0, st>>>(A, M, K, K, ah, al, ld);
   tc::k_split_bf16<<<blocks_for((int64_t)N * ld, 256), 256, 0, st>>>(B, N, K, K, bh, bl, ld);
   const float* xs = kind == 0 ? Y : X;      // the operand that is read as a bf16 pair
-  if (kind == 0 || kind == 4) tc::k_split_bf16<<<blocks_for(M * ldx, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldx);
+  if (kind == 0 || kind == 4 || kind % 100 == 11) tc::k_split_bf16<<<blocks_for(M * ldm, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldm);
   AVC_LAUNCH_TRY();
   const tc::SplitPtr a{ah, al, ld}, b{bh, bl, ld};
   const Split16 none{nullptr, nullptr, ldx};
@@ -718,6 +728,42 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
     case 5: {
       EpiGe e{OUT2, ld2, N};
       return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+  }
+  // kinds 108..111: 8..11 with one bf16 product (the colour net at color_products = 1)
+  const bool np1 = kind >= 108 && kind <= 111;
+  if (np1) kind -= 100;
+  if (kind < 6 || kind > 11) return AVC_E_BADCFG;
+  auto launch_color = [&](const auto& e) {
+    return np1 ? tc::launch_gemm_tc_nt<1>(st, M, N, K, a, b, e) : tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+  };
+  if (!OUT2 || (!v1 && kind != 10 && kind != 11)) return AVC_E_NULL;
+  __nv_bfloat16* o16 = reinterpret_cast<__nv_bfloat16*>(OUT2);
+  const Split16 split{o16, o16 + ld2, 2 * ld2};
+  switch (kind) {
+    case 6: {
+      EpiValue<true> e{v1, Y, ldx, OUT, ldx, s, N, split};
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    case 7: {
+      EpiBias e{v1, OUT, ldx, N, split};
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    case 8: {
+      EpiColor0 e{v1, X, v2, ldx, OUT, ldx, split};
+      return launch_color(e);
+    }
+    case 9: {
+      EpiRelu e{v1, OUT, ldx, split};
+      return launch_color(e);
+    }
+    case 10: {
+      EpiStore e{OUT, ldx, N, split};
+      return launch_color(e);
+    }
+    case 11: {
+      EpiDgradRelu e{nullptr, xh, OUT, ldx, Split16{o16, o16 + ld2, 2 * ld2}};
+      return launch_color(e);
     }
   }
   return AVC_E_BADCFG;

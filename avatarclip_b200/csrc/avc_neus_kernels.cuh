@@ -688,6 +688,13 @@ __global__ void k_heads_dgrad(const float* __restrict__ y6bar, const float* __re
 #define AVC_EPI_DIRECT \
   __device__ __forceinline__ void operator()(int row, int col, float4 a) const { (*this)(row, col, a, prefetch(row, col)); }
 
+// Ring-stored outputs (avc_gemm_tc.cuh) of the functors that write an fp32 copy and its split in whole 4-column groups
+// (every group with col < n): output 0 the fp32 copy, outputs 1 / 2 the hi / lo halves, extent n rounded up to 4.
+inline tc::OutOp epi_group_out(int i, float* out, int ldo, const Split16& s, int n) {
+  const int cols = (n + 3) & ~3;
+  return i == 0 ? tc::OutOp{out, ldo, cols} : tc::OutOp{i == 1 ? s.hi : s.lo, s.ld, cols};
+}
+
 // start of the last whole 4-column group below n, or `col` when that is smaller: an always-valid prefetch address
 __device__ __forceinline__ int clamp_group(int col, int n) { return max(0, min(col, (n - 4) & ~3)); }
 
@@ -707,16 +714,32 @@ struct EpiValue {
   const float* bias; float* D1; int ldz; float* OUT; int ldo; float oscale; int N; Split16 o16;
   struct Aux { float4 b; };
   __device__ __forceinline__ Aux prefetch(int, int col) const { return {load4_guarded(bias, col, N)}; }
-  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+  __device__ __forceinline__ void vals(int col, float4 a, const Aux& x, float hh[4], float dd[4]) const {
     AVC_EPI_UNPACK;
     const float bb[4] = {x.b.x, x.b.y, x.b.z, x.b.w};
-    float dd[4], hh[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       softplus100_both<FAST>(v[i] + bb[i], &hh[i], &dd[i]);
       hh[i] *= oscale;
       if (col + i >= N) { hh[i] = 0.f; dd[i] = 0.f; }
     }
+  }
+  // the NT tiles ring-store D1 (the whole padded width: its padding is zero), OUT and its split (columns < N: the rest
+  // of a skip layer's input row is the encoding, written by k_encode_fine)
+  using Out = tc::Outs<4, 4, 2, 2>;
+  tc::OutOp out_op(int i, int) const {
+    return i == 0 ? tc::OutOp{D1, ldz, ldz} : i == 1 ? tc::OutOp{OUT, ldo, N}
+                                                     : tc::OutOp{i == 2 ? o16.hi : o16.lo, o16.ld, N};
+  }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int col, float4 a, const Aux& x, const S& s) const {
+    float dd[4], hh[4];
+    vals(col, a, x, hh, dd);
+    s.f32(0, dd); s.f32(1, hh); s.split(2, hh);
+  }
+  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+    float dd[4], hh[4];
+    vals(col, a, x, hh, dd);
     if (D1) *reinterpret_cast<float4*>(D1 + (size_t)row * ldz + col) = make_float4(dd[0], dd[1], dd[2], dd[3]);
     if (col + 3 < N) {
       if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ldo + col) = make_float4(hh[0], hh[1], hh[2], hh[3]);
@@ -737,11 +760,22 @@ struct EpiBias {
   const float* bias; float* OUT; int ldo; int N; Split16 o16;
   struct Aux { float4 b; };
   __device__ __forceinline__ Aux prefetch(int, int col) const { return {load4_guarded(bias, col, N)}; }
-  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
-    AVC_EPI_UNPACK;
-    const float bb[4] = {x.b.x, x.b.y, x.b.z, x.b.w};
+  __device__ __forceinline__ void vals(int col, float4 a, const Aux& x, float v[4]) const {
+    const float aa[4] = {a.x, a.y, a.z, a.w}, bb[4] = {x.b.x, x.b.y, x.b.z, x.b.w};
 #pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] = (col + i < N) ? v[i] + bb[i] : 0.f;
+    for (int i = 0; i < 4; ++i) v[i] = (col + i < N) ? aa[i] + bb[i] : 0.f;
+  }
+  using Out = tc::Outs<4, 2, 2>;
+  tc::OutOp out_op(int i, int n) const { return epi_group_out(i, OUT, ldo, o16, n); }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int col, float4 a, const Aux& x, const S& s) const {
+    float v[4];
+    vals(col, a, x, v);
+    s.f32(0, v); s.split(1, v);
+  }
+  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+    float v[4];
+    vals(col, a, x, v);
     if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
     split16_put4(o16, (size_t)row, col, v);
   }
@@ -807,6 +841,15 @@ struct EpiGe {
     for (int i = 0; i < 4; ++i)
       if (col + i < E) GE[(size_t)row * EP + col + i] = gg[i] + v[i];
   }
+  // The NT tiles ring-store ge over its padded width EP: a padding column gets ge + acc = ge back (acc is 0 at columns
+  // >= E = N, whose B rows TMA reads as zeros), so only the columns < E change, as on the register path.
+  using Out = tc::Outs<4>;
+  tc::OutOp out_op(int, int) const { return {GE, EP, EP}; }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int, float4 a, const Aux& x, const S& s) const {
+    const float v[4] = {x.g.x + a.x, x.g.y + a.y, x.g.z + a.z, x.g.w + a.w};
+    s.f32(0, v);
+  }
   AVC_EPI_DIRECT
 };
 
@@ -819,8 +862,8 @@ struct EpiColor0 {
   __device__ __forceinline__ Aux prefetch(int row, int) const {
     return {*reinterpret_cast<const float4*>(cin + (size_t)row * 8), *reinterpret_cast<const float4*>(cin + (size_t)row * 8 + 4)};
   }
-  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
-    AVC_EPI_UNPACK;
+  __device__ __forceinline__ void vals(int col, float4 a, const Aux& x, float v[4]) const {
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
     const float cj[6] = {x.c0.x, x.c0.y, x.c0.z, x.c0.w, x.c1.x, x.c1.y};
 #pragma unroll
     for (int i = 0; i < 4; ++i) v[i] += bias[col + i];
@@ -832,6 +875,11 @@ struct EpiColor0 {
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) v[i] = fmaxf(v[i], 0.f);
+  }
+  // (not ring-stored: with the ring path the NT tiles spill a few registers at BN = 128)
+  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+    float v[4];
+    vals(col, a, x, v);
     if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
     split16_put4(o16, (size_t)row, col, v);
   }
@@ -845,10 +893,21 @@ struct EpiRelu {
   __device__ __forceinline__ Aux prefetch(int, int col) const {
     return {make_float4(bias[col], bias[col + 1], bias[col + 2], bias[col + 3])};
   }
+  __device__ __forceinline__ static void vals(float4 a, const Aux& x, float v[4]) {
+    v[0] = fmaxf(a.x + x.b.x, 0.f); v[1] = fmaxf(a.y + x.b.y, 0.f);
+    v[2] = fmaxf(a.z + x.b.z, 0.f); v[3] = fmaxf(a.w + x.b.w, 0.f);
+  }
+  using Out = tc::Outs<4, 2, 2>;
+  tc::OutOp out_op(int i, int n) const { return epi_group_out(i, OUT, ldo, o16, n); }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int, float4 a, const Aux& x, const S& s) const {
+    float v[4];
+    vals(a, x, v);
+    s.f32(0, v); s.split(1, v);
+  }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
-    AVC_EPI_UNPACK;
-    v[0] = fmaxf(v[0] + x.b.x, 0.f); v[1] = fmaxf(v[1] + x.b.y, 0.f);
-    v[2] = fmaxf(v[2] + x.b.z, 0.f); v[3] = fmaxf(v[3] + x.b.w, 0.f);
+    float v[4];
+    vals(a, x, v);
     if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
     split16_put4(o16, (size_t)row, col, v);
   }
@@ -866,12 +925,22 @@ struct EpiDgradRelu {
     const uint2 h = *reinterpret_cast<const uint2*>(Hhi + (size_t)row * o16.ld + col);
     return {make_uint4(h.x, h.y, 0u, 0u)};
   }
-  __device__ __forceinline__ void l2_prefetch(int m0, int n0, int bn, int M, int et, int nth) const {
-    if (Hm) tc::l2_prefetch_tile<4>(Hm, ld, ld, m0, n0, bn, M, et, nth);
-    else tc::l2_prefetch_tile<2>(Hhi, o16.ld, o16.ld, m0, n0, bn, M, et, nth);
+  using Out = tc::Outs<4, 2, 2>;
+  tc::OutOp out_op(int i, int n) const { return epi_group_out(i, OUT, ld, o16, n); }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int, float4 a, const Aux& x, const S& s) const {
+    float v[4];
+    vals(a, x, v);
+    s.f32(0, v); s.split(1, v);
   }
   __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
-    AVC_EPI_UNPACK;
+    float v[4];
+    vals(a, x, v);
+    if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ld + col) = make_float4(v[0], v[1], v[2], v[3]);
+    split16_put4(o16, (size_t)row, col, v);
+  }
+  __device__ __forceinline__ void vals(float4 a, const Aux& x, float v[4]) const {
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
     bool on[4];
     if (Hm) {
       on[0] = __uint_as_float(x.raw.x) > 0.f; on[1] = __uint_as_float(x.raw.y) > 0.f;
@@ -882,8 +951,6 @@ struct EpiDgradRelu {
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) v[i] = on[i] ? v[i] : 0.f;
-    if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ld + col) = make_float4(v[0], v[1], v[2], v[3]);
-    split16_put4(o16, (size_t)row, col, v);
   }
   AVC_EPI_DIRECT
 };
@@ -891,10 +958,22 @@ struct EpiDgradRelu {
 struct EpiStore {
   static constexpr int kProbeId = 8;      // slot of the optional NT stall probe (avc_gemm_tc.cuh)
   float* OUT; int ldo; int N; Split16 o16;
-  __device__ __forceinline__ void operator()(int row, int col, float4 a) const {
-    AVC_EPI_UNPACK;
+  __device__ __forceinline__ void vals(int col, float4 a, float v[4]) const {
+    const float aa[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] = (col + i < N) ? v[i] : 0.f;
+    for (int i = 0; i < 4; ++i) v[i] = (col + i < N) ? aa[i] : 0.f;
+  }
+  using Out = tc::Outs<4, 2, 2>;
+  tc::OutOp out_op(int i, int n) const { return epi_group_out(i, OUT, ldo, o16, n); }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int col, float4 a, const S& s) const {
+    float v[4];
+    vals(col, a, v);
+    s.f32(0, v); s.split(1, v);
+  }
+  __device__ __forceinline__ void operator()(int row, int col, float4 a) const {
+    float v[4];
+    vals(col, a, v);
     if (OUT) *reinterpret_cast<float4*>(OUT + (size_t)row * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
     split16_put4(o16, (size_t)row, col, v);
   }

@@ -10,6 +10,14 @@ struct EpiPlainStore {
     float v[4] = {a.x, a.y, a.z, a.w};
     for (int i = 0; i < 4 && col + i < N; ++i) C[(size_t)row * ldc + col + i] = v[i];
   }
+  // ring-stored when C's rows are whole 16 bytes (N % 4 == 0), else from registers
+  using Out = tc::Outs<4>;
+  tc::OutOp out_op(int, int) const { return {C, ldc, N}; }
+  template <typename S>
+  __device__ void ring(int, int, float4 a, const S& s) const {
+    const float v[4] = {a.x, a.y, a.z, a.w};
+    s.f32(0, v);
+  }
 };
 }  // namespace
 
@@ -59,5 +67,9 @@ int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, i
   if (nprod == 3) return tc::launch_gemm_tc_tn<3>(st, P, N1, N2, a, b, C, N2, colsum);
   return tc::launch_gemm_tc_tn<1>(st, P, N1, N2, a, b, C, N2, colsum);
 }
+
+// 1: the last wgmma NT launch of the calling host thread stored its outputs with TMA through the epilogue ring, 0: from
+// registers, -1: none yet.
+int avc_tc_nt_last_ring(void) { return tc::g_nt_last_ring; }
 
 }  // extern "C"

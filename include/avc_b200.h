@@ -439,9 +439,14 @@ int avc_tc_gemm_nt_test(const float* A, const float* B, int64_t M, int32_t N, in
  * workspace >= 4 * P * (round_up(N1,8) + round_up(N2,8)) + 2048 bytes. */
 int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, int32_t N2, int32_t nprod,
                         float* C, float* colsum, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+/* 1: the last wgmma NT launch of the calling host thread stored its outputs with TMA bulk stores through the epilogue
+ * ring, 0: from registers, -1: no launch yet (the tests check which path a shape takes). */
+int avc_tc_nt_last_ring(void);
 /* The backward epilogue functors of the NeuS path through the NT tiles on caller data: kind 0 second-order sweep,
  * 1 / 2 value backward without / with the sdf term, 3 gradient chain, 4 ReLU-mask dgrad, 5 encoding-gradient
- * accumulation (argument roles in avc_neus.cu).  workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes. */
+ * accumulation; and with the bf16 split of their output: 6 value chain, 7 feature bias, 8 colour lin0, 9 ReLU,
+ * 10 plain store, 11 ReLU-mask dgrad, 108..111 as 8..11 with one bf16 product (argument roles in avc_neus.cu).
+ * workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes. */
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
                     float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream);
@@ -538,10 +543,10 @@ int avc_uniform_fill(uint32_t seed, int32_t n, float lo, float hi, float* out, a
  * [4] epilogue waiting for the accumulator, [5] epilogue work); this call synchronises the device and copies them. */
 int avc_chain_debug_read(long long* out8);
 /* Stall probe of the wgmma NT tiles: only in a diagnostic build (-DAVC_NT_PROBE=1, tools/nt_probe.py); a regular
- * build returns AVC_E_BADCFG.  host_out[16][9]: per epilogue functor the summed cycles {producer waiting for a free
+ * build returns AVC_E_BADCFG.  host_out[16][10]: per epilogue functor the summed cycles {producer waiting for a free
  * stage, producer loop, consumers waiting for operands, consumers waiting for their turn, consumers' MMAs, consumers'
- * epilogues, consumers' loops, CTAs, consumers waiting for staged epilogue operands} (consumer slots: both consumer
- * warpgroups); reset != 0 clears the counters. */
+ * epilogues, consumers' loops, CTAs, consumers waiting for staged epilogue operands, consumers waiting for their TMA
+ * stores to release a ring slot} (consumer slots: both consumer warpgroups); reset != 0 clears the counters. */
 int avc_nt_probe_read(unsigned long long* host_out, int reset);
 
 int avc_march_count(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, int32_t* counts,

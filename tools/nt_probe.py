@@ -4,15 +4,17 @@
                                           # avc_neus.cu recompiled with -DAVC_NT_PROBE=1
     python tools/nt_probe.py --run OUT    # on the GPU: a few steps of the bench workload through the probe build,
                                           # per epilogue functor where each warp role's loop time went
-    python tools/nt_probe.py --run OUT --lib OTHER.so --slots 8    # another probe build (8 slots: before the
-                                          # epilogue-ring slot existed)
+    python tools/nt_probe.py --run OUT --lib OTHER.so --slots 9    # another probe build (9 slots: before the
+                                          # store-drain slot existed, 8: before the epilogue-ring slot)
 
 The probe takes clock64 stamps in the TMA producer and in the leading thread of each consumer warpgroup: the producer's
 waits for a free stage, the consumers' waits for operands and for their turn at the tensor pipe, and the time from a
 consumer's turn to its MMAs' completion and from there to the end of its epilogue, summed per functor
 (avc_gemm_tc.cuh, AVC_NT_PROBE), and the consumers' waits for the epilogue operands staged in shared memory
-(`waits_staged`, functors with a `Stage`).  `busy_over_wall` is the MMA and epilogue time of both consumer warpgroups over the loop
-time of one: above 1, the two worked at the same time (one's MMAs under the other's epilogue)."""
+(`waits_staged`, functors with a `Stage`), and their waits for the TMA stores of a ring slot to have read it before they
+rewrite it (`waits_store_drain`, functors with an `Out`).  `busy_over_wall` is the MMA and epilogue time of both
+consumer warpgroups over the loop time of one: above 1, the two worked at the same time (one's MMAs under the other's
+epilogue)."""
 import argparse
 import ctypes as C
 import json
@@ -41,7 +43,7 @@ def build():
     print("built", PROBE_LIB)
 
 
-def run(out_path, lib=PROBE_LIB, slots=9):
+def run(out_path, lib=PROBE_LIB, slots=10):
     os.environ["AVC_B200_LIB"] = lib
     sys.path.insert(0, ROOT)
     import torch
@@ -67,7 +69,7 @@ def run(out_path, lib=PROBE_LIB, slots=9):
     assert L.avc_nt_probe_read(buf, 1) == 0
     rep = {}
     for i in range(16):
-        v = [buf[i * slots + j] for j in range(slots)] + [0] * (9 - slots)
+        v = [buf[i * slots + j] for j in range(slots)] + [0] * (10 - slots)
         if v[7] == 0:
             continue
         ctas = v[7]
@@ -78,7 +80,7 @@ def run(out_path, lib=PROBE_LIB, slots=9):
             "producer_waits_free_stage": v[0] / max(v[1], 1),
             # shares of a consumer warpgroup's loop; the MMA share includes its operand and B-panel waits
             "consumer": {"waits_operands": v[2] / cons, "waits_turn": v[3] / cons, "mma": v[4] / cons,
-                         "epilogue": v[5] / cons, "waits_staged": v[8] / cons},
+                         "epilogue": v[5] / cons, "waits_staged": v[8] / cons, "waits_store_drain": v[9] / cons},
             "busy_over_wall": (v[4] + v[5]) / (cons / 2),
         }
     with open(out_path, "w") as f:
@@ -91,7 +93,7 @@ if __name__ == "__main__":
     ap.add_argument("--build", action="store_true")
     ap.add_argument("--run", metavar="OUT")
     ap.add_argument("--lib", default=PROBE_LIB, help="probe build to load (default: the one --build makes)")
-    ap.add_argument("--slots", type=int, default=9, help="counters per functor of that build")
+    ap.add_argument("--slots", type=int, default=10, help="counters per functor of that build")
     a = ap.parse_args()
     if a.build:
         build()
