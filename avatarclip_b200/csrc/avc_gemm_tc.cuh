@@ -270,13 +270,18 @@ struct EpiTraits<E, std::void_t<typename E::Aux>> {
   template <typename S>
   static __device__ __forceinline__ void ring(const E& e, int r, int c, float4 a, const Aux& x, const S& s) { e.ring(r, c, a, x, s); }
 };
+template <typename E, typename = void>
+struct HasStage : std::false_type {};
+template <typename E>
+struct HasStage<E, std::void_t<typename E::Stage>> : std::true_type {};
 // groups of 8 columns per epilogue batch: two batches of global operands are live beside the accumulator; with 32-byte
 // operands (EpiChainBwd, EpiDgrad) batches of 4 need more registers than ptxas grants a 384-thread kernel and spill
 // (RING: outputs stored through the epilogue ring, EpiOut below: batches of 2, so that two slots per consumer fit beside
-// the B panel)
+// the B panel; staged functors, whose outputs are ring-stored over their staged operands, too: with batches of 4 the
+// ring stores of EpiChain spill)
 template <typename E, bool RING = false>
 struct EpiBatch {
-  static constexpr int kB = (RING || sizeof(typename EpiTraits<E>::Aux) > 16) ? 2 : 4;
+  static constexpr int kB = (RING || HasStage<E>::value || sizeof(typename EpiTraits<E>::Aux) > 16) ? 2 : 4;
   static constexpr int kCols = 8 * kB;
 };
 
@@ -309,12 +314,14 @@ template <>
 struct EpiMaps<0> {};
 // Address of the 4 elements at (r, c) of a [rows][COLS] box as TMA reads and writes it: rows of span = COLS * ES bytes,
 // swizzled over the span (16-byte unit bits 4.. ^= address bits 7..; the box starts at a multiple of 8 rows' bytes)
+__device__ __forceinline__ uint32_t box_addr(uint32_t slab, int r, int c, int es, int span) {
+  const uint32_t lin = (uint32_t)(r * span + c * es);
+  return slab + (lin ^ (((lin >> 7) & (span / 16 - 1)) << 4));
+}
 template <int ES, int COLS>
 __device__ __forceinline__ uint32_t box_addr(uint32_t slab, int r, int c) {
-  constexpr int kSpan = COLS * ES;
-  static_assert(kSpan == 32 || kSpan == 64 || kSpan == 128, "swizzle span");
-  const uint32_t lin = (uint32_t)(r * kSpan + c * ES);
-  return slab + (lin ^ (((lin >> 7) & (kSpan / 16 - 1)) << 4));
+  static_assert(COLS * ES == 32 || COLS * ES == 64 || COLS * ES == 128, "swizzle span");
+  return box_addr(slab, r, c, ES, COLS * ES);
 }
 // 4 elements at (r, c) of a [64][cols] box as TMA wrote it
 // (volatile: stays behind the slot's full-barrier wait)
@@ -340,6 +347,12 @@ __device__ __forceinline__ uint4 stage_read(uint32_t slab, int r, int c) {
 // with boxes of 16 rows x kCols.  Rows >= M and columns past an output's extent are not written (TMA bounds), so the
 // extents restate which columns the functor's global path writes.  Columns < N go through ring(), groups wholly at
 // columns >= N are zeros.
+// A staged functor (EpiStage) writes its outputs in place over its staged operands, so its slots need no extra bytes:
+//   static constexpr tc::Over over(int i)      output i overwrites the warp's 16 rows of staged operand `op`, `off` of
+//                                              its own boxes into them; with pieces = 2 it is stored as two boxes of
+//                                              kCols / 2 columns, over the warp's rows of operands op and op + 1
+// Outputs that would overlap cannot be stored by one launch: the host rejects them (AVC_E_BADCFG).
+struct Over { int op, off, pieces; };
 template <int... ES>
 struct Outs {
   static constexpr int kN = sizeof...(ES);
@@ -355,25 +368,72 @@ struct EpiOut {
 template <typename E>
 struct EpiOut<E, std::void_t<typename E::Out>> {
   using O = typename E::Out;
-  static_assert(EpiStage<E>::kN == 0, "a functor stages its operands or ring-stores its outputs, not both");
-  static constexpr int kN = O::kN, kSlotBytes = kNtBM * EpiBatch<E, true>::kCols * O::kColBytes;
+  static constexpr int kN = O::kN;
+  static constexpr int kSlotBytes = EpiStage<E>::kN ? EpiStage<E>::kSlotBytes : kNtBM * EpiBatch<E, true>::kCols * O::kColBytes;
+};
+// Where the boxes of the ring-stored outputs lie in a slot: output i is stored as pieces(i) boxes of 16 rows x cols(i),
+// piece p of warp wq at byte at(i, p, wq) of the slot.
+template <typename E, bool STAGED = (EpiStage<E>::kN > 0)>
+struct OutLayout {      // store-only functors: [warp][output][16 rows][kCols]
+  using O = typename E::Out;
+  static constexpr int kCols = EpiBatch<E, true>::kCols;
+  __host__ __device__ static constexpr int pieces(int) { return 1; }
+  __host__ __device__ static constexpr int cols(int) { return kCols; }
+  __host__ __device__ static constexpr int at(int i, int, int wq) { return 16 * kCols * (wq * O::kColBytes + O::before(i)); }
+};
+template <typename E>
+struct OutLayout<E, true> {      // staged functors: in place over the staged operands, [operand][4 warps][16 rows][kCols]
+  using O = typename E::Out;
+  using St = typename E::Stage;
+  static constexpr int kCols = EpiBatch<E>::kCols;
+  __host__ __device__ static constexpr int pieces(int i) { return E::over(i).pieces; }
+  __host__ __device__ static constexpr int cols(int i) { return kCols / pieces(i); }
+  __host__ __device__ static constexpr int box_bytes(int i) { return 16 * cols(i) * O::es(i); }
+  __host__ __device__ static constexpr int part(int k) { return 16 * kCols * St::es(k); }      // a warp's rows of operand k
+  __host__ __device__ static constexpr int at(int i, int p, int wq) {
+    const int k = E::over(i).op + p;
+    return kNtBM * kCols * St::before(k) + wq * part(k) + E::over(i).off * box_bytes(i);
+  }
+  // every box inside the warp's rows of its operand and on its swizzle period (8 rows of its span): box_addr's swizzle
+  // is the one TMA applies
+  static constexpr bool fits() {
+    for (int i = 0; i < O::kN; ++i) {
+      const int span = cols(i) * O::es(i), period = 8 * span;
+      if (span != 32 && span != 64 && span != 128) return false;
+      for (int p = 0; p < pieces(i); ++p) {
+        const int k = E::over(i).op + p;
+        if (k >= St::kN || (E::over(i).off + 1) * box_bytes(i) > part(k)) return false;
+        if ((kNtBM * kCols * St::before(k)) % period || part(k) % period || (E::over(i).off * box_bytes(i)) % period) return false;
+      }
+    }
+    return true;
+  }
+  static constexpr bool overlap(int i, int j) {
+    for (int p = 0; p < pieces(i); ++p)
+      for (int q = 0; q < pieces(j); ++q) {
+        const int a = at(i, p, 0), b = at(j, q, 0);
+        if (a < b + box_bytes(j) && b < a + box_bytes(i)) return true;
+      }
+    return false;
+  }
 };
 // TMA bounds the columns of a store in whole 16-byte units (it writes past an extent up to the next 16 bytes), so a
 // launch whose stored outputs do not all end on 16 bytes keeps the functor's register stores (RING = false).
 // (measured on an H100: with an extent of 217 bf16 columns, a store box wrote through column 223, and with 217 fp32
 // columns through column 219)
 template <int N>
-struct EpiOutMaps { CUtensorMap m[N]; };      // per output: its tensor map (box 16 rows x kCols)
+struct EpiOutMaps { CUtensorMap m[N]; };      // per output: its tensor map (box 16 rows x OutLayout::cols)
 template <>
 struct EpiOutMaps<0> {};
-// A thread's view of its warp's part of a ring slot: row r (0..15) of the warp's box, columns c..c+3 of the batch.
+// A thread's view of its warp's part of a ring slot: row r (0..15) of the warp's boxes, columns c..c+3 of the batch.
 // Outputs whose bit in `mask` is clear are not stored, so they are not written here either.
-template <typename O, int COLS>
+template <typename L>
 struct RingSink {
-  uint32_t box; int r, c; uint32_t mask;
+  using O = typename L::O;
+  uint32_t slot; int wq, r, c; uint32_t mask;
   __device__ __forceinline__ uint32_t at(int i) const {
-    const uint32_t slab = box + 16 * COLS * O::before(i);
-    return O::es(i) == 4 ? box_addr<4, COLS>(slab, r, c) : box_addr<2, COLS>(slab, r, c);
+    const int p = L::pieces(i) == 1 ? 0 : c / L::cols(i);
+    return box_addr(slot + L::at(i, p, wq), r, c - p * L::cols(i), O::es(i), L::cols(i) * O::es(i));
   }
   __device__ __forceinline__ void f32(int i, const float v[4]) const {
     if (!((mask >> i) & 1u)) return;
@@ -399,6 +459,18 @@ struct RingSink {
     }
   }
 };
+// (lane 0 of a warp) one TMA bulk store per piece of every stored output from the warp's boxes in `slot`, as one bulk
+// group; (x, y) = the global column and row of the boxes
+template <typename L, int N>
+__device__ __forceinline__ void ring_store(const EpiOutMaps<N>& omaps, uint32_t mask, uint32_t slot, int wq, int x, int y) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    if (!((mask >> i) & 1u)) continue;
+#pragma unroll
+    for (int p = 0; p < L::pieces(i); ++p) tma_store_2d(&omaps.m[i], slot + L::at(i, p, wq), x + p * L::cols(i), y);
+  }
+  bulk_commit();
+}
 
 // ------------------------------------------------------------------------------------------------ NT kernel
 // The accumulator fragment gives a thread column PAIRS of two rows r and r + 8 (avc_wgmma.cuh).  One exchange with the
@@ -409,7 +481,10 @@ struct RingSink {
 // before `mma_done()` (which waits for the accumulator), every later one before the previous batch's arithmetic and
 // stores, so that a memory round trip is always in flight under other work.
 // Staged functors (EpiStage) read their operands from the consumer's epilogue ring instead: batch b is chunk q0 + b of the
-// ring (one slot per batch), waited for on its full barrier and released to the loader after the batch's arithmetic.
+// ring (one slot per batch), waited for on its full barrier.  Each warp writes its outputs over its own 16 rows of the
+// operands it has just read (OutLayout) and stores them with TMA.  A slot goes back to its loader (one empty-barrier
+// arrival per warp) once the warp's stores have read it: after committing batch b, lane 0 waits until only that batch's
+// stores may still read (`wait_group.read 1`) and releases batch b - 1's slot; the tile's last slot after `read 0`.
 // Functors with ring-stored outputs (EpiOut) write batch b into chunk q0 + b of the ring, and each warp sends its part
 // of the slot out with TMA bulk stores (one bulk group per batch).  Before a warp rewrites a slot, its lane 0 waits
 // until the stores issued from that slot SLOTS batches ago have read it (`wait_group.read SLOTS - 1`): no barrier.
@@ -435,6 +510,7 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
   };
   if constexpr (EpiStage<Epi>::kN > 0) {
     using St = typename Epi::Stage;
+    using L = OutLayout<Epi>;
     constexpr int kCols = EpiBatch<Epi>::kCols, kSlot = EpiStage<Epi>::kSlotBytes;
     mma_done();
 #pragma unroll
@@ -454,19 +530,40 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
         }
         aux[u] = Epi::from_stage(raw);
       }
+      __syncwarp();      // the warp has read its operands before any lane writes its outputs over them
 #pragma unroll
       for (int u = 0; u < kB; ++u) {
         const int j = kB * b + u;
         const float4 v = group(j);
         const int col = col0 + 8 * j;
-        if (row < M && col < N) Tr::apply(epi, row, col, v, aux[u]);
+        const RingSink<L> sink{slot, ring.wq, ring.r - 16 * ring.wq, ring.c + 8 * u, ring.omask};
+        if (row < M) {
+          if (col < N) Tr::ring(epi, row, col, v, aux[u], sink);
+          else sink.zero();
+        }
       }
+      fence_proxy_async();      // the generic-proxy writes above, before the async proxy reads them
       __syncwarp();
-      if ((lane & 31) == 0) mbar_arrive(ring.empty0 + 8 * s);      // one arrival per warp: the slot may be refilled
+      if (lane == 0) {
+        ring_store<L>(omaps, ring.omask, slot, ring.wq, ring.n0 + b * kCols, ring.m0 + 16 * ring.wq);
+        // one arrival per warp: the previous batch's slot may be refilled once its stores have read it
+        if (b > 0) {
+          AVC_PROBE(const long long t0 = clock64());
+          bulk_wait_read<1>();
+          AVC_PROBE(w_drain += clock64() - t0);
+          mbar_arrive(ring.empty0 + 8 * ((q - 1) % SLOTS));
+        }
+      }
+    }
+    if (lane == 0) {      // the last slot goes back before the next tile's MMAs, during which its loader refills
+      AVC_PROBE(const long long t0 = clock64());
+      bulk_wait_read<0>();
+      AVC_PROBE(w_drain += clock64() - t0);
+      mbar_arrive(ring.empty0 + 8 * ((ring.q0 + kNB - 1) % SLOTS));
     }
   } else if constexpr (RING) {
-    using O = typename Epi::Out;
-    constexpr int kCols = EpiBatch<Epi, true>::kCols, kSlot = EpiOut<Epi>::kSlotBytes, kWarpBytes = 16 * kCols * O::kColBytes;
+    using L = OutLayout<Epi>;
+    constexpr int kCols = EpiBatch<Epi, true>::kCols, kSlot = EpiOut<Epi>::kSlotBytes;
     typename Tr::Aux aux[2][kB];
     auto load = [&](int b) {
 #pragma unroll
@@ -480,7 +577,8 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
 #pragma unroll
     for (int b = 0; b < kNB; ++b) {
       if (b + 1 < kNB) load(b + 1);
-      const uint32_t box = ring.base + ((ring.q0 + b) % SLOTS) * kSlot + ring.wq * kWarpBytes;
+      // the warp's part of the slot: its boxes at L::at(i, 0, 0) from there
+      const uint32_t box = ring.base + ((ring.q0 + b) % SLOTS) * kSlot + L::at(0, 0, ring.wq);
       if (lane == 0) {
         AVC_PROBE(const long long t0 = clock64());
         bulk_wait_read<SLOTS - 1>();
@@ -492,7 +590,7 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
         const int j = kB * b + u;
         const float4 v = group(j);
         const int col = col0 + 8 * j;
-        const RingSink<O, kCols> sink{box, ring.r - 16 * ring.wq, ring.c + 8 * u, ring.omask};
+        const RingSink<L> sink{box, 0, ring.r - 16 * ring.wq, ring.c + 8 * u, ring.omask};
         if (row < M) {
           if (col < N) Tr::ring(epi, row, col, v, aux[b & 1][u], sink);
           else sink.zero();
@@ -500,13 +598,7 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
       }
       fence_proxy_async();      // the generic-proxy writes above, before the async proxy reads them
       __syncwarp();
-      if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < O::kN; ++i)
-          if ((ring.omask >> i) & 1u)
-            tma_store_2d(&omaps.m[i], box + 16 * kCols * O::before(i), ring.n0 + b * kCols, ring.m0 + 16 * ring.wq);
-        bulk_commit();
-      }
+      if (lane == 0) ring_store<L>(omaps, ring.omask, box, 0, ring.n0 + b * kCols, ring.m0 + 16 * ring.wq);
     }
   } else {
     typename Tr::Aux aux[2][kB];
@@ -547,9 +639,10 @@ __device__ __forceinline__ void epilogue_nt(const Epi& epi, const float (&acc)[B
 // warpgroups 0 and 1.  Each walks its consumer's tiles and issues, batch by batch, one chunk of every staged operand
 // (TMA, box kCols x 64) into the consumer's epilogue ring (EPI_SLOTS slots, full / empty mbarriers), so that the
 // operands of a tile land while its MMAs run.  The ring chunk counter (tile j: (j / 2) * batches + b) gives both sides the
-// slot and its parity.
-// Functors with ring-stored outputs (EpiOut) use the same rings, without loaders or mbarriers: the consumers' warps write
-// their outputs into them and store them with TMA (omaps: one tensor map per output, omask: the outputs stored).
+// slot and its parity.  Their outputs are stored with TMA from the same slots, written over the operands.
+// Store-only functors with ring-stored outputs (EpiOut) use the same rings, without loaders or mbarriers: the consumers'
+// warps write their outputs into them and store them with TMA (omaps: one tensor map per output, omask: the outputs
+// stored).
 template <int BN, int NPROD, bool RESB, typename Epi, bool RING = false>
 __global__ void __launch_bounds__(kNtThreads, 1)
 gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
@@ -557,7 +650,8 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
                   int M, int N, int K, Epi epi, int b_const, const __grid_constant__ EpiMaps<EpiStage<Epi>::kN> emaps,
                   const __grid_constant__ EpiOutMaps<EpiOut<Epi>::kN> omaps, uint32_t omask) {
   static_assert(!RING || EpiOut<Epi>::kN > 0, "only functors with an Out ring-store");
-  using Cfg = TcCfg<BN, NPROD, RESB, RING ? EpiOut<Epi>::kSlotBytes : EpiStage<Epi>::kSlotBytes>;
+  static_assert(RING || EpiStage<Epi>::kN == 0, "staged functors ring-store their outputs");
+  using Cfg = TcCfg<BN, NPROD, RESB, RING ? EpiOut<Epi>::kSlotBytes : 0>;
   constexpr int kStaged = EpiStage<Epi>::kN;
   constexpr int kEpiCols = EpiBatch<Epi, RING>::kCols, kEpiNB = BN / kEpiCols;      // ring chunks per tile
   extern __shared__ uint8_t smem_raw[];
@@ -738,7 +832,7 @@ template <int BN, int NPROD, bool RESB, typename Epi, bool RING>
 static inline int launch_gemm_tc_nt_kern(cudaStream_t st, int64_t M, int N, int K, const CUtensorMap (&mab)[4],
                                          const Epi& epi, bool b_const, const EpiMaps<EpiStage<Epi>::kN>& emaps,
                                          const EpiOutMaps<EpiOut<Epi>::kN>& omaps, uint32_t omask) {
-  using Cfg = TcCfg<BN, NPROD, RESB, RING ? EpiOut<Epi>::kSlotBytes : EpiStage<Epi>::kSlotBytes>;
+  using Cfg = TcCfg<BN, NPROD, RESB, RING ? EpiOut<Epi>::kSlotBytes : 0>;
   auto kern = gemm_tc_nt_kernel<BN, NPROD, RESB, Epi, RING>;
   static thread_local bool attr_set = false;    // per template instantiation and host thread (= device)
   if (!attr_set) {
@@ -781,18 +875,30 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
   EpiOutMaps<EpiOut<Epi>::kN> omaps{};
   uint32_t omask = 0;
   bool ring = false;
+  constexpr bool kStaged = EpiStage<Epi>::kN > 0;
   if constexpr (EpiOut<Epi>::kN > 0) {
     ring = true;
     for (int i = 0; i < EpiOut<Epi>::kN; ++i) {
       const OutOp op = epi.out_op(i, N);
       if (!op.base) continue;
       const int es = Epi::Out::es(i);      // TMA addresses whole 16 bytes: base, row pitch and extent
-      if (((uintptr_t)op.base & 15u) || (op.ld * es) % 16 || (op.cols * es) % 16) { ring = false; break; }
+      if (((uintptr_t)op.base & 15u) || (op.ld * es) % 16 || (op.cols * es) % 16) {
+        if (kStaged) return AVC_E_BADCFG;      // staged functors have no register stores
+        ring = false;
+        break;
+      }
       AVC_TRY(make_map_rows_cached(&omaps.m[i], Epi::Out::es(i), op.base, (uint64_t)M, (uint64_t)op.cols,
-                                   (uint64_t)op.ld, EpiBatch<Epi, true>::kCols, 16));      // one warp's box
+                                   (uint64_t)op.ld, OutLayout<Epi>::cols(i), 16));      // one warp's box
       omask |= 1u << i;
     }
+    if constexpr (kStaged) {      // outputs written in place over the staged operands must not overlap each other
+      static_assert(OutLayout<Epi>::fits(), "the outputs do not fit over the staged operands");
+      for (int i = 0; i < EpiOut<Epi>::kN; ++i)
+        for (int j = i + 1; j < EpiOut<Epi>::kN; ++j)
+          if (((omask >> i) & (omask >> j) & 1u) && OutLayout<Epi>::overlap(i, j)) return AVC_E_BADCFG;
+    }
   }
+  static_assert(!kStaged || EpiOut<Epi>::kN > 0, "a staged functor ring-stores its outputs");
   CUtensorMap mab[4];
   AVC_TRY(make_map_bf16_cached(&mab[0], A.hi, (uint64_t)M, (uint64_t)K, (uint64_t)A.ld, kBK, kNtBM));
   AVC_TRY(make_map_bf16_cached(&mab[2], B.hi, (uint64_t)N, (uint64_t)K, (uint64_t)B.ld, kBK, BN));
@@ -803,10 +909,14 @@ static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K,
     mab[1] = mab[0]; mab[3] = mab[2];
   }
   g_nt_last_ring = ring ? 1 : 0;
-  if constexpr (EpiOut<Epi>::kN > 0) {
-    if (ring) return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, true>(st, M, N, K, mab, epi, b_const, emaps, omaps, omask);
+  if constexpr (kStaged) {
+    return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, true>(st, M, N, K, mab, epi, b_const, emaps, omaps, omask);
+  } else {
+    if constexpr (EpiOut<Epi>::kN > 0) {
+      if (ring) return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, true>(st, M, N, K, mab, epi, b_const, emaps, omaps, omask);
+    }
+    return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, false>(st, M, N, K, mab, epi, b_const, emaps, omaps, 0);
   }
-  return launch_gemm_tc_nt_kern<BN, NPROD, RESB, Epi, false>(st, M, N, K, mab, epi, b_const, emaps, omaps, 0);
 }
 
 // N <= 64 -> one 64-wide tile, else 128-wide tiles (a 65536-row GEMM then has 1024 tiles = 7.8 waves over 132

@@ -676,6 +676,12 @@ const char* avc_build_arch(void) { return "sm_90a"; }
 //   kind 10 EpiStore        -> OUT, split
 //   kind 11 EpiDgradRelu    as kind 4, and the split (the mask is read at the split's pitch, 2 ld2)
 //   kinds 108..111          kinds 8..11 with one bf16 product on the hi halves (NPROD = 1)
+// The staged functors with the output sets the renderer launches them with (kind 0 is the second-order sweep's last
+// linear: zbar and the fp32 copy of ubar_next), the split into OUT2 as above:
+//   kind 12 EpiChainBwd  as 0, but ubar_next = the split only (its extent is ldx)
+//   kind 13 EpiDgrad     as 1, but zbar_prev = Y is only read: the new zbar_prev = the split only
+//   kind 14 EpiDgrad     as 13 with the sdf term of kind 2
+//   kind 15 EpiChain     as 3, but qt_prev = the split only; ge = OUT [M][ldx] += the columns >= Nv
 // workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes (kind 11: + 8 * M * ld2 instead of 4 * M * ldx).
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
@@ -695,8 +701,9 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
   cudaStream_t st = (cudaStream_t)stream;
   tc::k_split_bf16<<<blocks_for(M * ld, 256), 256, 0, st>>>(A, M, K, K, ah, al, ld);
   tc::k_split_bf16<<<blocks_for((int64_t)N * ld, 256), 256, 0, st>>>(B, N, K, K, bh, bl, ld);
-  const float* xs = kind == 0 ? Y : X;      // the operand that is read as a bf16 pair
-  if (kind == 0 || kind == 4 || kind % 100 == 11) tc::k_split_bf16<<<blocks_for(M * ldm, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldm);
+  const float* xs = (kind == 0 || kind == 12) ? Y : X;      // the operand that is read as a bf16 pair
+  if (kind == 0 || kind == 12 || kind == 4 || kind % 100 == 11)
+    tc::k_split_bf16<<<blocks_for(M * ldm, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldm);
   AVC_LAUNCH_TRY();
   const tc::SplitPtr a{ah, al, ld}, b{bh, bl, ld};
   const Split16 none{nullptr, nullptr, ldx};
@@ -729,6 +736,28 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
       EpiGe e{OUT2, ld2, N};
       return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
     }
+  }
+  if (kind >= 12 && kind <= 15) {
+    if (!OUT || !OUT2) return AVC_E_NULL;
+    __nv_bfloat16* o16 = reinterpret_cast<__nv_bfloat16*>(OUT2);
+    const Split16 split{o16, o16 + ld2, 2 * ld2};
+    if (kind == 12) {
+      EpiChainBwd e;
+      e.N = N; e.Np = ldx; e.D1 = X; e.QT = nullptr; e.qt16 = Split16{xh, xl, ldx}; e.ZBAR = OUT; e.UNEXT = nullptr;
+      e.ldu = ldx; e.s_next = s; e.u16 = split;
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    if (kind == 13 || kind == 14) {
+      EpiDgrad e;
+      e.Nprev = N; e.Npp = ldx; e.s = s; e.D1prev = X; e.ZBARprev = Y;
+      e.sdfbar = kind == 14 ? v1 : nullptr; e.wsdf = kind == 14 ? v2 : nullptr; e.sdf_inv_scale = s2;
+      e.z16 = split; e.store_f32 = 0;
+      return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
+    }
+    EpiChain e;
+    e.Nprev = Nv; e.Npp = ldx; e.s = s; e.D1prev = X; e.QTprev = nullptr; e.GE = OUT; e.EP = ldx; e.E = N - Nv;
+    e.q16 = split;
+    return tc::launch_gemm_tc_nt<3>(st, M, N, K, a, b, e);
   }
   // kinds 108..111: 8..11 with one bf16 product (the colour net at color_products = 1)
   const bool np1 = kind >= 108 && kind <= 111;

@@ -798,28 +798,54 @@ struct EpiChain {
   static __device__ __forceinline__ Aux from_stage(const uint4 (&r)[1]) {
     return {make_float4(__uint_as_float(r[0].x), __uint_as_float(r[0].y), __uint_as_float(r[0].z), __uint_as_float(r[0].w))};
   }
-  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+  // qt_prev of the 4 columns (0 at columns >= Nprev); the ge accumulations of the columns >= Nprev are issued here
+  __device__ __forceinline__ void vals(int row, int col, float4 a, const Aux& x, float q[4]) const {
     AVC_EPI_UNPACK;
+    const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w};      // D1prev[row][col + i] where col + i < Nprev <= Npp
     if (col + 3 < Nprev) {        // fast path: whole group inside the hidden part
-      const size_t o = (size_t)row * Npp + col;
-      float q[4] = {x.d.x * v[0] * s, x.d.y * v[1] * s, x.d.z * v[2] * s, x.d.w * v[3] * s};
-      if (QTprev) *reinterpret_cast<float4*>(QTprev + o) = make_float4(q[0], q[1], q[2], q[3]);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) q[i] = dd[i] * v[i] * s;
+      return;
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = col + i;
+      q[i] = c < Nprev ? dd[i] * v[i] * s : 0.f;
+      const int e = c - Nprev;
+      // exclusive element: a fire-and-forget RED instead of a dependent load + store (written as red.global: with
+      // atomicAdd the ring-storing NT tiles at BN = 128 spill about 300 bytes)
+      if (c >= Nprev && e < E)
+        asm volatile("red.global.add.f32 [%0], %1;" ::"l"(GE + (size_t)row * EP + e), "f"(v[i] * kSqrtHalf) : "memory");
+    }
+  }
+  // The NT tiles ring-store qt_prev or its split (not both: the outputs are written over the staged sp' stash, whose
+  // 16 x 32 fp32 box of a warp holds the fp32 copy or the hi and lo boxes) over the padded width Npp, whose padding gets
+  // zeros.  The ge accumulations stay red.global from ring().
+  using Out = tc::Outs<4, 2, 2>;
+  tc::OutOp out_op(int i, int) const {
+    return i == 0 ? tc::OutOp{QTprev, Npp, Npp} : tc::OutOp{i == 1 ? q16.hi : q16.lo, q16.ld, Npp};
+  }
+  __host__ __device__ static constexpr tc::Over over(int i) { return i == 0 ? tc::Over{0, 0, 1} : tc::Over{0, i - 1, 1}; }
+  template <typename S>
+  __device__ __forceinline__ void ring(int row, int col, float4 a, const Aux& x, const S& sk) const {
+    float q[4];
+    vals(row, col, a, x, q);
+    sk.f32(0, q); sk.split(1, q);
+  }
+  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+    float q[4];
+    vals(row, col, a, x, q);
+    if (col + 3 < Nprev) {
+      if (QTprev) *reinterpret_cast<float4*>(QTprev + (size_t)row * Npp + col) = make_float4(q[0], q[1], q[2], q[3]);
       split16_put4(q16, (size_t)row, col, q);
       return;
     }
-    const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w};      // D1prev[row][col + i] where col + i < Nprev <= Npp
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      int c = col + i;
-      if (c < Nprev) {
-        float qv = dd[i] * v[i] * s;
-        if (QTprev) QTprev[(size_t)row * Npp + c] = qv;
-        split16_put(q16, (size_t)row, c, qv);
-      } else {
-        if (c < Npp) { if (QTprev) QTprev[(size_t)row * Npp + c] = 0.f; split16_put(q16, (size_t)row, c, 0.f); }
-        int e = c - Nprev;
-        // exclusive element, result unused: compiles to a fire-and-forget RED instead of a dependent load + store
-        if (e < E) atomicAdd(GE + (size_t)row * EP + e, v[i] * kSqrtHalf);
+      const int c = col + i;
+      if (c < Npp) {
+        if (QTprev) QTprev[(size_t)row * Npp + c] = q[i];
+        split16_put(q16, (size_t)row, c, q[i]);
       }
     }
   }
@@ -1013,22 +1039,44 @@ struct EpiChainBwd {
   // Both engines call with col < N and col % 4 == 0, and Np (a multiple of 8) >= N: every group lies inside the PADDED
   // width.  The padding of the sp' stash and of qt is zero (EpiValue / EpiChain), so the padding columns of a group get
   // the zeros the padding of ubar / zbar must hold.
-  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+  __device__ __forceinline__ void vals(float4 a, const Aux& x, float u[4], float zb[4]) const {
     AVC_EPI_UNPACK;
-    const size_t o = (size_t)row * Np + col;
     const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w};
     float qq[4];
     if (QT) { qq[0] = __uint_as_float(x.q.x); qq[1] = __uint_as_float(x.q.y); qq[2] = __uint_as_float(x.q.z); qq[3] = __uint_as_float(x.q.w); }
     else split16_get4(make_uint2(x.q.x, x.q.y), make_uint2(x.q.z, x.q.w), qq);
-    float u[4], zb[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       u[i] = dd[i] * v[i] * s_next;
       zb[i] = kBeta * (1.f - dd[i]) * qq[i] * v[i];
     }
+  }
+  // The NT tiles ring-store zbar over the staged sp' stash and ubar_next's split over the staged split of qt, or, at the
+  // last linear, ubar_next's fp32 copy over both halves of qt (two boxes of 8 columns): not the copy and the split at
+  // once.  Every extent is the padded width Np, whose padding gets zeros (zero sp' / qt padding, acc = 0 past N).  Into
+  // a skip layer (N = 217 of a 256-wide ubar_next) that writes zeros to ubar_next's columns 217..223, which hold the
+  // encoding half of the skip input's adjoint: backward() launches k_fill_gebar after this GEMM, and it rewrites columns
+  // 217..255.
+  using Out = tc::Outs<4, 4, 2, 2>;
+  tc::OutOp out_op(int i, int) const {
+    return i == 0 ? tc::OutOp{ZBAR, Np, Np} : i == 1 ? tc::OutOp{UNEXT, ldu, Np}
+                                               : tc::OutOp{i == 2 ? u16.hi : u16.lo, u16.ld, Np};
+  }
+  __host__ __device__ static constexpr tc::Over over(int i) {
+    return i == 0 ? tc::Over{0, 0, 1} : i == 1 ? tc::Over{1, 0, 2} : tc::Over{i - 1, 0, 1};
+  }
+  template <typename S>
+  __device__ __forceinline__ void ring(int, int, float4 a, const Aux& x, const S& s) const {
+    float u[4], zb[4];
+    vals(a, x, u, zb);
+    s.f32(0, zb); s.f32(1, u); s.split(2, u);
+  }
+  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+    float u[4], zb[4];
+    vals(a, x, u, zb);
     if (UNEXT) *reinterpret_cast<float4*>(UNEXT + (size_t)row * ldu + col) = make_float4(u[0], u[1], u[2], u[3]);
     split16_put4(u16, (size_t)row, col, u);
-    *reinterpret_cast<float4*>(ZBAR + o) = make_float4(zb[0], zb[1], zb[2], zb[3]);
+    *reinterpret_cast<float4*>(ZBAR + (size_t)row * Np + col) = make_float4(zb[0], zb[1], zb[2], zb[3]);
   }
   AVC_EPI_DIRECT
 };
@@ -1055,19 +1103,34 @@ struct EpiDgrad {
   }
   // Both engines call with col < Nprev and col % 4 == 0, and Npp (a multiple of 8) >= Nprev: every group lies inside the
   // padded width, where the sp' stash and the zbar padding are zero, and so is the result.
-  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+  __device__ __forceinline__ void vals(int row, int col, float4 a, const Aux& x, float r[4]) const {
     AVC_EPI_UNPACK;
     float sb = sdfbar ? sdfbar[row] * sdf_inv_scale : 0.f;
-    const size_t o = (size_t)row * Npp + col;
     const float dd[4] = {x.d.x, x.d.y, x.d.z, x.d.w}, zo[4] = {x.zb.x, x.zb.y, x.zb.z, x.zb.w};
-    float r[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       float ab = v[i];
       if (sdfbar) ab = fmaf(sb, wsdf[col + i], ab);
       r[i] = fmaf(dd[i], ab * s, zo[i]);
     }
-    if (store_f32) *reinterpret_cast<float4*>(ZBARprev + o) = make_float4(r[0], r[1], r[2], r[3]);
+  }
+  // The NT tiles ring-store the new zbar_prev over the padded width Npp (its padding gets zeros): the split's hi and lo
+  // boxes over the staged sp' stash, the fp32 copy (store_f32) over the staged old zbar_prev.
+  using Out = tc::Outs<4, 2, 2>;
+  tc::OutOp out_op(int i, int) const {
+    return i == 0 ? tc::OutOp{store_f32 ? ZBARprev : nullptr, Npp, Npp} : tc::OutOp{i == 1 ? z16.hi : z16.lo, z16.ld, Npp};
+  }
+  __host__ __device__ static constexpr tc::Over over(int i) { return i == 0 ? tc::Over{1, 0, 1} : tc::Over{0, i - 1, 1}; }
+  template <typename S>
+  __device__ __forceinline__ void ring(int row, int col, float4 a, const Aux& x, const S& sk) const {
+    float r[4];
+    vals(row, col, a, x, r);
+    sk.f32(0, r); sk.split(1, r);
+  }
+  __device__ __forceinline__ void operator()(int row, int col, float4 a, const Aux& x) const {
+    float r[4];
+    vals(row, col, a, x, r);
+    if (store_f32) *reinterpret_cast<float4*>(ZBARprev + (size_t)row * Npp + col) = make_float4(r[0], r[1], r[2], r[3]);
     split16_put4(z16, (size_t)row, col, r);
   }
   AVC_EPI_DIRECT

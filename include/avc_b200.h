@@ -445,7 +445,9 @@ int avc_tc_nt_last_ring(void);
 /* The backward epilogue functors of the NeuS path through the NT tiles on caller data: kind 0 second-order sweep,
  * 1 / 2 value backward without / with the sdf term, 3 gradient chain, 4 ReLU-mask dgrad, 5 encoding-gradient
  * accumulation; and with the bf16 split of their output: 6 value chain, 7 feature bias, 8 colour lin0, 9 ReLU,
- * 10 plain store, 11 ReLU-mask dgrad, 108..111 as 8..11 with one bf16 product (argument roles in avc_neus.cu).
+ * 10 plain store, 11 ReLU-mask dgrad, 108..111 as 8..11 with one bf16 product; and with the output sets the renderer
+ * gives them: 12 second-order sweep with the split of ubar, 13 / 14 value backward with only the split of the new
+ * zbar_prev, without / with the sdf term, 15 gradient chain with only the split of qt_prev (argument roles in avc_neus.cu).
  * workspace >= 4 * (M + N) * round_up(K, 8) + 4 * M * ldx bytes. */
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
