@@ -11,7 +11,7 @@
 //
 // Consumer warpgroups issue wgmma.mma_async m64nBNk16 on shared-memory descriptors, keep their fp32 accumulator in
 // registers and run the epilogue straight from that fragment; a TMA producer fills a shared-memory ring (K step 64, one
-// 128-byte swizzle atom) guarded by full (TMA transaction count) / empty mbarriers.
+// 128-byte swizzle atom; 32 for TN) guarded by full (TMA transaction count) / empty mbarriers.
 //   NT (384 threads): persistent ping-pong.  A producer warpgroup and two consumer warpgroups that take turns at the
 //      tensor pipe, one 64-row tile each, so that one's epilogue runs under the other's MMAs; one column tile per CTA,
 //      B panel resident in shared memory when K <= 256.
@@ -110,6 +110,10 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"((uint64_t)map), "r"(bar), "r"(x), "r"(y) : "memory");
+}
+// C[0] += a, C[1] += b as one 8-byte reduction (C 8-byte aligned)
+__device__ __forceinline__ void red_add_v2(float* C, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(C), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
@@ -936,22 +940,29 @@ static inline int launch_gemm_tc_nt(cudaStream_t st, int64_t M, int N, int K, co
 
 // ------------------------------------------------------------------------------------------------ TN kernel
 // C[i*ldc + j] += sum_{p in slice} A[p,i] * B[p,j]   (i < N1, j < N2): weight gradients.  Both operands are read
-// "MN-major": the reduction index p is the row of the global arrays.  TMA boxes are 64 (i or j) x 64 (p); in shared
-// memory one box is an MN block [64 p][128 B] (SWIZZLE_128B); a 128-wide M tile is 2 blocks (one per consumer
-// warpgroup), a BN-wide N tile BN/64 blocks.  Descriptor: LBO = 8192 B (next 64-wide block), SBO = 1024 B (8 p-rows), a K
-// step of 16 p-rows is +2048 B.  Split over p across blockIdx.z; partial tiles meet in fp32 red.global.add.
+// "MN-major": the reduction index p is the row of the global arrays.  TMA boxes are 64 (i or j) x kTnBK = 32 (p); in
+// shared memory one box is an MN block [32 p][128 B] (SWIZZLE_128B); a 128-wide M tile is 2 blocks (one per consumer
+// warpgroup), a BN-wide N tile BN/64 blocks.  Descriptor: LBO = 4096 B (next 64-wide block), SBO = 1024 B (8 p-rows), a K
+// step of 16 p-rows is +2048 B, two K steps per stage.  Split over p across blockIdx.z; partial tiles meet in fp32
+// red.global.add, two columns per reduction where the host found C and ldc 8-byte aligned (red_v2): that halves the
+// flush, 4.2 M scalar reductions for a 256 x 256 output split 64 ways.
+// A stage is 32 p-rows rather than kBK = 64: at BN = 256 with split operands a 64-row stage is 96 KB and only two fit, and
+// as a consumer frees a stage only after it has issued the next one's MMAs, a single load was in flight; 48 KB stages
+// give four, and two or three loads stay in flight.
+constexpr int kTnBK = 32;
 template <int BN, int NPROD>
 struct TcTnCfg {
-  static constexpr int BLK = kBK * 128;                             // one 64 x 64 bf16 block: 8 KB
-  static constexpr int A_BYTES = (kBM / 64) * BLK;                  // 16 KB
+  static constexpr int BLK = kTnBK * 128;                           // one 64-wide x 32-row bf16 block: 4 KB
+  static constexpr int A_BYTES = (kBM / 64) * BLK;                  // 8 KB
   static constexpr int B_BYTES = (BN / 64) * BLK;
   static constexpr int NOP = (NPROD == 3) ? 2 : 1;
   static constexpr int STAGE_BYTES = NOP * (A_BYTES + B_BYTES);
   static constexpr int kBudget = kSmemMax - 1024 /*align*/ - 1024 /*ones*/ - 256 /*barriers*/;
-  static constexpr int STAGES = kBudget / STAGE_BYTES >= 4 ? 4 : kBudget / STAGE_BYTES;
+  static constexpr int STAGES = kBudget / STAGE_BYTES >= 8 ? 8 : kBudget / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 1024 + 256;
   static_assert(SMEM_BYTES <= kSmemMax, "exceeds the 227 KB of shared memory per CTA");
-  static_assert(STAGES >= 2, "tile too large for shared memory");
+  static_assert(STAGES >= 4, "tile too large for a four-stage ring");
+  static_assert(16 * STAGES <= 256, "mbarriers overflow their area");
 };
 
 template <int BN, int NPROD>
@@ -959,7 +970,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapBhi, const __grid_constant__ CUtensorMap mapBlo,
                   int P, int N1, int N2, int rows_per_split, float* __restrict__ C, int ldc,
-                  float* __restrict__ colsum /* += sum_p A[p,i]; nullptr: off */) {
+                  float* __restrict__ colsum /* += sum_p A[p,i]; nullptr: off */, int red_v2) {
   using Cfg = TcTnCfg<BN, NPROD>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -974,7 +985,7 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   const int i0 = blockIdx.x * kBM, j0 = blockIdx.y * BN;
   const int p_begin = blockIdx.z * rows_per_split;
   const int p_end = min(P, p_begin + rows_per_split);
-  const int nk = (p_end - p_begin + kBK - 1) / kBK;     // host guarantees rows_per_split % 64 == 0 and nk >= 1
+  const int nk = (p_end - p_begin + kTnBK - 1) / kTnBK;     // host guarantees rows_per_split % 64 == 0 and nk >= 1
 
   if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&mapAhi); tma_prefetch_desc(&mapBhi);
@@ -995,7 +1006,7 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
         const int s = kb % Cfg::STAGES;
         mbar_wait(empty0 + 8 * s, ((kb / Cfg::STAGES) & 1) ^ 1);
         const uint32_t st = smem_base + s * Cfg::STAGE_BYTES;
-        const int p0 = p_begin + kb * kBK;
+        const int p0 = p_begin + kb * kTnBK;
         mbar_expect_tx(full0 + 8 * s, Cfg::STAGE_BYTES);
         // rows beyond p_end inside the last box belong to the next split: they must not be counted twice, so the
         // tensor maps are built with `rows = P` and the host makes every split a multiple of 64 rows.
@@ -1032,7 +1043,7 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
       auto batch = [&](auto with_colsum) {
         wgmma_fence();
 #pragma unroll
-        for (int k4 = 0; k4 < kBK / 16; ++k4) {
+        for (int k4 = 0; k4 < kTnBK / 16; ++k4) {
           wgmma_bf16<BN, 1, 1>(acc, da + 128 * k4, db + 128 * k4, (kb | k4) ? 1u : 0u);
           if (NPROD == 3) {
             wgmma_bf16<BN, 1, 1>(acc, da + 128 * k4, db + kLoB + 128 * k4, 1u);
@@ -1061,13 +1072,18 @@ gemm_tc_tn_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
     const int r0 = i0 + 64 * g + 16 * wq + (lane >> 2);
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
-      const int c = j0 + 8 * j + 2 * (lane & 3);
+      const int c = j0 + 8 * j + 2 * (lane & 3);      // even: with red_v2, C + r * ldc + c is 8-byte aligned
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h;
+        float* q = C + (size_t)r * ldc + c;
         if (r < N1) {
-          if (c < N2) atomicAdd(C + (size_t)r * ldc + c, acc[4 * j + 2 * h]);
-          if (c + 1 < N2) atomicAdd(C + (size_t)r * ldc + c + 1, acc[4 * j + 2 * h + 1]);
+          if (red_v2 && c + 1 < N2) {
+            red_add_v2(q, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          } else {
+            if (c < N2) atomicAdd(q, acc[4 * j + 2 * h]);
+            if (c + 1 < N2) atomicAdd(q + 1, acc[4 * j + 2 * h + 1]);
+          }
         }
       }
     }
@@ -1084,14 +1100,16 @@ static inline int launch_gemm_tc_tn(cudaStream_t st, int64_t P, int N1, int N2, 
                                     float* C, int ldc, float* colsum = nullptr) {
   if (P <= 0 || N1 <= 0 || N2 <= 0) return 0;
   CUtensorMap mAh, mAl, mBh, mBl;
-  AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)P, (uint64_t)N1, (uint64_t)A.ld, 64, kBK));
-  AVC_TRY(make_map_bf16_cached(&mBh, B.hi, (uint64_t)P, (uint64_t)N2, (uint64_t)B.ld, 64, kBK));
+  AVC_TRY(make_map_bf16_cached(&mAh, A.hi, (uint64_t)P, (uint64_t)N1, (uint64_t)A.ld, 64, kTnBK));
+  AVC_TRY(make_map_bf16_cached(&mBh, B.hi, (uint64_t)P, (uint64_t)N2, (uint64_t)B.ld, 64, kTnBK));
   if (NPROD == 3) {
-    AVC_TRY(make_map_bf16_cached(&mAl, A.lo, (uint64_t)P, (uint64_t)N1, (uint64_t)A.ld, 64, kBK));
-    AVC_TRY(make_map_bf16_cached(&mBl, B.lo, (uint64_t)P, (uint64_t)N2, (uint64_t)B.ld, 64, kBK));
+    AVC_TRY(make_map_bf16_cached(&mAl, A.lo, (uint64_t)P, (uint64_t)N1, (uint64_t)A.ld, 64, kTnBK));
+    AVC_TRY(make_map_bf16_cached(&mBl, B.lo, (uint64_t)P, (uint64_t)N2, (uint64_t)B.ld, 64, kTnBK));
   } else {
     mAl = mAh; mBl = mBh;
   }
+  // 8-byte reductions when every even column of C starts on 8 bytes
+  const int red_v2 = ((uintptr_t)C & 7u) == 0 && ldc % 2 == 0;
   const int t1 = ceil_div(N1, kBM);
   auto go = [&](auto kern, int BN, int smem) -> int {
     AVC_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -1102,7 +1120,8 @@ static inline int launch_gemm_tc_tn(cudaStream_t st, int64_t P, int N1, int N2, 
     int rows = (int)round_up(ceil_div(P, splits), kBK);
     splits = ceil_div(P, rows);
     dim3 grid(t1, t2, splits);
-    AVC_CUDA_TRY(launch_pdl(kern, grid, dim3(kTcThreads), (size_t)smem, st, mAh, mAl, mBh, mBl, (int)P, N1, N2, rows, C, ldc, colsum));
+    AVC_CUDA_TRY(launch_pdl(kern, grid, dim3(kTcThreads), (size_t)smem, st, mAh, mAl, mBh, mBl, (int)P, N1, N2, rows, C, ldc,
+                            colsum, red_v2));
     AVC_LAUNCH_TRY();
     return 0;
   };
