@@ -556,6 +556,48 @@ int avc_march_count(const float* field, int32_t nx, int32_t ny, int32_t nz, floa
 int avc_march_emit(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, const int32_t* offsets,
                    float* verts, int64_t* keys, avc_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * ShapeGen: the coarse body shape from a text prompt (AvatarGen/ShapeGen/main.py:93-123, utils.py:9-35).
+ *
+ * avc_vae_decode is LinearVAE.decode (main.py:67-68): out[b][D] = W2[D][H] . (W1[H][L] . z[b][L] + b1[H]) + b2[D] +
+ * v_template[D] for 1 <= B <= 8 latents, fp32, the two layers kept apart (no nonlinearity between them).  W2 must be
+ * 16-byte aligned (AVC_E_ALIGN) and H a multiple of 4; workspace avc_vae_decode_workspace_bytes(B, H).
+ * avc_load_textures is neural_renderer's load_textures (nr.load_obj(..., load_texture=True, texture_size=8),
+ * utils.py:7) for ONE material image: image [height][width][3] float in [0, 1] as stored (row 0 = top; the vertical
+ * flip of load_obj happens inside), face_uv [F][3][2] (the UV triangle of every face, any real value: REPEAT wraps
+ * it into [0, 1)), is_update [F] (non-zero: the face uses this material), textures [F][R][R][R][3] updated in place
+ * for those faces only (the caller fills it with 1.0 first, as load_obj does).  Texel (i, j, k) is the bilinear
+ * sample at the barycentric point (i, j, k) / (i + j + k) of the UV triangle.  2 <= R <= 64.
+ * avc_raster_textured is render_one_batch's render (utils.py:9-32, neural_renderer Renderer(camera_mode='look_at'):
+ * 30 deg viewing angle, near 0.1, far 100, fill_back, black background) from eye / at / up (HOST pointers) of the
+ * vertices as given: light 0.5 + 0.5 relu(n . (0, 1, 0)) per face with n = normalize((v0 - v1) x (v2 - v1)) facing
+ * the eye, times the trilinear sample of the face's cube at the perspective-corrected barycentrics w_k (R - 1) z / z_k
+ * clamped to [0, R - 1 - 1e-5], then the supersample x supersample average.  rgb_out [n][n][3], row 0 at the top
+ * (neural_renderer's [3][n][n] image transposed to HWC).  Workspace: avc_raster_textured_workspace_bytes.
+ * AVC_E_BADCFG when eye == at or up is parallel to the viewing direction.
+ * avc_clip_prep_nearest: images [B][n][n][3] -> out [B][3][S][S], F.interpolate(size=S) (nearest: src =
+ * floor(dst * n / S)) then the CLIP Normalize (main.py:101-103).
+ * avc_codebook_argmax: cos_out[N] = F.normalize(codebook[N][D] - image_emb[D], dim=1) . F.normalize(delta[D])
+ * (main.py:106-107, norms clamped at 1e-12) and best_out (device int32) = its first argmax (main.py:108); the
+ * workspace holds at least 8 bytes.
+ * ------------------------------------------------------------------------------------------ */
+int avc_vae_decode_workspace_bytes(int32_t B, int32_t hidden, size_t* bytes);
+int avc_vae_decode(const float* z, int32_t B, int32_t latent, const float* W1, const float* b1, int32_t hidden,
+                   const float* W2, const float* b2, const float* v_template, int32_t out_dim, float* out,
+                   void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_load_textures(const float* image, int32_t height, int32_t width, const float* face_uv,
+                      const int32_t* is_update, int32_t F, int32_t R, float* textures, avc_stream_t stream);
+int avc_raster_textured_workspace_bytes(int32_t V, int32_t image_size, int32_t supersample, size_t* bytes);
+int avc_raster_textured(const float* verts, const int32_t* faces, const float* textures, int32_t V, int32_t F,
+                        int32_t R, const float* eye, const float* at, const float* up, int32_t image_size,
+                        int32_t supersample, float* rgb_out, void* workspace, size_t workspace_bytes,
+                        avc_stream_t stream);
+int avc_clip_prep_nearest(const float* images, int32_t B, int32_t n, int32_t out_size, float* out,
+                          avc_stream_t stream);
+int avc_codebook_argmax(const float* codebook, const float* image_emb, const float* delta, int32_t N, int32_t D,
+                        float* cos_out, int32_t* best_out, void* workspace, size_t workspace_bytes,
+                        avc_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
