@@ -293,29 +293,47 @@ def write_pc2(fname: str, vertices_list) -> str:
 
 
 # ---------------------------------------------------------------- generate_animation (drive.py:308-361)
+class Rig(NamedTuple):
+    """A mesh rigged to SMPL's skeleton: ``mesh`` cleaned and in SMPL's frame, ``nearest`` [V] int32 (the template
+    vertex whose skin weights each vertex takes), ``tpose`` [V,3] (the vertices un-posed to the zero pose)."""
+    mesh: Mesh
+    nearest: torch.Tensor
+    tpose: torch.Tensor
+
+
+def motion_transforms(smpl_t: dict, motion_npy: str) -> torch.Tensor:
+    """drive.py:282-293 + 243-245 for every frame of a motion: A [frames, 24, 12] on the SMPL tensors' device."""
+    nj = smpl_t["J_regressor"].shape[0]
+    if nj != 24:
+        raise ValueError(f"read_pose_my decodes 24 SMPL joints per frame; the SMPL tensors have {nj}")
+    motion = torch.from_numpy(_motion_axis_angle(motion_npy)).to(smpl_t["v_template"].device, torch.float32)
+    return _rel_transforms(smpl_t, motion.contiguous(), True)
+
+
+def rig_mesh(mesh: Mesh, smpl_t: dict, stand_pose_npy: str) -> Rig:
+    """drive.py:317-339 on a mesh as read from its PLY: rotate it into SMPL's frame, keep its largest piece, give every
+    vertex the nearest stand-pose template vertex and un-pose it by that vertex's skin weights."""
+    v = mesh.vertices
+    mesh = cleanup_mesh(mesh._replace(vertices=torch.stack([v[:, 0], -v[:, 2], v[:, 1]], 1).contiguous()))
+    nj = smpl_t["J_regressor"].shape[0]
+    template, pose_rot, _ = load_template_smpl(smpl_t, stand_pose_npy, v.device)
+    nearest = _nearest(mesh.vertices, template["vertices"].reshape(-1, 3))
+    A_stand = _rel_transforms(smpl_t, pose_rot.reshape(1, nj, 9).contiguous(), False)
+    return Rig(mesh, nearest, _inv_lbs(mesh.vertices, nearest, smpl_t["lbs_weights"], A_stand[0]))
+
+
 def generate_animation(mesh_ply: str, motion_npy: str, out_dir: str, smpl, stand_pose_npy: str,
                        frames_per_chunk: Optional[int] = None, device="cuda"):
     """drive.py:308-361 with its hard-coded paths as arguments.  Writes ``out_dir/<mesh name>_cleaned_apose.ply`` and
     ``out_dir/<motion name>.pc2``; returns both paths."""
     device = _cuda(device)
     s = smpl_tensors(smpl, device)
-    nj = s["J_regressor"].shape[0]
-    if nj != 24:
-        raise ValueError(f"read_pose_my decodes 24 SMPL joints per frame; the SMPL tensors have {nj}")
-    motion = torch.from_numpy(_motion_axis_angle(motion_npy)).to(device, torch.float32).contiguous()
-    mesh = read_ply(mesh_ply, device)
-    v = mesh.vertices
-    mesh = cleanup_mesh(mesh._replace(vertices=torch.stack([v[:, 0], -v[:, 2], v[:, 1]], 1).contiguous()))
+    A = motion_transforms(s, motion_npy)
+    mesh, nearest, tpose = rig_mesh(read_ply(mesh_ply, device), s, stand_pose_npy)
     os.makedirs(out_dir, exist_ok=True)
     name = os.path.splitext(os.path.basename(mesh_ply))[0]
     ply_path = write_ply(mesh, os.path.join(out_dir, f"{name}_cleaned_apose.ply"))
 
-    template, pose_rot, _ = load_template_smpl(s, stand_pose_npy, device)
-    nearest = _nearest(mesh.vertices, template["vertices"].reshape(-1, 3))
-    A_stand = _rel_transforms(s, pose_rot.reshape(1, nj, 9).contiguous(), False)
-    tpose = _inv_lbs(mesh.vertices, nearest, s["lbs_weights"], A_stand[0])
-
-    A = _rel_transforms(s, motion, True)
     frames, N = A.shape[0], tpose.shape[0]
     chunk = max(1, min(frames, frames_per_chunk or _CHUNK_BYTES // (N * 12)))
     dev_buf = [torch.empty(chunk, N, 3, dtype=torch.float32, device=device) for _ in range(2)]

@@ -598,6 +598,47 @@ int avc_codebook_argmax(const float* codebook, const float* image_emb, const flo
                         float* cos_out, int32_t* best_out, void* workspace, size_t workspace_bytes,
                         avc_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Video frames of a generated avatar (avatarclip_b200/video.py): one vertex-coloured mesh, smooth-shaded, over many
+ * frames per launch.  The reference has no renderer for its results (render_novel_image / interpolate_view cannot
+ * run, AvatarAnimate's visualize.py draws the grey SMPL body through pyrender); this one is the project's own.
+ *
+ * avc_video_adjacency: the vertex -> incident-face lists of faces [F][3] as CSR, built once per mesh: offsets [V + 1]
+ * (offsets[V] = the number of entries, at most 3F), vf [3F] the face ids of vertex v in vf[offsets[v] .. offsets[v+1]),
+ * in ascending face order (a face naming v twice is listed twice; an index outside [0, V) is skipped).
+ * 1 <= V, 1 <= F <= 2^29.  Workspace: avc_video_adjacency_workspace_bytes(V).
+ *
+ * avc_video_render: rgb_out [n_frames][n][n][3] uint8 (n = image_size, row 0 at the top) of the mesh with vertices
+ * verts + f * frame_stride ([V][3] per frame; frame_stride 0: every frame draws the same vertices).
+ *   - cameras: HOST [n_frames][13]: a world-to-camera [R | t] (row-major 3x4; camera x right, y down, z forward), then
+ *     the focal length in output pixels; the principal point is the image centre.  Each output pixel holds
+ *     supersample x supersample samples at the centres of its sub-pixels.
+ *   - Faces with a vertex at camera depth z <= 0.01 are skipped, both windings are drawn, and per sample the face of
+ *     the smallest perspective-correct depth wins (64-bit atomicMin of (depth bits | face id): ties to the smaller id).
+ *   - Vertex normal: the sum over the vertex's faces, in CSR order, of the un-normalised (v1 - v0) x (v2 - v0), per
+ *     frame (no float atomics: the frames are bitwise reproducible).
+ *   - Sample colour: the perspective-correct barycentric interpolation of the stored 0-255 colours (colors [V][3]
+ *     uint8, or NULL for a uniform grey of 200) times 0.25 + 0.75 max(0, n . v), n the interpolated normal,
+ *     normalised and flipped to face the camera, v the direction towards the camera along its axis (a headlight);
+ *     background (HOST [3] uint8) where no face won.  The pixel is the mean of its samples rounded to nearest.
+ *   - face_out: NULL, or [n_frames][n * supersample][n * supersample] int32, the winning face of every sample (-1:
+ *     none), row 0 at the top.
+ *   - AVC_E_BADCFG unless 1 <= image_size <= 4096, 1 <= supersample <= 4, 1 <= n_frames <= 65535, V >= 1,
+ *     1 <= F <= 2^29, frame_stride >= 0 and every focal length > 0.
+ *   - offsets / vf from avc_video_adjacency of the same faces.  Workspace: avc_video_render_workspace_bytes (about
+ *     n_frames * (32 V + 8 (n * supersample)^2) bytes).
+ * ------------------------------------------------------------------------------------------ */
+int avc_video_adjacency_workspace_bytes(int32_t V, size_t* bytes);
+int avc_video_adjacency(const int32_t* faces, int32_t V, int32_t F, int32_t* offsets, int32_t* vf, void* workspace,
+                        size_t workspace_bytes, avc_stream_t stream);
+int avc_video_render_workspace_bytes(int32_t V, int32_t F, int32_t n_frames, int32_t image_size, int32_t supersample,
+                                     size_t* bytes);
+int avc_video_render(const float* verts, int64_t frame_stride, const int32_t* faces, const int32_t* offsets,
+                     const int32_t* vf, const uint8_t* colors, int32_t V, int32_t F, const float* cameras,
+                     int32_t n_frames, int32_t image_size, int32_t supersample, const uint8_t* background,
+                     uint8_t* rgb_out, int32_t* face_out, void* workspace, size_t workspace_bytes,
+                     avc_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
