@@ -170,6 +170,136 @@ EncodeTargets make_targets(const NeusPlan& pl, const NeusWs& w) {
   return t;
 }
 
+// -------------------------------------------------------------------------------- per-point kernels and thin heads
+// The launches below are shared by the render and the kernel self-test (avc_neus_kernel_test).
+int encode_samples(const float* rays_o, const float* rays_d, const float* z, int nz, int pitch, int Rc, float scale,
+                   int multires, int E, int EP, const EncodeTargets& t, cudaStream_t st) {
+  k_encode_samples<<<blocks_for((int64_t)nz * Rc * 8, 256), 256, 0, st>>>(rays_o, rays_d, z, nz, pitch, Rc, scale,
+                                                                         multires, E, EP, t);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int encode_points(const float* pts, int64_t P, float scale, int multires, int E, int EP, const EncodeTargets& t,
+                  cudaStream_t st) {
+  k_encode_points<<<blocks_for(P * 8, 256), 256, 0, st>>>(pts, P, scale, multires, E, EP, t);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int encode_fine(const float* rays_o, const float* rays_d, const float* z_vals, int S, int64_t Rc, float sample_dist,
+                float scale, int multires, int E, int EP, float* cin, float* mid_z, float* inside, const EncodeTargets& t,
+                cudaStream_t st) {
+  k_encode_fine<<<blocks_for(Rc * S * 8, 256), 256, 0, st>>>(rays_o, rays_d, z_vals, S, Rc, sample_dist, scale, multires,
+                                                            E, EP, cin, mid_z, inside, t);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// sdf = (in[L] . W_L[0] + b_L[0]) / scale over the K inputs of the last linear only: the columns [K, Kp) of in[L]
+// (K = 4 mod 8) are padding nothing writes, and a NaN there times the zero padded weight would still be NaN.  K is a
+// multiple of 4, as the float4 loop needs.  Point p = r * nz + j is stored at sdf_out[r * pitch + j] (nz = 0: at p).
+int sdf_head(const NeusPlan& pl, const float* inL, const float* pack, int64_t P, float* sdf_out, int nz, int pitch,
+             cudaStream_t st) {
+  const LinDim& dl = pl.sdf[pl.L];
+  OutSdf os{sdf_out, 1.0f / pl.cfg.sdf_scale, nz, pitch};
+  k_thin_nt<1, OutSdf><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(inL, dl.Kp, dl.K, pack + pl.pk_wsdf, dl.Kp,
+                                                                    pack + pl.pk_bsdf, P, os);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// rgb6 = sigmoid of both colour heads on the last hidden colour activation ch[Lc]
+int color_heads(const NeusPlan& pl, const float* chL, const float* pack, int64_t P, float* rgb6, cudaStream_t st) {
+  OutHeads oh{rgb6};
+  k_thin_nt<6, OutHeads><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(chL, pl.Hc, pl.Hc, pack + pl.pk_W6, pl.Hc,
+                                                                      pack + pl.pk_b6, P, oh);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// nbar += cbar_0 . W0[:, 3:6]   (the normal columns of colour lin0)
+int nbar_add_color(const NeusPlan& pl, const float* cbar0, const float* pack, int64_t P, float* nbar, cudaStream_t st) {
+  OutNbarAdd on{nbar};
+  k_thin_nt<6, OutNbarAdd><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(cbar0, pl.Hc, pl.Hc, pack + pl.pk_c0xT, pl.Hc,
+                                                                        nullptr, P, on);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// cbar_Lc = (y6bar . W6) * [ch[Lc] > 0]; the fp32 copy may be NULL
+int heads_dgrad(const NeusPlan& pl, const float* y6bar, const float* pack, const float* chL, int64_t P, float* cbar,
+                const Split16& c16, cudaStream_t st) {
+  k_heads_dgrad<<<blocks_for(P * pl.Hc / 4, 256), 256, 0, st>>>(y6bar, pack + pl.pk_W6, pl.Hc, chL, P, cbar, c16);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// start of the reverse sweep: qt[L-1] (fp32 copy may be NULL) and ge from the stash softplus'(z[L-1])
+int chain_start(const NeusPlan& pl, const float* pack, const float* zprev, int64_t P, float* qt, float* ge,
+                const Split16& qt16, cudaStream_t st) {
+  const LinDim& dL = pl.sdf[pl.L];
+  const LinDim& dp = pl.sdf[pl.L - 1];
+  int64_t tot = P * (int64_t)(dp.Np / 4 > pl.EP ? dp.Np / 4 : pl.EP);   // threads: 4 qt columns each, 1 ge entry each
+  k_chain_start<<<blocks_for(tot, 256), 256, 0, st>>>(pack + pl.pk_wsdf, dL.K, dL.skip ? 1 : 0, pl.E, pl.EP, zprev, dp.N,
+                                                      dp.Np, P, qt, ge, qt16);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// n = D(y)^T ge -> cin[p][3:6] and grad_out (or NULL)
+int normals(const NeusPlan& pl, const float* ge, int64_t P, float* cin, float* grad_out, cudaStream_t st) {
+  k_normal<<<blocks_for(P, 128), 128, 0, st>>>(ge, pl.EP, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, cin, grad_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// gebar = D(y) nbar -> gebar and ubar_0 (fp32 copy or NULL, its split u16), pitch Kp_0
+int dge(const NeusPlan& pl, const float* cin, const float* nbar, int64_t P, float* ubar0, float* gebar, const Split16& u16,
+        cudaStream_t st) {
+  k_dge<<<blocks_for(P * 8, 256), 256, 0, st>>>(cin, nbar, pl.EP, pl.E, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, ubar0,
+                                                pl.sdf[0].Kp, gebar, u16);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// the encoding half of skip layer l's input adjoint: ubar_l[p][K_l - E + e] = gebar[p][e] / sqrt(2)
+int fill_gebar(const NeusPlan& pl, int l, const float* gebar, int64_t P, float* ubar, const Split16& u16, cudaStream_t st) {
+  const LinDim& d = pl.sdf[l];
+  k_fill_gebar<<<blocks_for(P * pl.E, 256), 256, 0, st>>>(gebar, pl.EP, pl.E, P, ubar, d.Kp, d.K - pl.E, u16);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+// SDFNetwork evaluators (avc_neus_sdf_eval): cin[p] = (x, 0, 0, 0, 0, 0) and out[p] = [sdf, feat]
+__global__ void k_points_to_cin(const float* __restrict__ pts, int64_t P, float* __restrict__ cin) {
+  int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  float4* c = reinterpret_cast<float4*>(cin + (size_t)p * 8);
+  c[0] = make_float4(pts[p * 3], pts[p * 3 + 1], pts[p * 3 + 2], 0.f);
+  c[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+__global__ void k_assemble_sdf_feat(const float* __restrict__ sdf, const float* __restrict__ feat, int Fp, int F, int64_t P,
+                                    float* __restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P * (F + 1)) return;
+  int64_t p = i / (F + 1);
+  int c = (int)(i - p * (F + 1));
+  out[i] = c == 0 ? sdf[p] : feat[(size_t)p * Fp + (c - 1)];
+}
+
+int points_to_cin(const float* pts, int64_t P, float* cin, cudaStream_t st) {
+  k_points_to_cin<<<blocks_for(P, 256), 256, 0, st>>>(pts, P, cin);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int assemble_sdf_feat(const NeusPlan& pl, const float* sdf, const float* feat, int64_t P, float* out, cudaStream_t st) {
+  k_assemble_sdf_feat<<<blocks_for(P * (pl.F + 1), 256), 256, 0, st>>>(sdf, feat, pl.Fp, pl.F, P, out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
 // -------------------------------------------------------------------------------- value chain
 // in[0] (and the skip columns) must hold the encoding of Pn points.  stash: keep z[l].
 // Leaves in[L] ready; writes sdf[Pn] (thin) and, when want_feat, feat[Pn][Fp].
@@ -233,10 +363,7 @@ int value_chain(const NeusPlan& pl, const NeusWs& w, int64_t Pn, bool stash, boo
     }
   }
   const LinDim& dl = pl.sdf[pl.L];
-  OutSdf os{sdf_out, 1.0f / pl.cfg.sdf_scale, sdf_nz, sdf_pitch};
-  k_thin_nt<1, OutSdf><<<blocks_for(Pn, 8 * kThinPPW), 256, 0, st>>>(w.in[pl.L], dl.Kp, dl.Kp, pack + pl.pk_wsdf, dl.Kp,
-                                                           pack + pl.pk_bsdf, Pn, os);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(sdf_head(pl, w.in[pl.L], pack, Pn, sdf_out, sdf_nz, sdf_pitch, st));
   if (want_feat) {
     // wgmma engine: every consumer of the features reads the split (colour lin0 A operand, its weight gradient)
     EpiBias e{pack + dl.pk_b, pl.cfg.engine == 1 ? nullptr : w.feat, pl.Fp, pl.F, w.feat16};
@@ -249,16 +376,9 @@ int value_chain(const NeusPlan& pl, const NeusWs& w, int64_t Pn, bool stash, boo
 // d sdf / d x by the reverse sweep of Appendix B (no second forward): needs the sp' stash of value_chain(stash = true)
 // and cin[p][0:3] = x.  Writes the raw gradient into cin[p][3:6] and, optionally, grad_out [P][3].
 int gradient_chain(const NeusPlan& pl, const NeusWs& w, int64_t P, float* grad_out, cudaStream_t st) {
-  const float* pack = w.pack;
-  const LinDim& dL = pl.sdf[pl.L];
-  const LinDim& dp = pl.sdf[pl.L - 1];
   // wgmma engine: qt_l is only ever consumed as a split operand (gradient chain, second-order sweep, dW)
   const bool tc1 = pl.cfg.engine == 1;
-  int64_t tot = P * (int64_t)(dp.Np / 4 > pl.EP ? dp.Np / 4 : pl.EP);   // threads: 4 qt columns each, 1 ge entry each
-  k_chain_start<<<blocks_for(tot, 256), 256, 0, st>>>(pack + pl.pk_wsdf, dL.K, dL.skip ? 1 : 0, pl.E, pl.EP,
-                                                      w.z[pl.L - 1], dp.N, dp.Np, P, tc1 ? nullptr : w.qt[pl.L - 1], w.ge,
-                                                      w.qt16[pl.L - 1]);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(chain_start(pl, w.pack, w.z[pl.L - 1], P, tc1 ? nullptr : w.qt[pl.L - 1], w.ge, w.qt16[pl.L - 1], st));
   for (int l = pl.L - 1; l >= 1; --l) {
     const LinDim& d = pl.sdf[l];
     const LinDim& dq = pl.sdf[l - 1];
@@ -271,9 +391,7 @@ int gradient_chain(const NeusPlan& pl, const NeusWs& w, int64_t P, float* grad_o
   const LinDim& d0 = pl.sdf[0];
   EpiGe eg{w.ge, pl.EP, pl.E};
   AVC_TRY(gemm_nt(pl, w, st, P, pl.E, d0.N, w.qt[0], d0.Np, w.qt16[0], d0.pk_WT, d0.Np, eg));
-  k_normal<<<blocks_for(P, 128), 128, 0, st>>>(w.ge, pl.EP, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, w.cin, grad_out);
-  AVC_LAUNCH_TRY();
-  return 0;
+  return normals(pl, w.ge, P, w.cin, grad_out, st);
 }
 
 // -------------------------------------------------------------------------------- placement
@@ -309,9 +427,7 @@ int place_samples(const NeusPlan& pl, const NeusWs& w, const float* rays_o, cons
   if (pl.cfg.n_importance == 0) return 0;
   EncodeTargets t = make_targets(pl, w);
   int64_t Pn = (int64_t)pl.n0 * Rc;
-  k_encode_samples<<<blocks_for(Pn * 8, 256), 256, 0, st>>>(rays_o, rays_d, w.zA, pl.n0, S, Rc, pl.cfg.sdf_scale,
-                                                            pl.cfg.sdf_multires, pl.E, pl.EP, t);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(encode_samples(rays_o, rays_d, w.zA, pl.n0, S, Rc, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E, pl.EP, t, st));
   AVC_TRY(value_chain(pl, w, Pn, false, false, w.sA, st, pl.n0, S));
   float *zc = w.zA, *sc = w.sA, *zn = w.zB, *sn = w.sB;
   int n = pl.n0;
@@ -321,9 +437,8 @@ int place_samples(const NeusPlan& pl, const NeusWs& w, const float* rays_o, cons
     AVC_TRY(upsample(rays_o, rays_d, zc, sc, n, S, Rc, inv_s, pl.per, w.newZ, st));
     if (!last) {
       Pn = (int64_t)pl.per * Rc;
-      k_encode_samples<<<blocks_for(Pn * 8, 256), 256, 0, st>>>(rays_o, rays_d, w.newZ, pl.per, pl.per, Rc,
-                                                                pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E, pl.EP, t);
-      AVC_LAUNCH_TRY();
+      AVC_TRY(encode_samples(rays_o, rays_d, w.newZ, pl.per, pl.per, Rc, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E,
+                             pl.EP, t, st));
       AVC_TRY(value_chain(pl, w, Pn, false, false, w.newS, st, 0, 0));   // newS is [Rc][per]: identity mapping
     }
     // the last round writes the merged depths straight into the caller's z_vals [Rc][S]
@@ -407,11 +522,9 @@ int fine_forward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, bool wr
   const int64_t P = io.Rc * pl.S;
   const float* pack = w.pack;
   EncodeTargets t = make_targets(pl, w);
-  k_encode_fine<<<blocks_for(P * 8, 256), 256, 0, st>>>(io.rays_o, io.rays_d, io.out.z_vals, pl.S, io.Rc,
-                                                    2.0f / (float)pl.n0, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E,
-                                                    pl.EP, w.cin, write_outputs ? io.out.mid_z_vals : nullptr,
-                                                    write_outputs ? io.out.inside_sphere : nullptr, t);
-  AVC_LAUNCH_TRY();
+  AVC_TRY(encode_fine(io.rays_o, io.rays_d, io.out.z_vals, pl.S, io.Rc, 2.0f / (float)pl.n0, pl.cfg.sdf_scale,
+                      pl.cfg.sdf_multires, pl.E, pl.EP, w.cin, write_outputs ? io.out.mid_z_vals : nullptr,
+                      write_outputs ? io.out.inside_sphere : nullptr, t, st));
   AVC_TRY(value_chain(pl, w, P, true, true, w.sdf, st));
   AVC_TRY(gradient_chain(pl, w, P, write_outputs ? io.out.gradients : nullptr, st));
   // ---- colour net
@@ -430,10 +543,7 @@ int fine_forward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, bool wr
                 (tc1 && l + 1 == pl.Lc) ? none16 : w.ch16[l + 1]};
       AVC_TRY(gemm_nt_color(pl, w, st, P, pl.Hc, pl.Hc, w.ch[l], pl.Hc, w.ch16[l], c.pk_W, pl.Hc, e));
     }
-    OutHeads oh{w.rgb6};
-    k_thin_nt<6, OutHeads><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(w.ch[pl.Lc], pl.Hc, pl.Hc, pack + pl.pk_W6, pl.Hc,
-                                                             pack + pl.pk_b6, P, oh);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(color_heads(pl, w.ch[pl.Lc], pack, P, w.rgb6, st));
   }
   if (write_outputs) AVC_TRY(composite_forward(make_composite_args(pl, w, io), io.out, w.ray_part, w.ctx, st));
   return 0;
@@ -484,10 +594,8 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
     AVC_TRY(thin_tn<6>(st, w.y6bar, 8, 1.f, w.ch[pl.Lc], pl.Hc, pl.Hc, P, wbar + dh.off_v, pl.Hc, 1, wbar + dh.off_b, 3,
                        wbar + dx.off_v, wbar + dx.off_b));
     // wgmma engine: the hidden linears consume cbar as a split operand; its fp32 copy is only read at layer 0
-    k_heads_dgrad<<<blocks_for(P * pl.Hc / 4, 256), 256, 0, st>>>(w.y6bar, pack + pl.pk_W6, pl.Hc, w.ch[pl.Lc], P,
-                                                              (pl.cfg.engine == 1 && pl.Lc > 1) ? nullptr : w.cbar[0],
-                                                              w.cbar16[0]);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(heads_dgrad(pl, w.y6bar, pack, w.ch[pl.Lc], P, (pl.cfg.engine == 1 && pl.Lc > 1) ? nullptr : w.cbar[0],
+                        w.cbar16[0], st));
   }
   // ---- colour hidden linears l = Lc-1 .. 0 ; cbar_l lives in w.cbar[cur]
   int cur = 0;
@@ -512,22 +620,16 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
       EpiStore es{pl.cfg.engine == 1 ? nullptr : w.featbar, pl.Fp, pl.F, w.featbar16};
       AVC_TRY(gemm_nt_color(pl, w, st, P, pl.F, pl.Hc, cb, pl.Hc, w.cbar16[cur], c.pk_WT, pl.Hc, es));
       // nbar += cbar . W0[:, 3:6]   (d/d points is discarded: pts is a leaf, models/fields.py:97)
-      OutNbarAdd on{w.nbar};
-      k_thin_nt<6, OutNbarAdd><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(cb, pl.Hc, pl.Hc, pack + pl.pk_c0xT, pl.Hc, nullptr,
-                                                                 P, on);
-      AVC_LAUNCH_TRY();
+      AVC_TRY(nbar_add_color(pl, cb, pack, P, w.nbar, st));
     }
   }
 
   // ---- SDF: second-order sweep in forward layer order
   int ucur = 0;
   {
-    const LinDim& d0 = pl.sdf[0];
     // wgmma engine: ubar_0 is only consumed as a split operand
-    k_dge<<<blocks_for(P * 8, 256), 256, 0, st>>>(w.cin, w.nbar, pl.EP, pl.E, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P,
-                                                  pl.cfg.engine == 1 ? nullptr : w.ubar[0], d0.Kp, w.gebar,
-                                                  with_ld(w.ubar16[0], d0.Kp));
-    AVC_LAUNCH_TRY();
+    AVC_TRY(dge(pl, w.cin, w.nbar, P, pl.cfg.engine == 1 ? nullptr : w.ubar[0], w.gebar,
+                with_ld(w.ubar16[0], pl.sdf[0].Kp), st));
   }
   for (int l = 0; l <= pl.L; ++l) {
     const LinDim& d = pl.sdf[l];
@@ -551,9 +653,7 @@ int fine_backward(const NeusPlan& pl, const NeusWs& w, const ChunkIO& io, const 
     e.u16 = unext16;
     AVC_TRY(gemm_nt(pl, w, st, P, d.N, d.K, ub, d.Kp, ub16, d.pk_W, d.Kp, e));
     if (dn.skip) {
-      k_fill_gebar<<<blocks_for(P * pl.E, 256), 256, 0, st>>>(w.gebar, pl.EP, pl.E, P, w.ubar[ucur ^ 1], dn.Kp,
-                                                              dn.K - pl.E, unext16);
-      AVC_LAUNCH_TRY();
+      AVC_TRY(fill_gebar(pl, l + 1, w.gebar, P, w.ubar[ucur ^ 1], unext16, st));
     }
     ucur ^= 1;
   }
@@ -798,14 +898,18 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
   return AVC_E_BADCFG;
 }
 
-// One compositing, scalar or placement kernel of the NeuS path on caller buffers, launched by the render's own host
-// helpers (argument roles in include/avc_b200.h).
+// One kernel of the NeuS path outside the GEMM tiles on caller buffers, launched by the render's own host helpers
+// (argument roles in include/avc_b200.h).
 int avc_neus_kernel_test(int32_t kind, const int64_t* d, const float* fs, const void* const* in, void* const* out,
                          avc_stream_t stream) {
   if (!d || !fs || !in || !out) return AVC_E_NULL;
   cudaStream_t st = (cudaStream_t)stream;
   const auto F32 = [](const void* p) { return (const float*)p; };
   const auto O32 = [](void* p) { return (float*)p; };
+  const auto pair = [](void* p, int ld) {      // a bf16 pair buffer [rows][2 ld]: hi in [0, ld), lo in [ld, 2 ld)
+    __nv_bfloat16* h = (__nv_bfloat16*)p;
+    return Split16{h, h ? h + ld : nullptr, 2 * ld};
+  };
   switch (kind) {
     case 0: return ctx_init(F32(in[0]), d[0], O32(out[0]), (int)d[1], st);
     case 1:
@@ -859,6 +963,101 @@ int avc_neus_kernel_test(int32_t kind, const int64_t* d, const float* fs, const 
       return merge(F32(in[0]), F32(in[1]), n, pitch, F32(in[2]), F32(in[3]), per, Rc, O32(out[0]), O32(out[1]), pitch_o,
                    st);
     }
+    case 18: {
+      const int NI = (int)d[0], lds = (int)d[1], ldh = (int)d[2], NC = (int)d[3], si = (int)d[5], sc = (int)d[6];
+      const int split = (int)d[7];
+      const int64_t P = d[4];
+      if (P < 1 || NC < 1 || lds < NI || ldh < NC) return AVC_E_SIZE;
+      if (NI == 1) return thin_tn<1>(st, F32(in[0]), lds, fs[0], F32(in[1]), ldh, NC, P, O32(out[0]), si, sc, O32(out[1]),
+                                     split, O32(out[2]), O32(out[3]));
+      if (NI == 6) return thin_tn<6>(st, F32(in[0]), lds, fs[0], F32(in[1]), ldh, NC, P, O32(out[0]), si, sc, O32(out[1]),
+                                     split, O32(out[2]), O32(out[3]));
+      return AVC_E_BADCFG;
+    }
+    case 19: {
+      if (d[2] < 1 || d[1] < 1 || d[0] < d[1]) return AVC_E_SIZE;
+      return colsum(st, F32(in[0]), (int)d[0], (int)d[1], d[2], fs[0], O32(out[0]));
+    }
+    case 25: {
+      if (d[0] < 1) return AVC_E_SIZE;
+      return points_to_cin(F32(in[0]), d[0], O32(out[0]), st);
+    }
+  }
+  if (kind < 9 || kind > 26) return AVC_E_BADCFG;
+  if (kind >= 12 && kind <= 14) {
+    // EncodeTargets: out[0] in0 or NULL, out[1..4] skip fp32 targets or NULL, out[5] the in0 pair, out[6..9] the skip
+    // pairs (bf16 [P][2 ld]: hi in columns [0, ld), lo in [ld, 2 ld) of each row; NULL: none)
+    const int multires = (int)d[0], E = 3 * (1 + 2 * multires), EP = (int)round_up(E, 8);
+    if (multires < 0 || multires > 10 || d[1] < EP || d[2] < 0 || d[2] > 4) return AVC_E_SIZE;
+    EncodeTargets t;
+    memset(&t, 0, sizeof(t));
+    t.in0 = O32(out[0]); t.ld0 = (int)d[1]; t.in0_16 = pair(out[5], t.ld0);
+    t.n_skip = (int)d[2];
+    for (int s = 0; s < t.n_skip; ++s) {
+      t.skip_ptr[s] = O32(out[1 + s]); t.skip_ld[s] = (int)d[3 + s]; t.skip_col[s] = (int)d[7 + s];
+      if (t.skip_col[s] < 0 || t.skip_col[s] + E > t.skip_ld[s]) return AVC_E_SIZE;
+      t.skip16[s] = pair(out[6 + s], t.skip_ld[s]);
+    }
+    if (kind == 12) {
+      if (d[11] < 1) return AVC_E_SIZE;
+      return encode_points(F32(in[0]), d[11], fs[0], multires, E, EP, t, st);
+    }
+    if (kind == 13) {
+      const int nz = (int)d[11], pitch = (int)d[12], Rc = (int)d[13];
+      if (nz < 1 || pitch < nz || Rc < 1) return AVC_E_SIZE;
+      return encode_samples(F32(in[0]), F32(in[1]), F32(in[2]), nz, pitch, Rc, fs[0], multires, E, EP, t, st);
+    }
+    const int S = (int)d[11];
+    if (S < 1 || d[12] < 1 || !out[10]) return AVC_E_SIZE;
+    return encode_fine(F32(in[0]), F32(in[1]), F32(in[2]), S, d[12], fs[1], fs[0], multires, E, EP, O32(out[10]),
+                       O32(out[11]), O32(out[12]), t, st);
+  }
+  // the kinds below run on a whole configuration: in[0] is a HOST avc_neus_cfg
+  NeusPlan pl;
+  AVC_TRY(build_plan((const avc_neus_cfg*)in[0], &pl));
+  if (kind >= 15 && d[0] < 1) return AVC_E_SIZE;      // d[0] = P
+  switch (kind) {
+    case 9: {
+      int64_t* o = (int64_t*)out[0];
+      const int64_t head[16] = {pl.L, pl.Lc, pl.E, pl.EP, pl.F, pl.Fp, pl.Hc, pl.pack_floats, pl.n_params, pl.off_var,
+                                pl.pk_wsdf, pl.pk_bsdf, pl.pk_c0x, pl.pk_c0xT, pl.pk_W6, pl.pk_b6};
+      for (int i = 0; i < 16; ++i) o[i] = head[i];
+      int64_t* q = o + 16;
+      auto put = [&](const LinDim& x) {
+        const int64_t r[11] = {x.K, x.N, x.Kp, x.Np, x.skip ? 1 : 0, x.off_g, x.off_v, x.off_b, x.pk_W, x.pk_WT, x.pk_b};
+        for (int i = 0; i < 11; ++i) *q++ = r[i];
+      };
+      for (int l = 0; l <= pl.L; ++l) put(pl.sdf[l]);
+      for (int l = 0; l <= pl.Lc; ++l) put(pl.col[l]);
+      put(pl.extra);
+      return 0;
+    }
+    case 10: {
+      NeusWs w;
+      memset(&w, 0, sizeof(w));
+      w.pack = O32(out[0]);
+      if (pl.cfg.engine == 1) {
+        if (!out[1]) return AVC_E_NULL;
+        w.pk_hi = (__nv_bfloat16*)out[1]; w.pk_lo = w.pk_hi + pl.pack_floats;
+      }
+      return prepare_weights(pl, w, F32(in[1]), st);
+    }
+    case 11: return weight_norm_backward_all(pl, F32(in[1]), F32(in[2]), O32(out[0]), st);
+    case 15: return sdf_head(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), (int)d[1], (int)d[2], st);
+    case 16: return color_heads(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), st);
+    case 17: return nbar_add_color(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), st);
+    case 20: return heads_dgrad(pl, F32(in[1]), F32(in[2]), F32(in[3]), d[0], O32(out[0]), pair(out[1], pl.Hc), st);
+    case 21:
+      return chain_start(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), O32(out[1]), pair(out[2], pl.sdf[pl.L - 1].Np),
+                         st);
+    case 22: return normals(pl, F32(in[1]), d[0], O32(out[0]), O32(out[1]), st);
+    case 23: return dge(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), O32(out[1]), pair(out[2], pl.sdf[0].Kp), st);
+    case 24: {
+      const int l = (int)d[1];
+      if (l < 1 || l > pl.L || !pl.sdf[l].skip) return AVC_E_BADCFG;
+      return fill_gebar(pl, l, F32(in[1]), d[0], O32(out[0]), pair(out[1], pl.sdf[l].Kp), st);
+    }
+    case 26: return assemble_sdf_feat(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), st);
   }
   return AVC_E_BADCFG;
 }
@@ -1015,9 +1214,7 @@ int avc_neus_sdf_query(const avc_neus_cfg* cfg, const float* params, const float
   EncodeTargets t = make_targets(pl, w);
   for (int64_t p0 = 0; p0 < P; p0 += cap) {
     int64_t n = (P - p0) < cap ? (P - p0) : cap;
-    k_encode_points<<<blocks_for(n * 8, 256), 256, 0, st>>>(pts + p0 * 3, n, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E,
-                                                        pl.EP, t);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(encode_points(pts + p0 * 3, n, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E, pl.EP, t, st));
     AVC_TRY(value_chain(pl, w, n, false, false, sdf_out + p0, st));
   }
   return 0;
@@ -1025,24 +1222,6 @@ int avc_neus_sdf_query(const avc_neus_cfg* cfg, const float* params, const float
 
 // SDFNetwork.forward / .sdf_hidden_appearance / .gradient (models/fields.py:72-107) on arbitrary points: convenience
 // evaluators of the boundary (not on the training path).  Always the exact-fp32 tiles (engine 0).
-namespace {
-__global__ void k_points_to_cin(const float* __restrict__ pts, int64_t P, float* __restrict__ cin) {
-  int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= P) return;
-  float4* c = reinterpret_cast<float4*>(cin + (size_t)p * 8);
-  c[0] = make_float4(pts[p * 3], pts[p * 3 + 1], pts[p * 3 + 2], 0.f);
-  c[1] = make_float4(0.f, 0.f, 0.f, 0.f);
-}
-__global__ void k_assemble_sdf_feat(const float* __restrict__ sdf, const float* __restrict__ feat, int Fp, int F, int64_t P,
-                                    float* __restrict__ out) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P * (F + 1)) return;
-  int64_t p = i / (F + 1);
-  int c = (int)(i - p * (F + 1));
-  out[i] = c == 0 ? sdf[p] : feat[(size_t)p * Fp + (c - 1)];
-}
-}  // namespace
-
 int avc_neus_sdf_eval(const avc_neus_cfg* cfg_in, const float* params, const float* pts, int64_t P, float* sdf_feat_out,
                       float* grad_out, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
   if (!cfg_in || !params || !pts || !workspace) return AVC_E_NULL;
@@ -1071,16 +1250,10 @@ int avc_neus_sdf_eval(const avc_neus_cfg* cfg_in, const float* params, const flo
   EncodeTargets t = make_targets(pl, w);
   for (int64_t p0 = 0; p0 < P; p0 += cap) {
     int64_t n = (P - p0) < cap ? (P - p0) : cap;
-    k_encode_points<<<blocks_for(n * 8, 256), 256, 0, st>>>(pts + p0 * 3, n, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E,
-                                                        pl.EP, t);
-    k_points_to_cin<<<blocks_for(n, 256), 256, 0, st>>>(pts + p0 * 3, n, w.cin);
-    AVC_LAUNCH_TRY();
+    AVC_TRY(encode_points(pts + p0 * 3, n, pl.cfg.sdf_scale, pl.cfg.sdf_multires, pl.E, pl.EP, t, st));
+    AVC_TRY(points_to_cin(pts + p0 * 3, n, w.cin, st));
     AVC_TRY(value_chain(pl, w, n, grad_out != nullptr, sdf_feat_out != nullptr, w.sdf, st));
-    if (sdf_feat_out) {
-      k_assemble_sdf_feat<<<blocks_for(n * (pl.F + 1), 256), 256, 0, st>>>(w.sdf, w.feat, pl.Fp, pl.F, n,
-                                                                          sdf_feat_out + p0 * (pl.F + 1));
-      AVC_LAUNCH_TRY();
-    }
+    if (sdf_feat_out) AVC_TRY(assemble_sdf_feat(pl, w.sdf, w.feat, n, sdf_feat_out + p0 * (pl.F + 1), st));
     if (grad_out) AVC_TRY(gradient_chain(pl, w, n, grad_out + p0 * 3, st));
   }
   return 0;

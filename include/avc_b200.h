@@ -452,7 +452,7 @@ int avc_tc_nt_last_ring(void);
 int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int32_t N, int32_t K, int32_t Nv,
                     const float* X, float* Y, int32_t ldx, const float* v1, const float* v2, float s, float s2, float* OUT,
                     float* OUT2, int32_t ld2, void* workspace, size_t workspace_bytes, avc_stream_t stream);
-/* One compositing, scalar or placement kernel of the NeuS path (avc_neus_kernels.cuh) on caller buffers, launched by the
+/* One kernel of the NeuS path outside the GEMM tiles (avc_neus_kernels.cuh) on caller buffers, launched by the
  * host helpers the render uses.  dims is a HOST int64 array, fscal a HOST float array, in / out HOST arrays of DEVICE
  * pointers (all fp32).  An input marked "or NULL" may be NULL exactly where the render passes NULL.  ctx is the [4+]
  * scalar block {inv_s, eik_num, eik_den, invs_bar}; the kinds add into its sums as the render does.
@@ -471,7 +471,33 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
  *   7 k_upsample       dims {n (2..256), pitch, Rc, per (1..64)};  fscal {inv_s};  in {rays_o, rays_d, z[Rc][pitch],
  *     sdf[Rc][pitch]};  out {newz[Rc][per]}
  *   8 k_merge          dims {n (<= 256), pitch, Rc, per (<= 64), pitch_o >= n + per};  in {z[Rc][pitch], sdf[Rc][pitch],
- *     newz[Rc][per], news[Rc][per] or NULL};  out {zo[Rc][pitch_o], so[Rc][pitch_o] (unused when news is NULL)} */
+ *     newz[Rc][per], news[Rc][per] or NULL};  out {zo[Rc][pitch_o], so[Rc][pitch_o] (unused when news is NULL)}
+ * A "pair" output is the two-term bf16 split of a [rows][ld] activation as ONE bf16 buffer [rows][2 ld]: hi in columns
+ * [0, ld), lo in [ld, 2 ld) of each row; NULL where the render passes no split.  Kinds 9..11, 15..17, 20..24 and 26 run
+ * on a whole configuration: in[0] is a HOST avc_neus_cfg, the widths and pitches below are those of its plan (K_l, Kp_l,
+ * Np_l of SDF linear l; E, EP the encoded width and its pitch; Hc, F), pack is what kind 10 writes.  dims[0] = P.
+ *   9 pack layout       out {HOST int64 [16 + 11 (L + Lc + 3)]}: {L, Lc, E, EP, F, Fp, Hc, pack_floats, n_params,
+ *     off_var, pk_wsdf, pk_bsdf, pk_c0x, pk_c0xT, pk_W6, pk_b6}, then per SDF linear 0..L, colour linear 0..Lc and
+ *     extra_lin: {K, N, Kp, Np, skip, off_g, off_v, off_b, pk_W, pk_WT, pk_b}
+ *  10 prepare_weights   in {cfg, params};  out {pack[pack_floats], engine 1: pk pair [2 pack_floats] (hi, then lo)}
+ *  11 k_wn_backward     in {cfg, params, wbar[n_params]};  out {grads[n_params]} (the g / v / bias slots of every linear)
+ *  12 k_encode_points, 13 k_encode_samples, 14 k_encode_fine: dims {multires, ld0, n_skip (<= 4), skip_ld[4],
+ *     skip_col[4], then 12: P; 13: nz, pitch, Rc; 14: S, Rc};  fscal {scale, 14: sample_dist};  in {12: pts[P][3];
+ *     13: rays_o, rays_d, z[Rc][pitch]; 14: rays_o, rays_d, z_vals[Rc][S]};  out {in0[P][ld0] or NULL, skip[4] fp32
+ *     [P][skip_ld] or NULL, in0 pair or NULL, skip pairs[4] or NULL, 14: cin[P][8], mid_z[P] or NULL, inside[P] or NULL}
+ *  15 k_thin_nt<1, OutSdf> (value chain's sdf head)  dims {P, nz, pitch};  in {cfg, in_L[P][Kp_L], pack};  out {sdf}
+ *  16 k_thin_nt<6, OutHeads>   in {cfg, ch[P][Hc], pack};  out {rgb6[P][8]}
+ *  17 k_thin_nt<6, OutNbarAdd> in {cfg, cbar[P][Hc], pack};  out {nbar[P][4] (added into)}
+ *  18 k_thin_tn<NI>     dims {NI (1 | 6), lds, ldh, NC, P, si, sc, split};  fscal {s_scale};  in {S[P][lds], Hm[P][ldh]};
+ *     out {out, bout or NULL, out2 or NULL, bout2 or NULL} (added into)
+ *  19 k_colsum          dims {ld, NC, P};  fscal {scale};  in {X[P][ld]};  out {out[NC] (added into)}
+ *  20 k_heads_dgrad     in {cfg, y6bar[P][8], pack, ch[P][Hc]};  out {cbar[P][Hc] or NULL, pair or NULL}
+ *  21 k_chain_start     in {cfg, pack, sp'(z)[P][Np_{L-1}]};  out {qt[P][Np_{L-1}] or NULL, ge[P][EP], pair or NULL}
+ *  22 k_normal          in {cfg, ge[P][EP]};  out {cin[P][8] (x read from 0:3, n written to 3:6), grad[P][3] or NULL}
+ *  23 k_dge             in {cfg, cin[P][8], nbar[P][4]};  out {ubar0[P][Kp_0] or NULL, gebar[P][EP], pair or NULL}
+ *  24 k_fill_gebar      dims {P, l (a skip layer)};  in {cfg, gebar[P][EP]};  out {ubar_l[P][Kp_l], pair or NULL}
+ *  25 k_points_to_cin   dims {P};  in {pts[P][3]};  out {cin[P][8]}
+ *  26 k_assemble_sdf_feat  in {cfg, sdf[P], feat[P][Fp]};  out {[P][F + 1]} */
 int avc_neus_kernel_test(int32_t kind, const int64_t* dims, const float* fscal, const void* const* in, void* const* out,
                          avc_stream_t stream);
 /* One kernel of the CLIP towers (avc_clip.cu) on caller buffers, launched by the host code the towers use (the GEMMs

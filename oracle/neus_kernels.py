@@ -1,11 +1,12 @@
-"""float64 references of the NeuS compositing, scalar and placement kernels (avc_neus_kernels.cuh), one function per
-kernel, taking the fp32 inputs the kernel reads.  They run on whatever device the inputs live on.
+"""float64 references of the NeuS kernels outside the GEMM tiles (avc_neus_kernels.cuh): compositing, scalars,
+placement, weight packing and its backward, the encoding, the thin contractions and the ends of the gradient chain.
+One function per kernel, taking the fp32 inputs the kernel reads.  They run on whatever device the inputs live on.
 
 The compositing forward is oracle.neus.composite itself; its backward is fp64 autograd through it, so the kernels'
 hand-derived backward is checked against an independent derivation.  Where a kernel rounds on purpose like torch eager
-fp32 (depth placement, mid-points, sample points, the ``radius < 1`` mask), the rounding is restated here as separately
-rounded fp32 operations, and the GPU tests compare those outputs exactly.  tests/test_neus_kernels_cpu.py pins each
-function against torch."""
+fp32 (depth placement, mid-points, sample points, the ``radius < 1`` mask, y = scale x, the sqrt(1/2) skip copies), the
+rounding is restated here as separately rounded fp32 operations, and the GPU tests compare those outputs exactly.
+tests/test_neus_kernels_cpu.py pins each function against torch."""
 from __future__ import annotations
 
 from typing import Dict, Optional
@@ -233,3 +234,122 @@ def merge(z, sdf, newz, news):
     zs, idx = torch.sort(torch.cat([z, newz], -1), dim=-1, stable=True)
     so = None if news is None else torch.cat([sdf, news], -1).gather(1, idx)
     return zs, so
+
+
+# --------------------------------------------------------------------------- weights
+def effective_weight(v, g, dtype=F64) -> torch.Tensor:
+    """k_pack_linear: W = g v / ||v|| per output row (torch.nn.utils.weight_norm, dim=0).  v [N,K], g [N] or [N,1]."""
+    return neus.effective_weight({"w.weight_v": v.to(dtype), "w.weight_g": g.to(dtype).reshape(-1, 1)}, "w")
+
+
+def wn_backward(v, g, wbar, dtype=F64):
+    """k_wn_backward: with vhat = v / ||v||, gbar = sum_k Wbar vhat and vbar = g / ||v|| (Wbar - gbar vhat).  The bias
+    gradient is a copy of the dense one (compared exactly).  Returns (gbar [N], vbar [N,K])."""
+    v, g, wbar = v.to(dtype), g.to(dtype).reshape(-1, 1), wbar.to(dtype)
+    nv = v.norm(dim=1, keepdim=True)
+    vh = v / nv
+    gbar = (wbar * vh).sum(1, keepdim=True)
+    return gbar.reshape(-1), g / nv * (wbar - gbar * vh)
+
+
+# --------------------------------------------------------------------------- encoding
+def scaled(x, scale: float) -> torch.Tensor:
+    """y = scale x rounded to fp32, the input of every sin / cos of the encoding kernels."""
+    return x.float() * torch.tensor(scale, dtype=torch.float32)
+
+
+def encode(x, scale: float, multires: int, dtype=F64) -> torch.Tensor:
+    """encode_group: positional_encode(y) of the fp32 y = scale x, in ``dtype``.  x [P,3] -> [P, 3 (1 + 2 multires)]."""
+    return neus.positional_encode(scaled(x, scale).to(dtype), multires)
+
+
+def skip_copy(e32: torch.Tensor) -> torch.Tensor:
+    """The skip layers' copy of an fp32 encoding: each value times the fp32 sqrt(1/2), rounded once."""
+    return e32.float() * torch.tensor(0.70710678118654752440, dtype=torch.float32)
+
+
+def sample_points(rays_o, rays_d, z) -> torch.Tensor:
+    """k_encode_samples' points o + d z in torch eager fp32 (renderer.py:182, :337).  z [R,n] -> [R,n,3]."""
+    return rays_o[:, None, :] + rays_d[:, None, :] * z[..., None]
+
+
+def inside_sphere(x) -> torch.Tensor:
+    """renderer.py:219: (||x|| < 1) with the norm rounded like the kernel (radius_f32)."""
+    return (radius_f32(x) < 1.0).float()
+
+
+# --------------------------------------------------------------------------- thin contractions
+def sdf_head(in_l, K: int, wsdf, bsdf, scale: float, dtype=F64) -> torch.Tensor:
+    """k_thin_nt<1, OutSdf>: (in_L[:, :K] . w_sdf + b_sdf) / scale: only the K inputs of the last linear."""
+    return (in_l[:, :K].to(dtype) @ wsdf[:K].to(dtype) + bsdf.to(dtype).reshape(())) / scale
+
+
+def color_heads(ch, W6, b6, dtype=F64) -> torch.Tensor:
+    """k_thin_nt<6, OutHeads>: sigmoid(ch W6[0:6]^T + b6[0:6]) -> [P,6]."""
+    return torch.sigmoid(ch.to(dtype) @ W6[0:6].to(dtype).T + b6[0:6].to(dtype))
+
+
+def nbar_add(nbar, cbar, c0xT, dtype=F64) -> torch.Tensor:
+    """k_thin_nt<6, OutNbarAdd>: nbar[:, 0:3] + cbar W0[:, 3:6]; c0xT is the packed [8][Hc] transpose of lin0's first
+    columns."""
+    return nbar[:, 0:3].to(dtype) + cbar.to(dtype) @ c0xT[3:6].to(dtype).T
+
+
+def thin_tn(S, Hm, s_scale: float = 1.0, dtype=F64):
+    """k_thin_tn: (s_scale S)^T Hm -> [NI, NC] and the bias sum sum_p s_scale S[p] -> [NI]."""
+    Ss = S.to(dtype) * s_scale
+    return Ss.T @ Hm.to(dtype), Ss.sum(0)
+
+
+def colsum(X, scale: float = 1.0, dtype=F64) -> torch.Tensor:
+    """k_colsum: scale sum_p X[p]."""
+    return X.to(dtype).sum(0) * scale
+
+
+def heads_dgrad(y6bar, W6, h, dtype=F64) -> torch.Tensor:
+    """k_heads_dgrad: (y6bar[:, 0:6] W6[0:6]) [h > 0] (ReLU' (0) = 0)."""
+    return (y6bar[:, 0:6].to(dtype) @ W6[0:6].to(dtype)) * (h > 0).to(dtype)
+
+
+# --------------------------------------------------------------------------- gradient chain
+SQRT_HALF = 0.70710678118654752440
+
+
+def chain_start(wsdf, zprev, n_prev: int, K_last: int, skip_last: bool, E: int, dtype=F64):
+    """k_chain_start: qt_{L-1} = sp'(z_{L-1}) * w_sdf[0:N_{L-1}] (times sqrt(1/2) when the last linear takes the skip
+    concat) and ge = the encoding part of w_sdf, w_sdf[K-E:K] sqrt(1/2), or 0.  Returns (qt [P, n_prev], ge [P, E])."""
+    s = SQRT_HALF if skip_last else 1.0
+    w = wsdf.to(dtype)
+    qt = zprev[:, :n_prev].to(dtype) * w[:n_prev] * s
+    P = zprev.shape[0]
+    ge = (w[K_last - E:K_last] * s).expand(P, E) if skip_last else torch.zeros(P, E, dtype=dtype, device=zprev.device)
+    return qt, ge
+
+
+def _bands(x, scale: float, multires: int, dtype):
+    y = scaled(x, scale).to(dtype)
+    return [(float(2 ** k), torch.sin(y * 2 ** k), torch.cos(y * 2 ** k)) for k in range(multires)]
+
+
+def normal(ge, x, scale: float, multires: int, dtype=F64) -> torch.Tensor:
+    """k_normal: n = D(y)^T ge with D the Jacobian of positional_encode at y = scale x (the scale of y and the 1 / scale
+    of the sdf cancel).  ge [P, >= E], x [P,3] -> [P,3]."""
+    g = ge.to(dtype)
+    n = g[:, 0:3].clone()
+    for k, (f, sn, cs) in enumerate(_bands(x, scale, multires, dtype)):
+        n = n + f * (cs * g[:, 3 + 6 * k:6 + 6 * k] - sn * g[:, 6 + 6 * k:9 + 6 * k])
+    return n
+
+
+def dge(x, nbar, scale: float, multires: int, dtype=F64) -> torch.Tensor:
+    """k_dge: gebar = D(y) nbar -> [P, E] (the same Jacobian as ``normal``, applied forward)."""
+    nb = nbar[:, 0:3].to(dtype)
+    cols = [nb]
+    for f, sn, cs in _bands(x, scale, multires, dtype):
+        cols += [f * cs * nb, -f * sn * nb]
+    return torch.cat(cols, -1)
+
+
+def fill_gebar(gebar, E: int) -> torch.Tensor:
+    """k_fill_gebar: the skip half of ubar, fp32 gebar[:, 0:E] times the fp32 sqrt(1/2), rounded once."""
+    return skip_copy(gebar[:, 0:E])

@@ -1,5 +1,6 @@
-"""The float64 references of the NeuS compositing, scalar and placement kernels (oracle/neus_kernels.py) against
-torch: autograd through oracle.neus in fp64, torch's conventions the kernels adopt (clip / clamp backward inclusive at
+"""The float64 references of the NeuS kernels outside the GEMM tiles (oracle/neus_kernels.py) against torch: autograd
+through oracle.neus in fp64 (and, for packing, encoding, thin contractions and the gradient chain, torch._weight_norm,
+the JVP / VJP of positional_encode, F.linear and oracle.neus.sdf_gradient), torch's conventions the kernels adopt (clip / clamp backward inclusive at
 the bounds, ReLU' (0) = 0, first-index max, searchsorted(right=True), at::linspace), and the deliberate rounding
 (bf16 split, separately rounded fp32 placement arithmetic) against hand-written bit patterns."""
 import math
@@ -227,3 +228,143 @@ def test_upsample_reference_matches_oracle():
     ref = neus.up_sample(o.double(), d.double(), z.double(), sdf.double(), per, 64.0)
     # the oracle takes the radius mask in fp64 and its u from an fp64 linspace: equal wherever neither matters
     assert (got - ref).abs().max().item() < 1e-6
+
+
+# --------------------------------------------------------------------------- weights, encoding, thin ops, gradient chain
+def _wide_rows(N, K, seed):
+    """Weight rows over six decades, negative g, and (for the backward) a Wbar row orthogonal to its v row."""
+    g = torch.Generator().manual_seed(seed)
+    v = torch.randn(N, K, generator=g, dtype=F64) * torch.logspace(-3, 3, N, dtype=F64)[:, None]
+    gg = torch.randn(N, generator=g, dtype=F64) * 3
+    gg[0] = -abs(gg[0])
+    wbar = torch.randn(N, K, generator=g, dtype=F64)
+    wbar[1] -= (wbar[1] @ v[1]) / (v[1] @ v[1]) * v[1]
+    return v, gg, wbar
+
+
+def test_pack_and_wn_backward_match_torch_weight_norm():
+    v, gg, wbar = _wide_rows(7, 45, 0)
+    vv, g2 = v.clone().requires_grad_(True), gg.reshape(-1, 1).clone().requires_grad_(True)
+    W = torch._weight_norm(vv, g2, 0)
+    assert (nk.effective_weight(v, gg) - W.detach()).abs().max().item() <= 1e-14 * W.abs().max().item()
+    gv, gg_ = torch.autograd.grad((W * wbar).sum(), [vv, g2])
+    gbar, vbar = nk.wn_backward(v, gg, wbar)
+    assert (gbar - gg_.reshape(-1)).abs().max().item() <= 1e-12 * gg_.abs().max().item()
+    for n in range(7):      # per row: the rows span six decades
+        assert (vbar[n] - gv[n]).abs().max().item() <= 1e-12 * gv[n].abs().max().item()
+    assert abs(gbar[1].item()) <= 1e-12 * wbar[1].norm().item()        # Wbar orthogonal to v: no g gradient
+
+
+def _edge_points(P, seed):
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(P, 3, generator=g) * 0.6
+    x[0] = 0.0                                          # the origin
+    x[1] = torch.tensor([1.0, 0.0, 0.0])                # exactly on |x| = 1
+    x[2] = torch.tensor([0.0, -1.0, 0.0])
+    return x
+
+
+@pytest.mark.parametrize("multires", [0, 1, 6, 7, 10])
+@pytest.mark.parametrize("scale", [0.5, 1.0, 2.0])
+def test_normal_and_dge_match_autograd_of_positional_encode(multires, scale):
+    """k_normal is the VJP and k_dge the JVP of x -> positional_encode(scale x), both divided by scale (the sdf carries
+    1 / scale)."""
+    P = 9
+    x = _edge_points(P, multires)
+    E = 3 * (1 + 2 * multires)
+    g = torch.Generator().manual_seed(100 + multires)
+    ge = torch.randn(P, E + 5, generator=g, dtype=F64)
+    nbar = torch.randn(P, 4, generator=g, dtype=F64)
+    nbar[3] = 0.0
+    enc = lambda xx: neus.positional_encode(xx * scale, multires)
+    assert torch.equal(nk.encode(x, scale, multires), enc(x.double()))       # scale is a power of 2: y exact
+    _, vjp = torch.func.vjp(enc, x.double())
+    (want_n,) = vjp(ge[:, :E])
+    got_n = nk.normal(ge, x, scale, multires)
+    assert (got_n - want_n / scale).abs().max().item() <= 1e-12 * max(1.0, want_n.abs().max().item())
+    _, want_g = torch.func.jvp(enc, (x.double(),), (nbar[:, 0:3],))
+    got_g = nk.dge(x, nbar, scale, multires)
+    assert got_g.shape == (P, E)
+    assert (got_g - want_g / scale).abs().max().item() <= 1e-12 * max(1.0, want_g.abs().max().item())
+    assert torch.all(got_g[3] == 0)
+
+
+def test_thin_contractions_match_linear_autograd():
+    g = torch.Generator().manual_seed(8)
+    P, Hc, K = 37, 20, 44
+    F_ = torch.nn.functional
+    # sdf head: F.linear over the first K inputs, divided by scale
+    inl = torch.randn(P, K + 4, generator=g, dtype=F64)
+    w, b = torch.randn(K + 4, generator=g, dtype=F64), torch.randn(1, generator=g, dtype=F64)
+    want = F_.linear(inl[:, :K], w[:K].reshape(1, K), b).reshape(-1) / 2.0
+    assert (nk.sdf_head(inl, K, w, b, 2.0) - want).abs().max().item() <= 1e-13
+    # heads: sigmoid of two linears on one activation; heads_dgrad = d/d pre-activation through the ReLU
+    pre = torch.randn(P, Hc, generator=g, dtype=F64)
+    pre[::3, 2] = 0.0                                   # h exactly 0 at the ReLU mask
+    W6 = torch.randn(8, Hc, generator=g, dtype=F64)
+    b6 = torch.randn(8, generator=g, dtype=F64)
+    pr = pre.clone().requires_grad_(True)
+    y = F_.linear(torch.relu(pr), W6[0:6], b6[0:6])
+    assert (nk.color_heads(torch.relu(pre), W6, b6) - torch.sigmoid(y.detach())).abs().max().item() <= 1e-14
+    y6bar = torch.randn(P, 8, generator=g, dtype=F64)
+    (gp,) = torch.autograd.grad((y * y6bar[:, 0:6]).sum(), pr)
+    assert (nk.heads_dgrad(y6bar, W6, torch.relu(pre)) - gp).abs().max().item() <= 1e-13
+    # weight / bias gradients of F.linear: thin_tn (with s_scale) and colsum
+    hm = torch.randn(P, Hc, generator=g, dtype=F64)
+    Wl = torch.randn(6, Hc, generator=g, dtype=F64, requires_grad=True)
+    bl = torch.randn(6, generator=g, dtype=F64, requires_grad=True)
+    S = torch.randn(P, 6, generator=g, dtype=F64)
+    gw, gb = torch.autograd.grad((F_.linear(hm, Wl, bl) * S * 0.5).sum(), [Wl, bl])
+    tw, tb = nk.thin_tn(S, hm, 0.5)
+    assert (tw - gw).abs().max().item() <= 1e-13 and (tb - gb).abs().max().item() <= 1e-13
+    assert (nk.colsum(S, 0.5) - gb).abs().max().item() <= 1e-13
+    # nbar += cbar W0[:, 3:6]: the adjoint of colour lin0's normal inputs
+    cin6 = torch.randn(P, 6, generator=g, dtype=F64, requires_grad=True)
+    W0x = torch.randn(Hc, 6, generator=g, dtype=F64)
+    cbar = torch.randn(P, Hc, generator=g, dtype=F64)
+    (gc,) = torch.autograd.grad((F_.linear(cin6, W0x) * cbar).sum(), cin6)
+    c0xT = torch.zeros(8, Hc, dtype=F64)
+    c0xT[0:6] = W0x.T
+    nb = torch.randn(P, 4, generator=g, dtype=F64)
+    assert (nk.nbar_add(nb, cbar, c0xT) - (nb[:, 0:3] + gc[:, 3:6])).abs().max().item() <= 1e-13
+
+
+def _softplus_d1(z):
+    return torch.where(z * 100.0 > 20.0, torch.ones_like(z), torch.sigmoid(z * 100.0))
+
+
+@pytest.mark.parametrize("skip_in,multires,scale", [((2,), 6, 1.0), ((3,), 10, 2.0), ((1, 3), 7, 0.5), ((), 0, 2.0)])
+def test_gradient_chain_references_match_sdf_gradient(skip_in, multires, scale):
+    """k_chain_start -> the reverse sweep of the EpiChain GEMMs -> k_normal, composed from the references, is
+    oracle.neus.sdf_gradient (autograd of SDFNetwork.forward) on a small network."""
+    conf = neus.SDFConf(d_out=9, d_hidden=76, n_layers=3, skip_in=skip_in, multires=multires, scale=scale)
+    g = torch.Generator().manual_seed(multires)
+    p = {k: v.double() + 0.05 * torch.randn(v.shape, generator=g, dtype=F64)
+         for k, v in neus.init_sdf_params(conf, g).items()}
+    x = _edge_points(11, 1).double()
+    want = neus.sdf_gradient(p, conf, x.clone(), create_graph=False)
+    L, E = conf.n_layers, conf.d_enc
+    W = [neus.effective_weight(p, f"lin{l}") for l in range(L + 1)]
+    enc = neus.positional_encode(x * scale, multires)
+    h, d1 = enc, []
+    for l in range(L + 1):
+        if l in skip_in:
+            h = torch.cat([h, enc], -1) / math.sqrt(2)
+        z = torch.nn.functional.linear(h, W[l], p[f"lin{l}.bias"])
+        if l < L:
+            d1.append(_softplus_d1(z))
+            h = neus.softplus100(z)
+    n_prev = W[L - 1].shape[0]
+    qt, ge = nk.chain_start(W[L][0], d1[L - 1], n_prev, W[L].shape[1], L in skip_in, E)
+    ge = ge.clone()
+    for l in range(L - 1, 0, -1):
+        u = qt @ W[l]
+        if l in skip_in:
+            np_ = W[l - 1].shape[0]
+            ge = ge + u[:, np_:] * nk.SQRT_HALF
+            u = u[:, :np_] * nk.SQRT_HALF
+        qt = d1[l - 1] * u
+    ge = ge + qt @ W[0]
+    got = nk.normal(ge, x, scale, multires)
+    assert (got - want).abs().max().item() <= 1e-12 * max(1.0, want.abs().max().item())
+
