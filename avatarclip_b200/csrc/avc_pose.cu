@@ -1,0 +1,794 @@
+// avc_pose.cu -- AvatarAnimate's pose stage (models/pose_generation.py, general.mode = pose): candidate SMPL body poses
+// from a text prompt, scored by CLIP on textured renders.
+//
+//   avc_vposer_decode          VPoser 2.x decode: decoder_net (Linear, LeakyReLU, Linear, LeakyReLU, Linear) then the
+//                              6D -> matrix (Gram-Schmidt) -> quaternion -> axis-angle tail (matrot2aa), one kernel per
+//                              tile of rows
+//   avc_realnvp_pack           the coupling nets' weights transposed for avc_realnvp_decode, once per checkpoint
+//   avc_realnvp_decode         VPoserRealNVP.decode (:233-240): the 8 conditional coupling blocks, the text feature folded
+//                              into each first linear's bias once per call, the whole chain in one kernel per tile of rows
+//   avc_smpl_pose_batch        smplx SMPL with zero betas for B body poses: pose blend shapes, kinematic chain, skinning;
+//                              each row is what avc_lbs_fwd computes for it (same arithmetic, same order)
+//   avc_raster_textured_batch  render.py:10-39's renders of B meshes from A eyes per group of rows, one launch per pass
+//                              for the whole batch; each image is what avc_raster_textured makes of it
+//   avc_cosine_topk            F.cosine_similarity of N rows against one vector + torch.topk (VPoserCodebook :322-324)
+//   avc_pose_suppress          VPoserCodebook.suppress_duplicated_poses (:304-317)
+//   avc_pose_score             get_pose_feature's mean over the cameras, calculate_pose_score's cosine, get_pose's
+//                              per-batch argmax (:88-89, 94, 273-274)
+#include <cfloat>
+#include <vector>
+
+#include "avc_common.cuh"
+#include "avc_raster.cuh"
+
+using namespace avc;
+
+namespace {
+
+constexpr float kLeaky = 0.01f;      // nn.LeakyReLU() default slope
+constexpr int kVpRows = 8;           // VPoser rows per CTA
+constexpr int kVpMaxH = 512;
+constexpr int kVpMaxL = 64;
+constexpr int kVpMaxOut = 192;       // 6 x up to 32 joints
+constexpr int kNvpRows = 16;         // RealNVP rows per CTA
+constexpr int kNvpMaxD = 32;
+constexpr int kNvpMaxH = 256;
+constexpr int kNvpMaxBlocks = 16;
+constexpr int kMaxCams = 16;
+constexpr int kSupMax = 64;
+constexpr int kSupMaxD = 96;
+constexpr int NJ_MAX = 32;
+
+// Wt[k][n] = W[n][col0 + k] for k < K  (W row-major with leading dimension ldw)
+__global__ void k_transpose(const float* __restrict__ W, int N, int K, int ldw, int col0, float* __restrict__ Wt) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N * K) return;
+  int k = i / N, n = i - k * N;
+  Wt[i] = W[(size_t)n * ldw + col0 + k];
+}
+
+// out[r][j] = act(sum_k in[r][k] Wt[k][j] + bias[j]) for ROWS rows held in shared memory; act 0 none, 1 LeakyReLU,
+// 2 tanh.  Threads stride over j; each weight is read once per CTA (coalesced along j).
+template <int ROWS>
+__device__ __forceinline__ void dense_rows(const float* in, int ldi, int K, const float* __restrict__ Wt, int N,
+                                           const float* __restrict__ bias, int act, float* out, int ldo) {
+  for (int j = threadIdx.x; j < N; j += blockDim.x) {
+    float acc[ROWS];
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) acc[r] = 0.f;
+    for (int k = 0; k < K; ++k) {
+      const float w = Wt[(size_t)k * N + j];
+#pragma unroll
+      for (int r = 0; r < ROWS; ++r) acc[r] = fmaf(in[r * ldi + k], w, acc[r]);
+    }
+    const float b = bias[j];
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) {
+      float v = acc[r] + b;
+      if (act == 1) v = v > 0.f ? v : kLeaky * v;
+      else if (act == 2) v = tanhf(v);
+      out[r * ldo + j] = v;
+    }
+  }
+}
+
+// ---------------------------------------------------------------- VPoser decode
+// ContinousRotReprDecoder + matrot2aa (torchgeometry rotation_matrix_to_quaternion / quaternion_to_angle_axis) of one
+// joint: x[6] read as a [3][2] matrix, columns a = (x0, x2, x4), c = (x1, x3, x5).
+__device__ __forceinline__ void rot6d_to_aa(const float* x, float* aa, float* rm) {
+  float a[3] = {x[0], x[2], x[4]}, c[3] = {x[1], x[3], x[5]};
+  float na = fmaxf(sqrtf(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]), 1e-12f);     // F.normalize
+  float b1[3] = {a[0] / na, a[1] / na, a[2] / na};
+  float dot = b1[0] * c[0] + b1[1] * c[1] + b1[2] * c[2];
+  float u[3] = {c[0] - dot * b1[0], c[1] - dot * b1[1], c[2] - dot * b1[2]};
+  float nu = fmaxf(sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]), 1e-12f);
+  float b2[3] = {u[0] / nu, u[1] / nu, u[2] / nu};
+  float b3[3] = {b1[1] * b2[2] - b1[2] * b2[1], b1[2] * b2[0] - b1[0] * b2[2], b1[0] * b2[1] - b1[1] * b2[0]};
+  // R = stack([b1, b2, b3], -1): R[i][j] = b_j[i]
+  float R[9] = {b1[0], b2[0], b3[0], b1[1], b2[1], b3[1], b1[2], b2[2], b3[2]};
+  if (rm)
+#pragma unroll
+    for (int i = 0; i < 9; ++i) rm[i] = R[i];
+  // rmat_t = R^T: m(i, j) = R[j][i]
+#define M(i, j) R[(j) * 3 + (i)]
+  float q[4], t;
+  if (M(2, 2) < 1e-6f) {
+    if (M(0, 0) > M(1, 1)) {
+      t = 1.f + M(0, 0) - M(1, 1) - M(2, 2);
+      q[0] = M(1, 2) - M(2, 1); q[1] = t; q[2] = M(0, 1) + M(1, 0); q[3] = M(2, 0) + M(0, 2);
+    } else {
+      t = 1.f - M(0, 0) + M(1, 1) - M(2, 2);
+      q[0] = M(2, 0) - M(0, 2); q[1] = M(0, 1) + M(1, 0); q[2] = t; q[3] = M(1, 2) + M(2, 1);
+    }
+  } else {
+    if (M(0, 0) < -M(1, 1)) {
+      t = 1.f - M(0, 0) - M(1, 1) + M(2, 2);
+      q[0] = M(0, 1) - M(1, 0); q[1] = M(2, 0) + M(0, 2); q[2] = M(1, 2) + M(2, 1); q[3] = t;
+    } else {
+      t = 1.f + M(0, 0) + M(1, 1) + M(2, 2);
+      q[0] = t; q[1] = M(1, 2) - M(2, 1); q[2] = M(2, 0) - M(0, 2); q[3] = M(0, 1) - M(1, 0);
+    }
+  }
+#undef M
+  const float st = sqrtf(t);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) q[i] = (q[i] / st) * 0.5f;
+  const float s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  const float s = sqrtf(s2), co = q[0];
+  const float two_theta = 2.f * (co < 0.f ? atan2f(-s, -co) : atan2f(s, co));
+  const float k = s2 > 0.f ? two_theta / s : 2.f;
+  aa[0] = q[1] * k; aa[1] = q[2] * k; aa[2] = q[3] * k;
+}
+
+struct VpWeights {
+  const float *w1t, *b1, *w2t, *b2, *w3t, *b3;   // transposed [K][N] copies in the workspace, biases as given
+};
+
+__global__ void __launch_bounds__(256)
+k_vposer_decode(const float* __restrict__ z, int B, int L, int H, int NJ, VpWeights w, float* __restrict__ pose_out,
+                float* __restrict__ rotmat_out) {
+  __shared__ float sz[kVpRows * kVpMaxL];
+  __shared__ float sh1[kVpRows * kVpMaxH];
+  __shared__ float sh2[kVpRows * kVpMaxH];
+  __shared__ float so[kVpRows * kVpMaxOut];
+  const int row0 = blockIdx.x * kVpRows, O = NJ * 6;
+  for (int i = threadIdx.x; i < kVpRows * L; i += blockDim.x) {
+    const int r = i / L, row = row0 + r;
+    sz[i] = row < B ? z[(size_t)row * L + (i - r * L)] : 0.f;
+  }
+  __syncthreads();
+  dense_rows<kVpRows>(sz, L, L, w.w1t, H, w.b1, 1, sh1, H);       // decoder_net.0 + LeakyReLU (Dropout: eval)
+  __syncthreads();
+  dense_rows<kVpRows>(sh1, H, H, w.w2t, H, w.b2, 1, sh2, H);      // decoder_net.3 + LeakyReLU
+  __syncthreads();
+  dense_rows<kVpRows>(sh2, H, H, w.w3t, O, w.b3, 0, so, O);       // decoder_net.5
+  __syncthreads();
+  for (int i = threadIdx.x; i < kVpRows * NJ; i += blockDim.x) {
+    const int r = i / NJ, j = i - r * NJ, row = row0 + r;
+    if (row >= B) continue;
+    float aa[3];
+    rot6d_to_aa(so + r * O + j * 6, aa, rotmat_out ? rotmat_out + ((size_t)row * NJ + j) * 9 : nullptr);
+    float* p = pose_out + ((size_t)row * NJ + j) * 3;
+    p[0] = aa[0]; p[1] = aa[1]; p[2] = aa[2];
+  }
+}
+
+// ---------------------------------------------------------------- RealNVP decode
+// the transposed weights, packed once per checkpoint, per coupling net (block i, net n: 0 = s, 1 = t): w1t [D][H]
+// (the x columns of the first linear), w2t [H][H], w3t [H][D]
+struct NvpPack {
+  size_t w1t, w2t, w3t, stride;
+};
+
+__host__ __device__ inline NvpPack nvp_pack(int D, int H) {
+  NvpPack p;
+  p.w1t = 0;
+  p.w2t = p.w1t + (size_t)D * H;
+  p.w3t = p.w2t + (size_t)H * H;
+  p.stride = p.w3t + (size_t)H * D;
+  return p;
+}
+
+// params per net: W1 [H][D+E], b1 [H], W2 [H][H], b2 [H], W3 [D][H], b3 [D]
+__host__ __device__ inline size_t nvp_param_stride(int D, int E, int H) {
+  return (size_t)H * (D + E) + H + (size_t)H * H + H + (size_t)D * H + D;
+}
+
+// net blockIdx.y: the three transposes into its slot of the pack
+__global__ void k_realnvp_pack(const float* __restrict__ params, int D, int E, int H, float* __restrict__ pack) {
+  const float* W1 = params + (size_t)blockIdx.y * nvp_param_stride(D, E, H);
+  const float* W2 = W1 + (size_t)H * (D + E) + H;
+  const float* W3 = W2 + (size_t)H * H + H;
+  const NvpPack pk = nvp_pack(D, H);
+  float* P = pack + (size_t)blockIdx.y * pk.stride;
+  const int total = max(H * H, D * H);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    int k = i / H, n = i - k * H;
+    if (i < H * H) P[pk.w2t + i] = W2[(size_t)n * H + k];    // w2t[k][n] = W2[n][k]
+    if (i < D * H) {
+      P[pk.w1t + i] = W1[(size_t)n * (D + E) + k];            // w1t[k][n] = W1[n][k], k < D
+      const int k3 = i / D, n3 = i - k3 * D;
+      P[pk.w3t + i] = W3[(size_t)n3 * H + k3];                // w3t[k][n] = W3[n][k]
+    }
+  }
+}
+
+// c[net][j] = b1[j] + sum_e W1[j][D + e] f[e], one CTA per net
+__global__ void k_realnvp_fold(const float* __restrict__ params, const float* __restrict__ f, int D, int E, int H,
+                               float* __restrict__ fold) {
+  const float* W1 = params + (size_t)blockIdx.x * nvp_param_stride(D, E, H);
+  const float* b1 = W1 + (size_t)H * (D + E);
+  float* c = fold + (size_t)blockIdx.x * H;
+  for (int j = threadIdx.x; j < H; j += blockDim.x) {
+    const float* wr = W1 + (size_t)j * (D + E) + D;
+    float acc = 0.f;
+    for (int e = 0; e < E; ++e) acc = fmaf(wr[e], f[e], acc);
+    c[j] = acc + b1[j];
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_realnvp_decode(const float* __restrict__ z, int B, int D, int E, int H, int nb, const float* __restrict__ params,
+                 const float* __restrict__ pack, const float* __restrict__ fold, const float* __restrict__ mask,
+                 float* __restrict__ x_out) {
+  __shared__ float sx[kNvpRows * kNvpMaxD], sxm[kNvpRows * kNvpMaxD];
+  __shared__ float sh1[kNvpRows * kNvpMaxH], sh2[kNvpRows * kNvpMaxH];
+  __shared__ float ss[kNvpRows * kNvpMaxD], st[kNvpRows * kNvpMaxD];
+  const int row0 = blockIdx.x * kNvpRows;
+  for (int i = threadIdx.x; i < kNvpRows * D; i += blockDim.x) {
+    const int r = i / D, row = row0 + r;
+    sx[i] = row < B ? z[(size_t)row * D + (i - r * D)] : 0.f;
+  }
+  const NvpPack pk = nvp_pack(D, H);
+  const size_t ps = nvp_param_stride(D, E, H);
+  for (int blk = 0; blk < nb; ++blk) {
+    const float* m = mask + (size_t)blk * D;
+    __syncthreads();
+    for (int i = threadIdx.x; i < kNvpRows * D; i += blockDim.x) sxm[i] = sx[i] * m[i % D];   // x_ = x * mask
+    for (int net = 0; net < 2; ++net) {
+      const float* P = pack + (size_t)(blk * 2 + net) * pk.stride;
+      const float* W = params + (size_t)(blk * 2 + net) * ps;
+      const float* b2 = W + (size_t)H * (D + E) + H + (size_t)H * H;
+      const float* b3 = b2 + H + (size_t)D * H;
+      __syncthreads();
+      dense_rows<kNvpRows>(sxm, D, D, P + pk.w1t, H, fold + (size_t)(blk * 2 + net) * H, 1, sh1, H);
+      __syncthreads();
+      dense_rows<kNvpRows>(sh1, H, H, P + pk.w2t, H, b2, 1, sh2, H);
+      __syncthreads();
+      dense_rows<kNvpRows>(sh2, H, H, P + pk.w3t, D, b3, net == 0 ? 2 : 0, net == 0 ? ss : st, D);
+    }
+    __syncthreads();
+    // s, t = net(...) * (1 - mask);  x = x_ + (1 - mask) * (x * exp(s) + t)
+    for (int i = threadIdx.x; i < kNvpRows * D; i += blockDim.x) {
+      const float om = 1.f - m[i % D];
+      const float s = ss[i] * om, t = st[i] * om;
+      sx[i] = sxm[i] + om * (sx[i] * expf(s) + t);
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < kNvpRows * D; i += blockDim.x) {
+    const int r = i / D, row = row0 + r;
+    if (row < B) x_out[(size_t)row * D + (i - r * D)] = sx[i];
+  }
+}
+
+// ---------------------------------------------------------------- SMPL for a batch of body poses
+// J = J_regressor . v_template: the joint regression of k_lbs_joints_chain (avc_lbs.cu), same reduction order
+__global__ void __launch_bounds__(256)
+k_pose_joints(const float* __restrict__ v, const float* __restrict__ J_regressor, int V, int NJ, float* __restrict__ J) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int j = warp; j < NJ; j += nw) {
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    const float* jr = J_regressor + (size_t)j * V;
+    for (int i = lane; i < V; i += 32) {
+      float w = jr[i];
+      a0 = fmaf(w, v[i * 3 + 0], a0); a1 = fmaf(w, v[i * 3 + 1], a1); a2 = fmaf(w, v[i * 3 + 2], a2);
+    }
+    a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
+    if (lane == 0) { J[j * 3] = a0; J[j * 3 + 1] = a1; J[j * 3 + 2] = a2; }
+  }
+}
+
+struct Orient {
+  float r[3];
+};
+
+// one warp per pose row, lane j = joint j: batch_rodrigues of (global_orient, body_pose, zeros), the pose feature and
+// the kinematic chain of k_lbs_joints_chain, written per row: A [B][NJ][12], feat [B][(NJ-1)*9]
+__global__ void __launch_bounds__(128)
+k_pose_chain(const float* __restrict__ body_pose, int P, int B, Orient go, const float* __restrict__ Jg,
+             const int* __restrict__ parents, int NJ, float* __restrict__ A_out, float* __restrict__ feat_out) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;                        // warp-uniform
+  const int j = lane;
+  const bool act = j < NJ;
+  float* feat = feat_out + (size_t)b * (NJ - 1) * 9;
+  float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  if (act) {
+    float rv[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const int q = (j - 1) * 3 + c;
+      rv[c] = j == 0 ? go.r[c] : (q < P ? body_pose[(size_t)b * P + q] : 0.f);
+    }
+    float rx = rv[0], ry = rv[1], rz = rv[2];
+    const float eps = 1e-8f;
+    float ang = sqrtf((rx + eps) * (rx + eps) + (ry + eps) * (ry + eps) + (rz + eps) * (rz + eps));
+    float x = rx / ang, y = ry / ang, z = rz / ang;
+    float s, c;
+    sincosf(ang, &s, &c);     // its Payne-Hanek path for |ang| > 105615 is the kernel's 32-byte stack frame
+    float K[9] = {0, -z, y, z, 0, -x, -y, x, 0};
+    float KK[9];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int bb = 0; bb < 3; ++bb) KK[a * 3 + bb] = K[a * 3] * K[bb] + K[a * 3 + 1] * K[3 + bb] + K[a * 3 + 2] * K[6 + bb];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = ((i % 4 == 0) ? 1.f : 0.f) + s * K[i] + (1.f - c) * KK[i];
+    if (j >= 1)
+#pragma unroll
+      for (int i = 0; i < 9; ++i) feat[(j - 1) * 9 + i] = R[i] - ((i % 4 == 0) ? 1.f : 0.f);
+  }
+  const int par = act ? parents[j] : -1;
+  float Jx = act ? Jg[j * 3] : 0.f, Jy = act ? Jg[j * 3 + 1] : 0.f, Jz = act ? Jg[j * 3 + 2] : 0.f;
+  float tx = Jx, ty = Jy, tz = Jz;
+  {
+    int p = par < 0 ? 0 : par;
+    float px = __shfl_sync(0xffffffffu, Jx, p), py = __shfl_sync(0xffffffffu, Jy, p), pz = __shfl_sync(0xffffffffu, Jz, p);
+    if (act && j >= 1) { tx -= px; ty -= py; tz -= pz; }
+  }
+  float T[12] = {R[0], R[1], R[2], tx, R[3], R[4], R[5], ty, R[6], R[7], R[8], tz};
+  int depth = 0;
+  {
+    int p = par;
+    for (int it = 0; it < NJ_MAX; ++it) {
+      int pp = __shfl_sync(0xffffffffu, par, p < 0 ? 0 : p);
+      if (p >= 0) { ++depth; p = pp; }
+    }
+  }
+  int maxd = depth;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) maxd = max(maxd, __shfl_xor_sync(0xffffffffu, act ? maxd : 0, o));
+  for (int d = 1; d <= maxd; ++d) {
+    float Pm[12];
+#pragma unroll
+    for (int i = 0; i < 12; ++i) Pm[i] = __shfl_sync(0xffffffffu, T[i], par < 0 ? 0 : par);
+    if (act && depth == d) {
+      float Nw[12];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) Nw[r * 4 + c] = Pm[r * 4] * T[c] + Pm[r * 4 + 1] * T[4 + c] + Pm[r * 4 + 2] * T[8 + c];
+        Nw[r * 4 + 3] = Pm[r * 4] * T[3] + Pm[r * 4 + 1] * T[7] + Pm[r * 4 + 2] * T[11] + Pm[r * 4 + 3];
+      }
+#pragma unroll
+      for (int i = 0; i < 12; ++i) T[i] = Nw[i];
+    }
+  }
+  if (act) {
+    float* a = A_out + ((size_t)b * NJ + j) * 12;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      a[r * 4 + 0] = T[r * 4]; a[r * 4 + 1] = T[r * 4 + 1]; a[r * 4 + 2] = T[r * 4 + 2];
+      a[r * 4 + 3] = T[r * 4 + 3] - (T[r * 4] * Jx + T[r * 4 + 1] * Jy + T[r * 4 + 2] * Jz);
+    }
+  }
+}
+
+constexpr int kSkinRows = 8;
+
+struct PostRot {
+  float m[9];
+  int on;
+};
+
+// thread per vertex, kSkinRows pose rows per CTA: the [rows][207] x [207][3V] pose blend contraction (each posedirs
+// element read once for all rows, each row's terms summed in k_lbs_skin's order), then the blended transform
+__global__ void __launch_bounds__(128)
+k_pose_skin(const float* __restrict__ v_template, const float* __restrict__ posedirs, const float* __restrict__ feat,
+            const float* __restrict__ A, const float* __restrict__ lbs_weights, int V, int NJ, int NF, int B, PostRot pr,
+            float* __restrict__ verts) {
+  __shared__ float sA[kSkinRows][NJ_MAX * 12];
+  __shared__ float sF[kSkinRows][NJ_MAX * 9];
+  const int b0 = blockIdx.y * kSkinRows;
+  const int nr = min(kSkinRows, B - b0);
+  for (int i = threadIdx.x; i < kSkinRows * NJ * 12; i += blockDim.x) {
+    const int r = i / (NJ * 12), k = i - r * NJ * 12;
+    sA[r][k] = r < nr ? A[(size_t)(b0 + r) * NJ * 12 + k] : 0.f;
+  }
+  for (int i = threadIdx.x; i < kSkinRows * NF; i += blockDim.x) {
+    const int r = i / NF, k = i - r * NF;
+    sF[r][k] = r < nr ? feat[(size_t)(b0 + r) * NF + k] : 0.f;
+  }
+  __syncthreads();
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  float p[kSkinRows][3];
+  const float t0 = v_template[v * 3], t1 = v_template[v * 3 + 1], t2 = v_template[v * 3 + 2];
+#pragma unroll
+  for (int r = 0; r < kSkinRows; ++r) { p[r][0] = t0; p[r][1] = t1; p[r][2] = t2; }
+  const size_t ld = (size_t)V * 3;
+  for (int k = 0; k < NF; ++k) {
+    const float* pd = posedirs + (size_t)k * ld + (size_t)v * 3;
+    const float d0 = pd[0], d1 = pd[1], d2 = pd[2];
+#pragma unroll
+    for (int r = 0; r < kSkinRows; ++r) {
+      const float f = sF[r][k];
+      p[r][0] = fmaf(f, d0, p[r][0]); p[r][1] = fmaf(f, d1, p[r][1]); p[r][2] = fmaf(f, d2, p[r][2]);
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < kSkinRows; ++r) {
+    if (r >= nr) break;
+    float T[12];
+#pragma unroll
+    for (int i = 0; i < 12; ++i) T[i] = 0.f;
+    for (int j = 0; j < NJ; ++j) {
+      const float w = lbs_weights[(size_t)v * NJ + j];
+#pragma unroll
+      for (int i = 0; i < 12; ++i) T[i] = fmaf(w, sA[r][j * 12 + i], T[i]);
+    }
+    const float p0 = p[r][0], p1 = p[r][1], p2 = p[r][2];
+    float o0 = T[0] * p0 + T[1] * p1 + T[2] * p2 + T[3];
+    float o1 = T[4] * p0 + T[5] * p1 + T[6] * p2 + T[7];
+    float o2 = T[8] * p0 + T[9] * p1 + T[10] * p2 + T[11];
+    if (pr.on) {     // row vector times matrix: o @ m
+      const float q0 = o0 * pr.m[0] + o1 * pr.m[3] + o2 * pr.m[6];
+      const float q1 = o0 * pr.m[1] + o1 * pr.m[4] + o2 * pr.m[7];
+      const float q2 = o0 * pr.m[2] + o1 * pr.m[5] + o2 * pr.m[8];
+      o0 = q0; o1 = q1; o2 = q2;
+    }
+    float* out = verts + ((size_t)(b0 + r) * V + v) * 3;
+    out[0] = o0; out[1] = o1; out[2] = o2;
+  }
+}
+
+// ---------------------------------------------------------------- batched textured render
+// images are [A][B] (angle-major); mesh b uses the cameras of its group b / G: cams[(b / G) * A + a]
+__global__ void k_project_batch(const float* __restrict__ verts, int V, int B, int G, int A,
+                                const LookAtCam* __restrict__ cams, float4* __restrict__ proj) {
+  const int img = blockIdx.y, a = img / B, b = img - a * B;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= V) return;
+  const LookAtCam c = cams[(b / G) * A + a];
+  project_look_at(i, verts + (size_t)b * V * 3, c, proj + (size_t)img * V);
+}
+
+__global__ void k_raster_batch(const float4* __restrict__ proj, int V, const int* __restrict__ faces, int F, int is,
+                               unsigned long long* __restrict__ zbuf) {
+  const int img = blockIdx.y;
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  raster_face(f, proj + (size_t)img * V, faces, is, 0.1f, 100.f, zbuf + (size_t)img * is * is);
+}
+
+__global__ void k_resolve_batch(const unsigned long long* __restrict__ zbuf, const int* __restrict__ faces,
+                                const float* __restrict__ verts, const float4* __restrict__ proj,
+                                const float* __restrict__ tex, int R, int V, int B, int G, int A,
+                                const LookAtCam* __restrict__ cams, int n, int ss, float* __restrict__ rgb) {
+  const int img = blockIdx.y, a = img / B, b = img - a * B;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n * n) return;
+  const LookAtCam c = cams[(b / G) * A + a];
+  resolve_textured(p, zbuf + (size_t)img * c.is * c.is, faces, verts + (size_t)b * V * 3, proj + (size_t)img * V, tex,
+                   R, c, n, ss, rgb + (size_t)img * n * n * 3);
+}
+
+// ---------------------------------------------------------------- scores and selection
+__device__ __forceinline__ unsigned ordered_bits(float f) {
+  unsigned u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// key = (ordered value bits, ~index): the larger key is the larger value, on ties the smaller index
+__device__ __forceinline__ unsigned long long sel_key(float v, int i) {
+  return ((unsigned long long)ordered_bits(v) << 32) | (unsigned)(0xffffffffu - (unsigned)i);
+}
+
+__device__ __forceinline__ double block_sum_d(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  double s = 0.0;
+  for (int k = 0; k < nw; ++k) s += red[k];
+  return s;
+}
+
+// one CTA per row: F.cosine_similarity(X[i], y) = sum_j (x_j / max(|x|, eps)) (y_j / max(|y|, eps)), sums in fp64
+__global__ void k_rows_cos(const float* __restrict__ X, const float* __restrict__ y, int D, float eps,
+                           float* __restrict__ cos_out) {
+  __shared__ double red[32];
+  const int i = blockIdx.x;
+  double xx = 0.0, xy = 0.0, yy = 0.0;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) {
+    const double a = X[(size_t)i * D + j], b = y[j];
+    xx += a * a; xy += a * b; yy += b * b;
+  }
+  xx = block_sum_d(xx, red);
+  xy = block_sum_d(xy, red);
+  yy = block_sum_d(yy, red);
+  if (threadIdx.x == 0) cos_out[i] = (float)(xy / (fmax(sqrt(xx), (double)eps) * fmax(sqrt(yy), (double)eps)));
+}
+
+__device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v, unsigned long long* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
+    v = u > v ? u : v;
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  __syncthreads();
+  if (lane == 0) red[w] = v;
+  __syncthreads();
+  unsigned long long m = 0;
+  for (int k = 0; k < nw; ++k) m = red[k] > m ? red[k] : m;
+  return m;
+}
+
+// one CTA: k rounds, each the largest key below the previous round's (keys are distinct)
+__global__ void __launch_bounds__(1024) k_topk(const float* __restrict__ v, int N, int k, int* __restrict__ idx_out) {
+  __shared__ unsigned long long red[32];
+  unsigned long long prev = ~0ull;
+  for (int r = 0; r < k; ++r) {
+    unsigned long long best = 0;
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+      const unsigned long long key = sel_key(v[i], i);
+      if (key < prev && key > best) best = key;
+    }
+    best = block_max_u64(best, red);
+    if (threadIdx.x == 0) idx_out[r] = (int)(0xffffffffu - (unsigned)(best & 0xffffffffu));
+    prev = best;
+  }
+}
+
+// one CTA: pairwise mean absolute differences (fp32 differences, fp64 sum, rounded to fp32 like the reference's
+// tensor mean), then the greedy pass of suppress_duplicated_poses in list order
+__global__ void __launch_bounds__(256)
+k_pose_suppress(const float* __restrict__ poses, int P, int Dp, float threshold, int* __restrict__ keep_out,
+                int* __restrict__ count_out) {
+  __shared__ float sp[kSupMax * kSupMaxD];
+  __shared__ float dist[kSupMax][kSupMax];
+  __shared__ int kept[kSupMax];
+  for (int i = threadIdx.x; i < P * Dp; i += blockDim.x) sp[i] = poses[i];
+  __syncthreads();
+  for (int t = threadIdx.x; t < P * P; t += blockDim.x) {
+    const int i = t / P, j = t - i * P;
+    if (j >= i) continue;
+    double s = 0.0;
+    for (int d = 0; d < Dp; ++d) s += (double)fabsf(sp[i * Dp + d] - sp[j * Dp + d]);
+    dist[i][j] = (float)(s / Dp);
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  int n = 0;
+  for (int i = 0; i < P; ++i) {
+    float md = 10.f;
+    for (int q = 0; q < n; ++q) md = fminf(dist[i][kept[q]], md);
+    if (n == 0 || md > threshold) kept[n++] = i;
+  }
+  for (int q = 0; q < n; ++q) keep_out[q] = kept[q];
+  *count_out = n;
+}
+
+// one CTA per pose b: feature = mean_a emb[a][b] (fp64 sum / A, rounded), score = cosine(feature, text) (eps 1e-8),
+// then the group's first argmax through a 64-bit atomicMax
+__global__ void k_pose_score(const float* __restrict__ emb, int A, int B, int Dm, const float* __restrict__ text, int G,
+                             float* __restrict__ score_out, unsigned long long* __restrict__ keys) {
+  __shared__ double red[32];
+  const int b = blockIdx.x;
+  double xx = 0.0, xy = 0.0, yy = 0.0;
+  for (int j = threadIdx.x; j < Dm; j += blockDim.x) {
+    double s = 0.0;
+    for (int a = 0; a < A; ++a) s += emb[((size_t)a * B + b) * Dm + j];
+    const double f = (float)(s / A), t = text[j];
+    xx += f * f; xy += f * t; yy += t * t;
+  }
+  xx = block_sum_d(xx, red);
+  xy = block_sum_d(xy, red);
+  yy = block_sum_d(yy, red);
+  if (threadIdx.x == 0) {
+    const float sc = (float)(xy / (fmax(sqrt(xx), 1e-8) * fmax(sqrt(yy), 1e-8)));
+    score_out[b] = sc;
+    atomicMax(keys + b / G, sel_key(sc, b % G));
+  }
+}
+
+__global__ void k_group_best(const unsigned long long* __restrict__ keys, int n, int* __restrict__ best) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) best[g] = (int)(0xffffffffu - (unsigned)(keys[g] & 0xffffffffu));
+}
+
+}  // namespace
+
+extern "C" {
+
+int avc_vposer_decode_workspace_bytes(int32_t latent, int32_t hidden, int32_t n_joints, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (latent < 1 || latent > kVpMaxL || hidden < 1 || hidden > kVpMaxH || n_joints < 1 || n_joints * 6 > kVpMaxOut)
+    return AVC_E_SIZE;
+  Carver c(nullptr);
+  c.take<float>((size_t)latent * hidden);
+  c.take<float>((size_t)hidden * hidden);
+  c.take<float>((size_t)hidden * n_joints * 6);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_vposer_decode(const float* z, int32_t B, int32_t latent, const float* W1, const float* b1, int32_t hidden,
+                      const float* W2, const float* b2, const float* W3, const float* b3, int32_t n_joints,
+                      float* pose_out, float* rotmat_out, void* workspace, size_t workspace_bytes,
+                      avc_stream_t stream) {
+  if (!z || !W1 || !b1 || !W2 || !b2 || !W3 || !b3 || !pose_out || !workspace) return AVC_E_NULL;
+  size_t need = 0;
+  AVC_TRY(avc_vposer_decode_workspace_bytes(latent, hidden, n_joints, &need));
+  if (B < 1 || workspace_bytes < need) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int L = latent, H = hidden, O = n_joints * 6;
+  Carver c(workspace);
+  float* w1t = c.take<float>((size_t)L * H);
+  float* w2t = c.take<float>((size_t)H * H);
+  float* w3t = c.take<float>((size_t)H * O);
+  k_transpose<<<(H * L + 255) / 256, 256, 0, st>>>(W1, H, L, L, 0, w1t);
+  k_transpose<<<(H * H + 255) / 256, 256, 0, st>>>(W2, H, H, H, 0, w2t);
+  k_transpose<<<(O * H + 255) / 256, 256, 0, st>>>(W3, O, H, H, 0, w3t);
+  VpWeights w{w1t, b1, w2t, b2, w3t, b3};
+  k_vposer_decode<<<(B + kVpRows - 1) / kVpRows, 256, 0, st>>>(z, B, L, H, n_joints, w, pose_out, rotmat_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+static bool nvp_sizes_ok(int dim, int hidden, int n_blocks) {
+  return dim >= 1 && dim <= kNvpMaxD && hidden >= 1 && hidden <= kNvpMaxH && n_blocks >= 1 && n_blocks <= kNvpMaxBlocks;
+}
+
+int avc_realnvp_pack_floats(int32_t dim, int32_t hidden, int32_t n_blocks, size_t* floats) {
+  if (!floats) return AVC_E_NULL;
+  if (!nvp_sizes_ok(dim, hidden, n_blocks)) return AVC_E_SIZE;
+  *floats = nvp_pack(dim, hidden).stride * 2 * n_blocks;
+  return 0;
+}
+
+int avc_realnvp_pack(const float* params, int32_t dim, int32_t feat_dim, int32_t hidden, int32_t n_blocks, float* pack,
+                     avc_stream_t stream) {
+  if (!params || !pack) return AVC_E_NULL;
+  if (!nvp_sizes_ok(dim, hidden, n_blocks) || feat_dim < 0) return AVC_E_SIZE;
+  const int H = hidden;
+  const dim3 grid((max(H, dim) * H + 255) / 256, 2 * n_blocks);
+  k_realnvp_pack<<<grid, 256, 0, (cudaStream_t)stream>>>(params, dim, feat_dim, H, pack);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_realnvp_decode_workspace_bytes(int32_t dim, int32_t hidden, int32_t n_blocks, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (!nvp_sizes_ok(dim, hidden, n_blocks)) return AVC_E_SIZE;
+  Carver c(nullptr);
+  c.take<float>((size_t)hidden * 2 * n_blocks);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_realnvp_decode(const float* z, int32_t B, int32_t dim, const float* feature, int32_t feat_dim,
+                       const float* params, const float* pack, const float* mask, int32_t n_blocks, int32_t hidden,
+                       float* x_out, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!z || !feature || !params || !pack || !mask || !x_out || !workspace) return AVC_E_NULL;
+  size_t need = 0;
+  AVC_TRY(avc_realnvp_decode_workspace_bytes(dim, hidden, n_blocks, &need));
+  if (B < 1 || feat_dim < 0 || workspace_bytes < need) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = dim, E = feat_dim, H = hidden;
+  float* fold = static_cast<float*>(workspace);
+  k_realnvp_fold<<<2 * n_blocks, 256, 0, st>>>(params, feature, D, E, H, fold);
+  k_realnvp_decode<<<(B + kNvpRows - 1) / kNvpRows, 256, 0, st>>>(z, B, D, E, H, n_blocks, params, pack, fold, mask,
+                                                                  x_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_smpl_pose_batch_workspace_bytes(int32_t B, int32_t n_joints, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (B < 1 || n_joints < 2 || n_joints > NJ_MAX) return AVC_E_SIZE;
+  Carver c(nullptr);
+  c.take<float>((size_t)n_joints * 3);
+  c.take<float>((size_t)B * n_joints * 12);
+  c.take<float>((size_t)B * (n_joints - 1) * 9);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_smpl_pose_batch(const float* v_template, const float* J_regressor, const int32_t* parents,
+                        const float* posedirs, const float* lbs_weights, int32_t V, int32_t n_joints,
+                        const float* body_pose, int32_t pose_dim, int32_t B, const float* global_orient,
+                        const float* post_rot, float* verts_out, void* workspace, size_t workspace_bytes,
+                        avc_stream_t stream) {
+  if (!v_template || !J_regressor || !parents || !posedirs || !lbs_weights || !body_pose || !global_orient ||
+      !verts_out || !workspace)
+    return AVC_E_NULL;
+  size_t need = 0;
+  AVC_TRY(avc_smpl_pose_batch_workspace_bytes(B, n_joints, &need));
+  if (V < 1 || pose_dim < 0 || pose_dim > (n_joints - 1) * 3 || workspace_bytes < need) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver c(workspace);
+  float* J = c.take<float>((size_t)n_joints * 3);
+  float* A = c.take<float>((size_t)B * n_joints * 12);
+  float* feat = c.take<float>((size_t)B * (n_joints - 1) * 9);
+  Orient go{{global_orient[0], global_orient[1], global_orient[2]}};
+  PostRot pr{};
+  pr.on = post_rot != nullptr;
+  if (post_rot)
+    for (int i = 0; i < 9; ++i) pr.m[i] = post_rot[i];
+  k_pose_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, J);
+  k_pose_chain<<<(B + 3) / 4, 128, 0, st>>>(body_pose, pose_dim, B, go, J, parents, n_joints, A, feat);
+  dim3 grid((V + 127) / 128, (B + kSkinRows - 1) / kSkinRows);
+  k_pose_skin<<<grid, 128, 0, st>>>(v_template, posedirs, feat, A, lbs_weights, V, n_joints, (n_joints - 1) * 9, B, pr,
+                                    verts_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_raster_textured_batch_workspace_bytes(int32_t V, int32_t n_images, int32_t n_cams, int32_t image_size,
+                                              int32_t supersample, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (V < 1 || n_images < 1 || n_images > 65535 || n_cams < 1 || image_size < 1 || image_size > 4096 ||
+      supersample < 1 || supersample > 4)
+    return AVC_E_SIZE;
+  const size_t is = (size_t)image_size * supersample;
+  Carver c(nullptr);
+  c.take<LookAtCam>(n_cams);
+  c.take<float4>((size_t)n_images * V);
+  c.take<unsigned long long>((size_t)n_images * is * is);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_raster_textured_batch(const float* verts, int32_t B, int32_t group, const int32_t* faces,
+                              const float* textures, int32_t V, int32_t F, int32_t R, const float* eyes, int32_t A,
+                              const float* at, const float* up, int32_t image_size, int32_t supersample,
+                              float* rgb_out, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!verts || !faces || !textures || !eyes || !at || !up || !rgb_out || !workspace) return AVC_E_NULL;
+  if (B < 1 || group < 1 || A < 1 || A > kMaxCams || F < 1 || R < 2 || R > 64) return AVC_E_SIZE;
+  const int ngroups = (B + group - 1) / group;
+  size_t need = 0;
+  AVC_TRY(avc_raster_textured_batch_workspace_bytes(V, A * B, ngroups * A, image_size, supersample, &need));
+  if (workspace_bytes < need) return AVC_E_SIZE;
+  const int is = image_size * supersample;
+  std::vector<LookAtCam> hc((size_t)ngroups * A);
+  for (int i = 0; i < ngroups * A; ++i)
+    if (!make_look_at_cam(eyes + 3 * i, at, up, is, &hc[i])) return AVC_E_BADCFG;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver c(workspace);
+  LookAtCam* cams = c.take<LookAtCam>((size_t)ngroups * A);
+  float4* proj = c.take<float4>((size_t)A * B * V);
+  unsigned long long* zbuf = c.take<unsigned long long>((size_t)A * B * is * is);
+  // from pageable memory: the call returns once hc is staged, so it may be freed on return
+  AVC_CUDA_TRY(cudaMemcpyAsync(cams, hc.data(), sizeof(LookAtCam) * hc.size(), cudaMemcpyHostToDevice, st));
+  AVC_CUDA_TRY(cudaMemsetAsync(zbuf, 0xff, sizeof(unsigned long long) * (size_t)A * B * is * is, st));
+  const unsigned nimg = (unsigned)(A * B);
+  k_project_batch<<<dim3((V + 255) / 256, nimg), 256, 0, st>>>(verts, V, B, group, A, cams, proj);
+  k_raster_batch<<<dim3((F + 127) / 128, nimg), 128, 0, st>>>(proj, V, faces, F, is, zbuf);
+  k_resolve_batch<<<dim3((image_size * image_size + 255) / 256, nimg), 256, 0, st>>>(
+      zbuf, faces, verts, proj, textures, R, V, B, group, A, cams, image_size, supersample, rgb_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_cosine_topk(const float* rows, int32_t N, int32_t D, const float* vec, float eps, int32_t k, float* cos_out,
+                    int32_t* idx_out, avc_stream_t stream) {
+  if (!rows || !vec || !cos_out || !idx_out) return AVC_E_NULL;
+  if (N < 1 || D < 1 || k < 1 || k > N) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  k_rows_cos<<<N, 128, 0, st>>>(rows, vec, D, eps, cos_out);
+  k_topk<<<1, 1024, 0, st>>>(cos_out, N, k, idx_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_pose_suppress(const float* poses, int32_t P, int32_t dim, float threshold, int32_t* keep_out,
+                      int32_t* count_out, avc_stream_t stream) {
+  if (!poses || !keep_out || !count_out) return AVC_E_NULL;
+  if (P < 1 || P > kSupMax || dim < 1 || dim > kSupMaxD) return AVC_E_SIZE;
+  k_pose_suppress<<<1, 256, 0, (cudaStream_t)stream>>>(poses, P, dim, threshold, keep_out, count_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_pose_score(const float* emb, int32_t A, int32_t B, int32_t dim, const float* text, int32_t group,
+                   float* score_out, int32_t* best_out, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!emb || !text || !score_out || !best_out || !workspace) return AVC_E_NULL;
+  if (A < 1 || B < 1 || dim < 1 || group < 1) return AVC_E_SIZE;
+  const int ng = (B + group - 1) / group;
+  if (workspace_bytes < sizeof(unsigned long long) * ng) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* keys = static_cast<unsigned long long*>(workspace);
+  AVC_CUDA_TRY(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * ng, st));
+  k_pose_score<<<B, 128, 0, st>>>(emb, A, B, dim, text, group, score_out, keys);
+  k_group_best<<<(ng + 255) / 256, 256, 0, st>>>(keys, ng, best_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+}  // extern "C"

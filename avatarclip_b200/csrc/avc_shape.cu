@@ -143,95 +143,6 @@ __global__ void k_load_textures(const float* __restrict__ image, int IH, int IW,
                     r1[x1 * 3 + ch] * (wx1 * wy1));
 }
 
-// ---------------------------------------------------------------- textured look_at rasteriser
-struct LookAtCam {
-  float eye[3];
-  float rx[3], ry[3], rz[3];   // rows of look_at()'s rotation
-  float inv_width;             // 1 / tan(viewing_angle = 30 deg)
-  int is;                      // supersampled image size
-};
-
-// look_at() + perspective(), the vertices as given (ShapeGen does not re-orient them): [V] x_ndc, y_ndc, z_cam
-__global__ void k_project_look_at(const float* __restrict__ v, int V, LookAtCam c, float4* __restrict__ proj) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= V) return;
-  float dx = v[i * 3] - c.eye[0], dy = v[i * 3 + 1] - c.eye[1], dz = v[i * 3 + 2] - c.eye[2];
-  float cx = c.rx[0] * dx + c.rx[1] * dy + c.rx[2] * dz;
-  float cy = c.ry[0] * dx + c.ry[1] * dy + c.ry[2] * dz;
-  float cz = c.rz[0] * dx + c.rz[1] * dy + c.rz[2] * dz;
-  proj[i] = make_float4(cx / cz * c.inv_width, cy / cz * c.inv_width, cz, 0.f);
-}
-
-// resolve: per supersample the winning face's colour -- trilinear sample of its R^3 cube at the perspective-corrected
-// barycentrics, times the face's light -- then the ss x ss average.  No flip (ShapeGen keeps neural_renderer's image).
-__global__ void k_resolve_textured(const unsigned long long* __restrict__ zbuf, const int* __restrict__ faces,
-                                   const float* __restrict__ verts, const float4* __restrict__ proj,
-                                   const float* __restrict__ tex, int R, LookAtCam c, int n, int ss,
-                                   float* __restrict__ rgb) {
-  int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n * n) return;
-  int y = p / n, x = p - y * n;
-  const int is = c.is;
-  float acc[3] = {0.f, 0.f, 0.f};
-  for (int sy = 0; sy < ss; ++sy)
-    for (int sx = 0; sx < ss; ++sx) {
-      const int row = y * ss + sy, xi = x * ss + sx;
-      unsigned long long zb = zbuf[(size_t)row * is + xi];
-      if (zb == ~0ull) continue;
-      const int f = (int)(zb & 0xffffffffu);
-      const float zp = __uint_as_float((unsigned)(zb >> 32));
-      const int i0 = faces[f * 3], i1 = faces[f * 3 + 1], i2 = faces[f * 3 + 2];
-      // lighting in the world frame: n = normalize((v0 - v1) x (v2 - v1)), the copy facing the eye is the one drawn
-      const float* v0 = verts + 3 * i0;
-      const float* v1 = verts + 3 * i1;
-      const float* v2 = verts + 3 * i2;
-      float a[3] = {v0[0] - v1[0], v0[1] - v1[1], v0[2] - v1[2]}, b[3] = {v2[0] - v1[0], v2[1] - v1[1], v2[2] - v1[2]};
-      float nx = a[1] * b[2] - a[2] * b[1], ny = a[2] * b[0] - a[0] * b[2], nz = a[0] * b[1] - a[1] * b[0];
-      float nl = fmaxf(sqrtf(nx * nx + ny * ny + nz * nz), 1e-5f);
-      float s = (nx * (c.eye[0] - v1[0]) + ny * (c.eye[1] - v1[1]) + nz * (c.eye[2] - v1[2])) >= 0.f ? 1.f : -1.f;
-      const float light = 0.5f + 0.5f * fmaxf(s * ny / nl, 0.f);
-      // screen barycentrics at the supersample centre, then w_k (R - 1) z_pixel / z_k
-      const float4 pa = proj[i0], pb = proj[i1], pc = proj[i2];
-      const int yi = is - 1 - row;
-      const float xp = (2.f * xi + 1.f - is) / is, yp = (2.f * yi + 1.f - is) / is;
-      const float det = (pb.y - pc.y) * (pa.x - pc.x) + (pc.x - pb.x) * (pa.y - pc.y);
-      const float w0 = ((pb.y - pc.y) * (xp - pc.x) + (pc.x - pb.x) * (yp - pc.y)) / det;
-      const float w1 = ((pc.y - pa.y) * (xp - pc.x) + (pa.x - pc.x) * (yp - pc.y)) / det;
-      const float w2 = 1.f - w0 - w1;
-      const float wz[3] = {w0 * zp / pa.z, w1 * zp / pb.z, w2 * zp / pc.z};
-      float ti[3];
-      int tb[3];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        ti[k] = fminf(fmaxf(wz[k] * (R - 1), 0.f), (float)(R - 1) - 1e-5f);
-        tb[k] = (int)ti[k];
-        ti[k] -= (float)tb[k];
-      }
-      const float* cube = tex + (size_t)f * R * R * R * 3;
-      float col[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-      for (int corner = 0; corner < 8; ++corner) {
-        float w = 1.f;
-        int idx = 0;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const int hi = (corner >> k) & 1;
-          w *= hi ? ti[k] : 1.f - ti[k];
-          idx = idx * R + min(tb[k] + hi, R - 1);
-        }
-        col[0] += w * cube[idx * 3];
-        col[1] += w * cube[idx * 3 + 1];
-        col[2] += w * cube[idx * 3 + 2];
-      }
-      acc[0] += col[0] * light;
-      acc[1] += col[1] * light;
-      acc[2] += col[2] * light;
-    }
-  const float inv = 1.f / (float)(ss * ss);
-  float* o = rgb + (size_t)p * 3;
-  o[0] = acc[0] * inv; o[1] = acc[1] * inv; o[2] = acc[2] * inv;
-}
-
 // ---------------------------------------------------------------- CLIP preprocessing
 // images [B][n][n][3] -> out [B][3][S][S]: nearest (src = floor(dst * n / S)), then (x - mean) / std, each step in
 // double rounded to float like the reference's in-place ops on a float32 tensor with float64 operands.
@@ -287,16 +198,6 @@ __global__ void k_codebook_cos(const float* __restrict__ C, const float* __restr
 
 __global__ void k_codebook_best(const unsigned long long* __restrict__ key, int* __restrict__ best) {
   *best = (int)(0xffffffffu - (unsigned)(*key & 0xffffffffu));
-}
-
-inline void cross3(const float* a, const float* b, float* o) {
-  o[0] = a[1] * b[2] - a[2] * b[1]; o[1] = a[2] * b[0] - a[0] * b[2]; o[2] = a[0] * b[1] - a[1] * b[0];
-}
-inline bool normalize3(float* a) {
-  float n = sqrtf(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]);
-  if (!(n > 0.f)) return false;
-  a[0] /= n; a[1] /= n; a[2] /= n;
-  return true;
 }
 
 }  // namespace
@@ -367,17 +268,9 @@ int avc_raster_textured(const float* verts, const int32_t* faces, const float* t
   size_t need = 0;
   AVC_TRY(avc_raster_textured_workspace_bytes(V, image_size, supersample, &need));
   if (workspace_bytes < need || F < 1 || R < 2 || R > 64) return AVC_E_SIZE;
-  LookAtCam cam;
-  // look_at(): z = normalize(at - eye), x = normalize(cross(up, z)), y = normalize(cross(z, x))
-  for (int i = 0; i < 3; ++i) { cam.eye[i] = eye[i]; cam.rz[i] = at[i] - eye[i]; }
-  if (!normalize3(cam.rz)) return AVC_E_BADCFG;
-  cross3(up, cam.rz, cam.rx);
-  if (!normalize3(cam.rx)) return AVC_E_BADCFG;
-  cross3(cam.rz, cam.rx, cam.ry);
-  normalize3(cam.ry);
-  cam.inv_width = 1.0f / tanf(30.0f * 3.14159265358979323846f / 180.0f);
   const int is = image_size * supersample;
-  cam.is = is;
+  LookAtCam cam;
+  if (!make_look_at_cam(eye, at, up, is, &cam)) return AVC_E_BADCFG;
   cudaStream_t st = (cudaStream_t)stream;
   Carver c(workspace);
   float4* proj = c.take<float4>(V);

@@ -625,6 +625,70 @@ int avc_codebook_argmax(const float* codebook, const float* image_emb, const flo
                         avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * AvatarAnimate's pose stage: candidate body poses from a text prompt (AvatarAnimate/models/pose_generation.py,
+ * VPoserCodebook and VPoserRealNVP).  All fp32.
+ *
+ * avc_vposer_decode is VPoser 2.x decode: decoder_net = Linear(latent, hidden) W1 [hidden][latent], LeakyReLU(0.01),
+ * Linear W2 [hidden][hidden], LeakyReLU, Linear W3 [6 n_joints][hidden] (nn.Linear layouts), then per joint
+ * ContinousRotReprDecoder (the 6 values as a [3][2] matrix, Gram-Schmidt of its columns with F.normalize's 1e-12 clamp,
+ * b3 = b1 x b2) and matrot2aa (torchgeometry's rotation_matrix_to_quaternion, eps 1e-6, and quaternion_to_angle_axis).
+ * pose_out [B][n_joints][3]; rotmat_out [B][n_joints][3][3] or NULL.  latent <= 64, hidden <= 512, n_joints <= 32.
+ * Workspace: avc_vposer_decode_workspace_bytes.
+ * avc_realnvp_decode is VPoserRealNVP.decode (:233-240) of z [B][dim] conditioned on one feature [feat_dim] shared by
+ * every row.  params packs the 2 n_blocks coupling nets, block-major, s before t, each as W1 [hidden][dim + feat_dim],
+ * b1 [hidden], W2 [hidden][hidden], b2 [hidden], W3 [dim][hidden], b3 [dim]; mask [n_blocks][dim].  The s net ends in
+ * tanh.  pack [avc_realnvp_pack_floats] is what avc_realnvp_pack made of params (the weights transposed; once per
+ * checkpoint).  x_out [B][dim].  dim <= 32, hidden <= 256, n_blocks <= 16.  Workspace: avc_realnvp_decode_workspace_bytes
+ * (the folded first-layer biases, 8 hidden n_blocks bytes).
+ * avc_smpl_pose_batch is smplx SMPL with zero betas (v_shaped = v_template) for B poses: joint 0 = global_orient (HOST
+ * [3], shared), joints 1.. = body_pose [B][pose_dim] (pose_dim <= 3 (n_joints - 1), missing joints zero), axis-angle.
+ * Row b of verts_out [B][V][3] is avc_lbs_fwd(v_template, that pose, pose2rot = 1) bit for bit, times post_rot (HOST
+ * [3][3] applied as v @ post_rot, or NULL).  Workspace: avc_smpl_pose_batch_workspace_bytes(B, n_joints).
+ * avc_raster_textured_batch renders B meshes verts [B][V][3] (shared faces and textures) from A <= 16 eyes per group
+ * of `group` consecutive meshes: eyes HOST [ceil(B / group)][A][3], at / up HOST [3].  rgb_out [A][B][n][n][3]
+ * (angle-major); image (a, b) is avc_raster_textured(verts[b], eye = eyes[b / group][a]) bit for bit.  Workspace:
+ * avc_raster_textured_batch_workspace_bytes(V, A B, ceil(B / group) A, n, supersample), about A B (16 V + 8 (n ss)^2).
+ * avc_cosine_topk: cos_out[N] = F.cosine_similarity(rows[N][D], vec[D]) (torch's form: each operand divided by
+ * max(|.|, eps)), sums in fp64; idx_out[k] the k largest, descending, ties to the smaller index.
+ * avc_pose_suppress: suppress_duplicated_poses (:304-317) of poses [P <= 64][dim <= 96] in list order: a pose is kept
+ * when its smallest mean absolute difference to the kept ones (10 when none) exceeds threshold.  keep_out [P] the kept
+ * indices in order, count_out [1] (DEVICE).
+ * avc_pose_score: feature[b] = mean over a of emb [A][B][dim], score_out[b] = F.cosine_similarity(feature[b], text)
+ * (eps 1e-8), best_out[g] = the first argmax of the scores of rows [g group, (g + 1) group).  Workspace: 8 ceil(B /
+ * group) bytes.
+ * ------------------------------------------------------------------------------------------ */
+int avc_vposer_decode_workspace_bytes(int32_t latent, int32_t hidden, int32_t n_joints, size_t* bytes);
+int avc_vposer_decode(const float* z, int32_t B, int32_t latent, const float* W1, const float* b1, int32_t hidden,
+                      const float* W2, const float* b2, const float* W3, const float* b3, int32_t n_joints,
+                      float* pose_out, float* rotmat_out, void* workspace, size_t workspace_bytes,
+                      avc_stream_t stream);
+int avc_realnvp_pack_floats(int32_t dim, int32_t hidden, int32_t n_blocks, size_t* floats);
+int avc_realnvp_pack(const float* params, int32_t dim, int32_t feat_dim, int32_t hidden, int32_t n_blocks, float* pack,
+                     avc_stream_t stream);
+int avc_realnvp_decode_workspace_bytes(int32_t dim, int32_t hidden, int32_t n_blocks, size_t* bytes);
+int avc_realnvp_decode(const float* z, int32_t B, int32_t dim, const float* feature, int32_t feat_dim,
+                       const float* params, const float* pack, const float* mask, int32_t n_blocks, int32_t hidden,
+                       float* x_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_smpl_pose_batch_workspace_bytes(int32_t B, int32_t n_joints, size_t* bytes);
+int avc_smpl_pose_batch(const float* v_template, const float* J_regressor, const int32_t* parents,
+                        const float* posedirs, const float* lbs_weights, int32_t V, int32_t n_joints,
+                        const float* body_pose, int32_t pose_dim, int32_t B, const float* global_orient,
+                        const float* post_rot, float* verts_out, void* workspace, size_t workspace_bytes,
+                        avc_stream_t stream);
+int avc_raster_textured_batch_workspace_bytes(int32_t V, int32_t n_images, int32_t n_cams, int32_t image_size,
+                                              int32_t supersample, size_t* bytes);
+int avc_raster_textured_batch(const float* verts, int32_t B, int32_t group, const int32_t* faces,
+                              const float* textures, int32_t V, int32_t F, int32_t R, const float* eyes, int32_t A,
+                              const float* at, const float* up, int32_t image_size, int32_t supersample,
+                              float* rgb_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_cosine_topk(const float* rows, int32_t N, int32_t D, const float* vec, float eps, int32_t k, float* cos_out,
+                    int32_t* idx_out, avc_stream_t stream);
+int avc_pose_suppress(const float* poses, int32_t P, int32_t dim, float threshold, int32_t* keep_out,
+                      int32_t* count_out, avc_stream_t stream);
+int avc_pose_score(const float* emb, int32_t A, int32_t B, int32_t dim, const float* text, int32_t group,
+                   float* score_out, int32_t* best_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Video frames of a generated avatar (avatarclip_b200/video.py): one vertex-coloured mesh, smooth-shaded, over many
  * frames per launch.  The reference has no renderer for its results (render_novel_image / interpolate_view cannot
  * run, AvatarAnimate's visualize.py draws the grey SMPL body through pyrender); this one is the project's own.
