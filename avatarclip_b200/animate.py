@@ -8,8 +8,8 @@ Two generators of models/pose_generation.py run here:
   * ``VPoserRealNVP`` (:176-285): per candidate ``num_batch`` x ``num_sample`` prior draws through the text-conditioned
     RealNVP and VPoser, each pose posed on SMPL, rendered with the UV texture from 5 cameras and scored by CLIP; the
     best of the batches is kept, then the candidates are sorted by a fresh score.
-The gradient-based ``PoseOptimizer`` / ``VPoserOptimizer`` and the motion stage (``general.mode = motion``) are not
-available and are refused before any file is read.
+The gradient-based ``PoseOptimizer`` / ``VPoserOptimizer`` are not available and are refused before any file is read;
+the motion stage (``general.mode = motion``) is ``python -m avatarclip_b200.motion``.
 
 Everything on the hot path runs in libavc_b200.so: ``avc_vposer_decode``, ``avc_realnvp_decode``,
 ``avc_smpl_pose_batch``, ``avc_raster_textured_batch``, ``avc_clip_prep_nearest``, the CLIP towers,
@@ -254,10 +254,16 @@ def pose_score(emb: torch.Tensor, text: torch.Tensor, group: int):
 
 
 # ---------------------------------------------------------------- loaders
-def load_vposer(path) -> dict:
+VPOSER_ENCODER_KEYS = tuple([f"encoder_net.{i}.{k}" for i in (1, 4) for k in ("weight", "bias", "running_mean",
+                                                                               "running_var")] +
+                            [f"encoder_net.{i}.{k}" for i in (2, 6, 7, "8.mu") for k in ("weight", "bias")])
+
+
+def load_vposer(path, encoder: bool = False) -> dict:
     """human_body_prior's ``load_model(path, remove_words_in_model_weights='vp_model.')``, decoder only: ``path`` is the
     VPoser directory (the last of ``snapshots/*.ckpt``, a Lightning checkpoint whose ``state_dict`` holds
-    ``vp_model.decoder_net.{0,3,5}.{weight,bias}``), one such checkpoint file, or a state dict."""
+    ``vp_model.decoder_net.{0,3,5}.{weight,bias}``), one such checkpoint file, or a state dict.  With ``encoder`` the
+    result also holds ``VPOSER_ENCODER_KEYS`` (what ``VPoser.encode(x).mean`` reads)."""
     if isinstance(path, Mapping):
         sd = path
     else:
@@ -271,6 +277,8 @@ def load_vposer(path) -> dict:
         sd = ck.get("state_dict", ck)
     sd = {k.replace("vp_model.", ""): v for k, v in sd.items()}
     keys = [f"decoder_net.{i}.{k}" for i in (0, 3, 5) for k in ("weight", "bias")]
+    if encoder:
+        keys += VPOSER_ENCODER_KEYS
     missing = [k for k in keys if k not in sd]
     if missing:
         raise ValueError(f"VPoser weights: missing {missing}")
@@ -441,8 +449,13 @@ def refusal(conf) -> Optional[str]:
     """Why ``conf`` cannot run here, or None."""
     mode = conf.get_string("general.mode", "pose")
     if mode != "pose":
-        return (f"general.mode = {mode}: the motion stage (MotionInterpolation / MotionOptimizer) is not available; "
-                "only general.mode = pose runs")
+        return (f"general.mode = {mode}: this command runs the pose stage only; the motion stage runs as python -m "
+                "avatarclip_b200.motion")
+    return pose_generator_refusal(conf)
+
+
+def pose_generator_refusal(conf) -> Optional[str]:
+    """Why the conf's pose_generator cannot run here, or None."""
     typ = conf.get("pose_generator", {}).get("type", None)
     if typ in OUT_OF_SCOPE:
         return f"pose_generator.type = {typ} is not available: it {OUT_OF_SCOPE[typ]}"
@@ -518,6 +531,11 @@ def parse_args(argv=None):
     why = refusal(conf)
     if why:
         parser.error(why)
+    return a, conf, resolve_pose_paths(parser, a, conf)
+
+
+def resolve_pose_paths(parser, a, conf) -> dict:
+    """The pose_generator kwargs with its weight path resolved (and ``a.vposer``), every file checked to exist."""
     pg = dict(conf["pose_generator"])
     # an explicit flag, else the conf's path, else the reference's default
     pick = lambda flag, key: getattr(a, flag) or pg.get(key) or DEFAULT_PATHS[flag]
@@ -536,7 +554,7 @@ def parse_args(argv=None):
             parser.error(f"{flag}: no such file: {path}")
     if not os.path.exists(a.vposer):
         parser.error(f"--vposer: no such directory or file: {a.vposer}")
-    return a, conf, pg
+    return pg
 
 
 def write_candidates(out_dir: str, poses: torch.Tensor, images: np.ndarray) -> List[str]:

@@ -153,6 +153,50 @@ k_vposer_decode(const float* __restrict__ z, int B, int L, int H, int NJ, VpWeig
   }
 }
 
+// ---------------------------------------------------------------- VPoser encode (.mean)
+// eval-mode BatchNorm1d of ROWS rows in place: (x - running_mean) * (1 / sqrt(running_var + eps)) * weight + bias;
+// bn = (weight, bias, running_mean, running_var), each [n]
+__device__ __forceinline__ void batchnorm_rows(float* x, int rows, int n, const float* __restrict__ bn) {
+  for (int i = threadIdx.x; i < rows * n; i += blockDim.x) {
+    const int c = i % n;
+    const float invstd = 1.f / sqrtf(bn[3 * n + c] + 1e-5f);
+    x[i] = (x[i] - bn[2 * n + c]) * invstd * bn[c] + bn[n + c];
+  }
+}
+
+struct VpEncWeights {
+  const float *bn1, *w1t, *b1, *bn2, *w2t, *b2, *w3t, *b3, *wmt, *bm;
+};
+
+__global__ void __launch_bounds__(256)
+k_vposer_encode(const float* __restrict__ x, int B, int NI, int H, int L, VpEncWeights w, float* __restrict__ mu_out) {
+  __shared__ float sx[kVpRows * kVpMaxOut];
+  __shared__ float sh1[kVpRows * kVpMaxH];
+  __shared__ float sh2[kVpRows * kVpMaxH];
+  const int row0 = blockIdx.x * kVpRows;
+  for (int i = threadIdx.x; i < kVpRows * NI; i += blockDim.x) {
+    const int r = i / NI, row = row0 + r;
+    sx[i] = row < B ? x[(size_t)row * NI + (i - r * NI)] : 0.f;
+  }
+  __syncthreads();
+  batchnorm_rows(sx, kVpRows, NI, w.bn1);                          // encoder_net.1
+  __syncthreads();
+  dense_rows<kVpRows>(sx, NI, NI, w.w1t, H, w.b1, 1, sh1, H);      // encoder_net.2 + LeakyReLU
+  __syncthreads();
+  batchnorm_rows(sh1, kVpRows, H, w.bn2);                          // encoder_net.4 (Dropout: eval)
+  __syncthreads();
+  dense_rows<kVpRows>(sh1, H, H, w.w2t, H, w.b2, 0, sh2, H);       // encoder_net.6
+  __syncthreads();
+  dense_rows<kVpRows>(sh2, H, H, w.w3t, H, w.b3, 0, sh1, H);       // encoder_net.7
+  __syncthreads();
+  dense_rows<kVpRows>(sh1, H, H, w.wmt, L, w.bm, 0, sh2, L);       // encoder_net.8.mu
+  __syncthreads();
+  for (int i = threadIdx.x; i < kVpRows * L; i += blockDim.x) {
+    const int r = i / L, row = row0 + r;
+    if (row < B) mu_out[(size_t)row * L + (i - r * L)] = sh2[i];
+  }
+}
+
 // ---------------------------------------------------------------- RealNVP decode
 // the transposed weights, packed once per checkpoint, per coupling net (block i, net n: 0 = s, 1 = t): w1t [D][H]
 // (the x columns of the first linear), w2t [H][H], w3t [H][D]
@@ -617,6 +661,45 @@ int avc_vposer_decode(const float* z, int32_t B, int32_t latent, const float* W1
   k_transpose<<<(O * H + 255) / 256, 256, 0, st>>>(W3, O, H, H, 0, w3t);
   VpWeights w{w1t, b1, w2t, b2, w3t, b3};
   k_vposer_decode<<<(B + kVpRows - 1) / kVpRows, 256, 0, st>>>(z, B, L, H, n_joints, w, pose_out, rotmat_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_vposer_encode_workspace_bytes(int32_t n_in, int32_t hidden, int32_t latent, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (n_in < 1 || n_in > kVpMaxOut || hidden < 1 || hidden > kVpMaxH || latent < 1 || latent > kVpMaxL)
+    return AVC_E_SIZE;
+  Carver c(nullptr);
+  c.take<float>((size_t)n_in * hidden);
+  c.take<float>((size_t)hidden * hidden);
+  c.take<float>((size_t)hidden * hidden);
+  c.take<float>((size_t)hidden * latent);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_vposer_encode(const float* x, int32_t B, int32_t n_in, const float* bn1, const float* W1, const float* b1,
+                      int32_t hidden, const float* bn2, const float* W2, const float* b2, const float* W3,
+                      const float* b3, const float* Wmu, const float* bmu, int32_t latent, float* mu_out,
+                      void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!x || !bn1 || !W1 || !b1 || !bn2 || !W2 || !b2 || !W3 || !b3 || !Wmu || !bmu || !mu_out || !workspace)
+    return AVC_E_NULL;
+  size_t need = 0;
+  AVC_TRY(avc_vposer_encode_workspace_bytes(n_in, hidden, latent, &need));
+  if (B < 1 || workspace_bytes < need) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int NI = n_in, H = hidden, L = latent;
+  Carver c(workspace);
+  float* w1t = c.take<float>((size_t)NI * H);
+  float* w2t = c.take<float>((size_t)H * H);
+  float* w3t = c.take<float>((size_t)H * H);
+  float* wmt = c.take<float>((size_t)H * L);
+  k_transpose<<<(H * NI + 255) / 256, 256, 0, st>>>(W1, H, NI, NI, 0, w1t);
+  k_transpose<<<(H * H + 255) / 256, 256, 0, st>>>(W2, H, H, H, 0, w2t);
+  k_transpose<<<(H * H + 255) / 256, 256, 0, st>>>(W3, H, H, H, 0, w3t);
+  k_transpose<<<(L * H + 255) / 256, 256, 0, st>>>(Wmu, L, H, H, 0, wmt);
+  VpEncWeights w{bn1, w1t, b1, bn2, w2t, b2, w3t, b3, wmt, bmu};
+  k_vposer_encode<<<(B + kVpRows - 1) / kVpRows, 256, 0, st>>>(x, B, NI, H, L, w, mu_out);
   AVC_LAUNCH_TRY();
   return 0;
 }

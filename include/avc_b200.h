@@ -688,6 +688,66 @@ int avc_pose_suppress(const float* poses, int32_t P, int32_t dim, float threshol
 int avc_pose_score(const float* emb, int32_t A, int32_t B, int32_t dim, const float* text, int32_t group,
                    float* score_out, int32_t* best_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
 
+/* avc_vposer_encode is VPoser 2.x encode(x).mean in eval mode: encoder_net = BatchNorm1d(n_in) (running statistics,
+ * eps 1e-5), Linear(n_in, hidden) W1, LeakyReLU(0.01), BatchNorm1d(hidden), Dropout (identity), Linear W2 [hidden]
+ * [hidden], Linear W3 [hidden][hidden], then the NormalDistDecoder's mu head Wmu [latent][hidden].  Each batch norm
+ * is given as bn[4][n] = (weight, bias, running_mean, running_var).  x [B][n_in] -> mu_out [B][latent].  n_in <= 192,
+ * hidden <= 512, latent <= 64.  Workspace: avc_vposer_encode_workspace_bytes. */
+int avc_vposer_encode_workspace_bytes(int32_t n_in, int32_t hidden, int32_t latent, size_t* bytes);
+int avc_vposer_encode(const float* x, int32_t B, int32_t n_in, const float* bn1, const float* W1, const float* b1,
+                      int32_t hidden, const float* bn2, const float* W2, const float* b2, const float* W3,
+                      const float* b3, const float* Wmu, const float* bmu, int32_t latent, float* mu_out,
+                      void* workspace, size_t workspace_bytes, avc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * AvatarAnimate's MotionOptimizer without its CLIP term (AvatarAnimate/models/motion_generation.py:249-358).  fp32.
+ *
+ * The decoder is MotionXTransformerDecoder in eval mode: nn.TransformerDecoder of n_layers post-LN layers (d_model =
+ * latent, n_heads heads, feed-forward ff with exact GELU, LayerNorm eps 1e-5, no final norm) over the query rows
+ * pe [n_frames][latent] (the positional table), with the latent as the single memory token, then the final linear to
+ * n_out = 6 x joints.  params is, per layer, in this order: self_attn.in_proj_weight [3 latent][latent], in_proj_bias,
+ * self_attn.out_proj weight [latent][latent], bias, the v rows of multihead_attn.in_proj_weight [latent][latent]
+ * (rows 2 latent .. 3 latent) and of its in_proj_bias, multihead_attn.out_proj weight, bias, linear1 weight
+ * [ff][latent], bias, linear2 weight [latent][ff], bias, norm1 weight, bias, norm2 weight, bias, norm3 weight, bias;
+ * after the layers final.weight [n_out][latent], final.bias.  avc_motion_param_count gives the total.
+ * The motion is rotation_6d_to_matrix -> matrix_to_quaternion -> quaternion_to_axis_angle of joints 1..21 of each row
+ * (MotionOptimizer.decode's columns 3:66): motion_out [n_frames][63].
+ * AVC_E_BADCFG unless 32 <= latent <= 512, latent / n_heads <= 64 (and divides), 1 <= n_layers <= 16, ff <= 4096,
+ * 2 <= n_frames <= 64 and n_out a multiple of 6 of at least 132.
+ *
+ * avc_motion_decode: MotionOptimizer.decode(latent [latent]).
+ * avc_motion_optimize: n_iter iterations of get_motion's loop (clip_coef = 0) from latent_init [latent] (DEVICE):
+ *   loss = sum_k recon_coef[k] min_t mean_(joint, 6) (g6(motion[t]) - g6(poses[k]))^2
+ *          - delta_coef mse(motion[:-1], motion[1:])   (the last term only when delta_coef > 0)
+ *   with g6 = matrix_to_rotation_6d(axis_angle_to_matrix(.)), then the gradient with respect to the latent and the
+ *   Adam step of avc_adam_step_dev (lr, beta1, beta2, eps).  torch.min's gradient goes to the first frame of equal
+ *   minima.  poses [n_poses][63] (DEVICE, n_poses <= 16), recon_coef HOST [n_poses].  Writes latent_out [latent]
+ *   (after the last step), motion_out [n_frames][63] (decoded at the last iteration, before its step, as the
+ *   reference returns it), when loss_out is not NULL loss_out [n_iter] (each iteration's loss), and when grad_out
+ *   is not NULL grad_out [latent] (the last iteration's gradient with respect to the latent).  One
+ *   iteration's launches are captured once as a CUDA graph on a private stream and replayed n_iter times, ordered
+ *   after earlier and before later work on `stream`; the call does not wait for the device.
+ * Workspace: avc_motion_workspace_bytes (both calls).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct avc_motion_dims {
+  int32_t latent;
+  int32_t n_layers;
+  int32_t n_heads;
+  int32_t ff;
+  int32_t n_frames;
+  int32_t n_out;
+} avc_motion_dims;
+
+int avc_motion_param_count(const avc_motion_dims* dims, int64_t* count);
+int avc_motion_workspace_bytes(const avc_motion_dims* dims, size_t* bytes);
+int avc_motion_decode(const avc_motion_dims* dims, const float* params, const float* pe, const float* latent,
+                      float* motion_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_motion_optimize(const avc_motion_dims* dims, const float* params, const float* pe, const float* poses,
+                        int32_t n_poses, const float* recon_coef, float delta_coef, float lr, float beta1, float beta2,
+                        float eps, int32_t n_iter, const float* latent_init, float* latent_out, float* motion_out,
+                        float* loss_out, float* grad_out, void* workspace, size_t workspace_bytes,
+                        avc_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Video frames of a generated avatar (avatarclip_b200/video.py): one vertex-coloured mesh, smooth-shaded, over many
  * frames per launch.  The reference has no renderer for its results (render_novel_image / interpolate_view cannot
