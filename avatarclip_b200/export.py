@@ -28,11 +28,19 @@ The file:
     is the identity in glTF's y-up frame, and reads no translation.  So at every frame p_drive = R_x(pi/2) (p_glb - J_0)
     + J_0.
 
+  * Texture (with ``--conf``): ``bake.bake_texture`` fills a per-face atlas from the NeuS run's colour field.  The
+    primitive then has one vertex per face corner (the atlas splits every face off its neighbours; positions and skin
+    weights are the shared vertex's), NORMAL (``bake.vertex_normals`` of the bind pose, smooth across the split),
+    TEXCOORD_0 (origin at the top left) and no COLOR_0.  The material's baseColorTexture is a PNG in a buffer view,
+    its bytes the sRGB ``to8b`` bytes the PLY holds; the sampler is LINEAR without mipmaps (a face's footprint never
+    leaves its own texels) and CLAMP_TO_EDGE.
+
 Left out: FBX itself (it needs Autodesk's proprietary SDK; Blender converts the .glb to FBX), the reference's all-zero
 blend shape, non-zero beta (Avatar2FBX fixes beta = 0) and ``cleanup_mesh`` (Avatar2FBX does not run it).
 
     python -m avatarclip_b200.export --mesh exp/.../meshes/00029500.ply --smpl smpl.npz \\
-        --stand_pose stand_pose.npy [--motion action.npy --fps 30] --out avatar.glb
+        --stand_pose stand_pose.npy [--motion action.npy --fps 30] --out avatar.glb \\
+        [--conf confs/examples/hulk.conf [--case smpl] [--checkpoint ckpt_030000.pth] [--texture_size 2048]]
 """
 from __future__ import annotations
 
@@ -46,7 +54,7 @@ import sys
 import numpy as np
 import torch
 
-from . import _lib, drive
+from . import _lib, bake, drive
 from .drive import Mesh, _cuda, _f32
 
 # The SMPL joints under Mixamo's bone names, in SMPL's joint order
@@ -118,11 +126,14 @@ def find_nearest_ind(new_vertices, template_object) -> torch.Tensor:
 
 
 # ---------------------------------------------------------------- export_fbx.py:44-109
-def rig_avatar(mesh_ply: str, smpl, stand_pose_npy: str, resolution: int = DEFAULT_RESOLUTION, device="cuda") -> dict:
+def rig_avatar(mesh_ply: str, smpl, stand_pose_npy: str, resolution: int = DEFAULT_RESOLUTION, device="cuda",
+               ply_frame: bool = False) -> dict:
     """export_fbx.py:50-109 for one PLY: the content of the reference's ``smpl_object``, in metres, as host arrays:
     ``vertices`` [N,3] T-pose (SMPL's zero pose), ``triangles`` [T,3], ``joints`` [24,3] (J_regressor . v_template),
     ``nearest`` [N] (template vertex whose weights each vertex takes), ``colors`` [N,3] float32 in [0, 1] or None,
-    plus what the skin needs: ``lbs_weights`` [M,24] and ``parents`` [24] of the SMPL tensors, and ``name``."""
+    plus what the skin needs: ``lbs_weights`` [M,24] and ``parents`` [24] of the SMPL tensors, and ``name``.
+    ``ply_frame`` adds ``vertices_ply`` [N,3] float32: the clustered vertices in the PLY (NeuS) frame, before the
+    rotation and the un-posing, where ``bake.bake_texture`` reads the colour field."""
     device = _cuda(device)
     s = drive.smpl_tensors(smpl, device)
     nj = s["J_regressor"].shape[0]
@@ -135,10 +146,13 @@ def rig_avatar(mesh_ply: str, smpl, stand_pose_npy: str, resolution: int = DEFAU
     nearest = _nearest_f32(rot, template["vertices"].reshape(-1, 3))
     A_stand, joints = drive._rel_transforms(s, pose_rot.reshape(1, nj, 9).contiguous(), False, return_joints=True)
     tpose = drive._inv_lbs(rot, nearest, s["lbs_weights"], A_stand[0])
-    return dict(name=os.path.splitext(os.path.basename(mesh_ply))[0], vertices=tpose.cpu().numpy(),
-                triangles=mesh.triangles.cpu().numpy(), joints=joints.cpu().numpy(),
-                nearest=nearest.cpu().numpy().astype(np.int64), colors=mesh.vertex_colors,
-                lbs_weights=s["lbs_weights"].cpu().numpy(), parents=s["parents"].cpu().numpy().astype(np.int64))
+    rig = dict(name=os.path.splitext(os.path.basename(mesh_ply))[0], vertices=tpose.cpu().numpy(),
+               triangles=mesh.triangles.cpu().numpy(), joints=joints.cpu().numpy(),
+               nearest=nearest.cpu().numpy().astype(np.int64), colors=mesh.vertex_colors,
+               lbs_weights=s["lbs_weights"].cpu().numpy(), parents=s["parents"].cpu().numpy().astype(np.int64))
+    if ply_frame:
+        rig["vertices_ply"] = v.cpu().numpy()
+    return rig
 
 
 # ---------------------------------------------------------------- glTF 2.0 binary
@@ -185,7 +199,7 @@ class _Glb:
             view["target"] = target
         self.blob += data + b"\0" * (-len(data) % 4)
         self.views.append(view)
-        n = {"SCALAR": 1, "VEC3": 3, "VEC4": 4, "MAT4": 16}[typ]
+        n = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4, "MAT4": 16}[typ]
         acc = {"bufferView": len(self.views) - 1, "componentType": comp, "count": int(arr.size // n), "type": typ}
         if minmax:
             a = np.asarray(arr, dtype=np.float64).reshape(-1, n)
@@ -193,11 +207,18 @@ class _Glb:
         self.accessors.append(acc)
         return len(self.accessors) - 1
 
+    def add_bytes(self, data: bytes) -> int:
+        """A buffer view of raw bytes (an embedded image): returns its index."""
+        self.views.append({"buffer": 0, "byteOffset": len(self.blob), "byteLength": len(data)})
+        self.blob += data + b"\0" * (-len(data) % 4)
+        return len(self.views) - 1
 
-def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 30) -> str:
+
+def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 30, texture=None) -> str:
     """Write ``rig`` (``rig_avatar``'s dictionary; host arrays or tensors) as a glTF 2.0 binary at ``path``; with
     ``motion_npy`` (rows [F, >= 72] of SMPL axis-angle, as ``drive`` reads them) also one animation of F keys at
-    ``fps``.  Layout in the module docstring.  Returns ``path``."""
+    ``fps``; with ``texture`` = (uv [3T,2], image uint8 [H,W,3] RGB), ``bake.bake_texture``'s result, a textured
+    primitive, which also needs ``rig["normals"]`` [N,3].  Layout in the module docstring.  Returns ``path``."""
     FLOAT, UINT, UBYTE = 5126, 5125, 5121
     pos = _np(rig["vertices"]).astype(np.float32).reshape(-1, 3)
     tri = _np(rig["triangles"]).astype(np.uint32).reshape(-1, 3)
@@ -212,9 +233,23 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
         raise ValueError(f"write_glb: fps must be > 0, got {fps}")
     motion = None if motion_npy is None else drive._motion_axis_angle(motion_npy)
 
+    if texture is not None:
+        uv, image = _np(texture[0]).astype(np.float32).reshape(-1, 2), np.asarray(_np(texture[1]), dtype=np.uint8)
+        if rig.get("normals") is None:
+            raise ValueError("write_glb: a textured primitive needs rig['normals'] (bake.vertex_normals)")
+        if uv.shape[0] != tri.size or image.ndim != 3 or image.shape[2] != 3:
+            raise ValueError(f"write_glb: texture needs uv [{tri.size}, 2] and an RGB image [H, W, 3], got uv "
+                             f"{list(uv.shape)}, image {list(image.shape)}")
+        corner = tri.reshape(-1).astype(np.int64)           # one vertex per face corner: the UV seams split every face
+        normals = _np(rig["normals"]).astype(np.float32).reshape(-1, 3)[corner]
+        pos, weights, tri = pos[corner], weights[corner], np.arange(tri.size, dtype=np.uint32).reshape(-1, 3)
+
     g = _Glb()
     attrs = {"POSITION": g.add(pos, FLOAT, "VEC3", 34962, minmax=True)}
-    if rig.get("colors") is not None:
+    if texture is not None:
+        attrs["NORMAL"] = g.add(normals, FLOAT, "VEC3", 34962)
+        attrs["TEXCOORD_0"] = g.add(uv, FLOAT, "VEC2", 34962)
+    elif rig.get("colors") is not None:
         col = srgb_to_linear(np.clip(_np(rig["colors"]).reshape(-1, 3), 0.0, 1.0)).astype(np.float32)
         attrs["COLOR_0"] = g.add(col, FLOAT, "VEC3", 34962)
     js, ws = _skin_sets(weights)
@@ -248,6 +283,14 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
         "skins": [{"name": "smpl", "joints": [1 + j for j in range(nj)], "skeleton": roots[0],
                    "inverseBindMatrices": ibm_acc}],
     }
+    if texture is not None:
+        png = g.add_bytes(bake.encode_png(image))
+        gltf["materials"] = [{"name": "baked_texture", "pbrMetallicRoughness": {"baseColorTexture": {"index": 0},
+                                                                              "metallicFactor": 0.0,
+                                                                              "roughnessFactor": 1.0}}]
+        gltf["textures"] = [{"sampler": 0, "source": 0}]
+        gltf["samplers"] = [{"magFilter": 9729, "minFilter": 9729, "wrapS": 33071, "wrapT": 33071}]   # LINEAR, CLAMP
+        gltf["images"] = [{"bufferView": png, "mimeType": "image/png"}]
     if motion is not None:
         q = axis_angle_to_quat(motion[:, 3:3 * nj].reshape(motion.shape[0], nj - 1, 3))     # [F, nj-1, 4]
         for k in range(1, q.shape[0]):                                 # short arc between successive keys
@@ -275,14 +318,31 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
 
 
 def export_avatar(mesh_ply: str, out_glb: str, smpl, stand_pose_npy: str, motion_npy: str | None = None,
-                  fps: float = 30, resolution: int = DEFAULT_RESOLUTION, device="cuda") -> str:
-    """``rig_avatar`` + ``write_glb``: the .glb of one PLY, optionally animated by ``motion_npy``.  Returns its path."""
+                  fps: float = 30, resolution: int = DEFAULT_RESOLUTION, device="cuda", conf: str | None = None,
+                  case: str = "smpl", checkpoint: str | None = None, texture_size: int | None = None) -> str:
+    """``rig_avatar`` + ``write_glb``: the .glb of one PLY, optionally animated by ``motion_npy``.  With ``conf`` (the
+    NeuS run's conf) the mesh also gets a texture of ``texture_size`` (default ``bake.DEFAULT_TEXTURE_SIZE``) baked
+    from the run's colour field: the Runner is built as ``--mode validate_mesh`` builds it (its last checkpoint), or
+    from ``checkpoint`` (a path, or a name under the run's checkpoints directory).  Returns the path."""
+    if conf is None and (checkpoint is not None or texture_size is not None):
+        raise ValueError("export_avatar: checkpoint and texture_size need conf (the NeuS run to bake from)")
     if motion_npy is not None:
         drive._motion_axis_angle(motion_npy)           # reject a bad motion before the GPU work
-    rig = rig_avatar(mesh_ply, smpl, stand_pose_npy, resolution, device)
+    rig = rig_avatar(mesh_ply, smpl, stand_pose_npy, resolution, device, ply_frame=conf is not None)
+    texture = None
+    if conf is not None:
+        from .runner import Runner
+        T = bake.DEFAULT_TEXTURE_SIZE if texture_size is None else int(texture_size)
+        bake.atlas_grid(len(rig["triangles"]), T)      # refuse a texture too small for the faces before any render
+        runner = Runner(conf, "validate_mesh", case, is_continue=checkpoint is None, device=device)
+        if checkpoint is not None:
+            runner.load_checkpoint(checkpoint)
+        texture = bake.bake_texture(runner, rig["vertices_ply"], rig["triangles"], T)
+        rig["normals"] = bake.vertex_normals(torch.from_numpy(rig["vertices"]).to(_cuda(device)),
+                                             torch.from_numpy(rig["triangles"])).cpu().numpy()
     out_dir = os.path.dirname(os.path.abspath(out_glb))
     os.makedirs(out_dir, exist_ok=True)
-    return write_glb(rig, out_glb, motion_npy, fps)
+    return write_glb(rig, out_glb, motion_npy, fps, texture=texture)
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -302,13 +362,27 @@ def build_parser() -> argparse.ArgumentParser:
                    help="voxel = largest extent / resolution for the vertex clustering")
     p.add_argument("--out", required=True, help="the .glb to write")
     p.add_argument("--device", default="cuda")
+    t = p.add_argument_group("texture", "bake a base-colour texture from the NeuS run that made the mesh")
+    t.add_argument("--conf", default=None, help="the run's conf (as --mode validate_mesh reads it)")
+    t.add_argument("--case", default=None, help="CASE_NAME of the conf (default smpl)")
+    t.add_argument("--checkpoint", default=None,
+                   help="ckpt_XXXXXX.pth under the run's checkpoints directory, or a path (default: the last one)")
+    t.add_argument("--texture_size", type=int, default=None,
+                   help=f"texels per side of the square texture (default {bake.DEFAULT_TEXTURE_SIZE})")
     return p
 
 
 def main(argv=None) -> int:
     parser = build_parser()
     a = parser.parse_args(argv)
-    for flag, path in (("--mesh", a.mesh), ("--smpl", a.smpl), ("--stand_pose", a.stand_pose), ("--motion", a.motion)):
+    if a.conf is None:
+        for flag, val in (("--case", a.case), ("--checkpoint", a.checkpoint), ("--texture_size", a.texture_size)):
+            if val is not None:
+                parser.error(f"{flag} needs --conf (the NeuS run to bake the texture from)")
+    if a.texture_size is not None and not 1 <= a.texture_size <= bake.MAX_TEXTURE_SIZE:
+        parser.error(f"--texture_size must be in [1, {bake.MAX_TEXTURE_SIZE}]")
+    for flag, path in (("--mesh", a.mesh), ("--smpl", a.smpl), ("--stand_pose", a.stand_pose), ("--motion", a.motion),
+                       ("--conf", a.conf)):
         if path is not None and not os.path.isfile(path):
             parser.error(f"{flag}: no such file: {path}")
     if not a.fps > 0:
@@ -327,7 +401,15 @@ def main(argv=None) -> int:
             drive._motion_axis_angle(a.motion)
         except (ValueError, OSError) as e:
             parser.error(f"--motion: {e}")
-    print(export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device))
+    if a.conf is None:
+        print(export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device))
+        return 0
+    try:
+        out = export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device, conf=a.conf,
+                            case=a.case or "smpl", checkpoint=a.checkpoint, texture_size=a.texture_size)
+    except bake.AtlasTooSmall as e:
+        parser.error(f"--texture_size: {e}")
+    print(out)
     return 0
 
 

@@ -561,18 +561,39 @@ class Runner:
         if vertices.shape[0] == 0:
             write_ply(path, vertices, triangles, np.zeros((0, 3), dtype=np.uint8))
             return path
-        pt = torch.from_numpy(vertices).to(self.device).float()
+        write_ply(path, vertices, triangles, self.surface_colors(torch.from_numpy(vertices).to(self.device).float()))
+        logging.info("End")
+        return path
+
+    def surface_colors(self, points, chunk: Optional[int] = None, perturb: Optional[float] = None) -> np.ndarray:
+        """main.py:858-911: the colour of surface points [N,3] from the best of six axis views -> uint8 [N,3] (``to8b``).
+        Each point is rendered along the ray from the eyes (0, 0, +-2), (0, +-2, 0), (+-2, 0, 0) in that order; a later
+        view replaces the kept colour where its rendered depth is strictly closer to the point's distance.  ``chunk``
+        rays per render call (None: ``train.batch_size``, as the reference); only the colour and depth of a chunk are
+        kept, so memory grows with N, not with N x samples.  ``perturb`` overrides the renderer's jitter (None: the
+        conf's ``perturb``, drawn afresh per call as the reference does; 0: mid-bin samples, so the result is a
+        function of the points alone, whatever the chunk size)."""
+        pt = torch.as_tensor(points).to(self.device).float().reshape(-1, 3)
+        step = self.batch_size if chunk is None else int(chunk)
         bg = torch.ones([1, 3], device=self.device) if self.use_white_bkgd else None
         ckey = "extra_color_fine" if self.extra_color else "color_fine"
+        kw = {} if perturb is None else {"perturb_overwrite": float(perturb)}
         rgb_final = diff_final = None
         for eye in ([0, 0, 2], [0, 0, -2], [0, 2, 0], [0, -2, 0], [2, 0, 0], [-2, 0, 0]):                  # main.py:861-868
             ro = torch.tensor(eye, dtype=torch.float32, device=self.device).reshape(1, 3).repeat(pt.shape[0], 1)
             rd = pt - ro
             dist = torch.norm(rd, dim=-1)
             rd = rd / dist.reshape(-1, 1)
-            o = self._render_batches(ro, rd, bg, keys=(ckey, "weights", "mid_z_vals"))
-            rgb = o[ckey]
-            depth = (o["mid_z_vals"] * o["weights"]).sum(dim=1)
+            rgbs, depths = [], []
+            with torch.no_grad():
+                for ro_b, rd_b in zip(ro.split(step), rd.split(step)):
+                    near, far = self.dataset.near_far_from_sphere(ro_b, rd_b)
+                    o = self.renderer.render(ro_b, rd_b, near, far, cos_anneal_ratio=self.get_cos_anneal_ratio(),
+                                             background_rgb=bg, **kw)
+                    rgbs.append(o[ckey])
+                    depths.append((o["mid_z_vals"] * o["weights"]).sum(dim=1))
+                    del o
+            rgb, depth = torch.cat(rgbs, 0), torch.cat(depths, 0)
             diff = (depth - dist).abs()
             if rgb_final is None:
                 rgb_final, diff_final = rgb.clone(), diff.clone()
@@ -580,9 +601,7 @@ class Runner:
                 ind = diff_final > diff                                                                     # main.py:907-911
                 rgb_final[ind] = rgb[ind]
                 diff_final[ind] = diff[ind]
-        write_ply(path, vertices, triangles, to8b(rgb_final.cpu().numpy()))
-        logging.info("End")
-        return path
+        return to8b(rgb_final.cpu().numpy())
 
     def render_geometry_cast_light(self):
         """main.py:634-739: 512 x 512 close-up of the head, texture x Lambert shading (ambience 0, black background)."""

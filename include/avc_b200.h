@@ -789,6 +789,38 @@ int avc_video_render(const float* verts, int64_t frame_stride, const int32_t* fa
                      uint8_t* rgb_out, int32_t* face_out, void* workspace, size_t workspace_bytes,
                      avc_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Texture baking of a generated avatar (avatarclip_b200/bake.py): a closed-form per-face atlas of a T x T texture.
+ *
+ * avc_bake_atlas_grid: faces 2k and 2k + 1 share square cell k; the cells lie row-major on an m x m grid,
+ * m = ceil(sqrt(ceil(F / 2))), each c = floor(T / m) texels wide.  Writes m and c; AVC_E_BADCFG when c < 8 (the
+ * smallest T that fits is 8 m), AVC_E_SIZE unless 1 <= F <= 2^30 and 1 <= T <= 16384.
+ *
+ * avc_bake_texel_points: texel (x, y) (row y from the top, texel index y T + x) of cell k = (y / c) m + x / c has
+ * cell-local coordinates (i, j) = (x mod c, y mod c).  Face 2k owns the texels with i >= j, face 2k + 1 those with
+ * i < j.  Face 2k's corners 0, 1, 2 sit at the cell-local points (3, 1), (c - 1, 1), (c - 1, c - 3) (x right, y down, in
+ * texels); face 2k + 1's at their mirror images (1, 3), (1, c - 1), (c - 3, c - 1).  Each UV triangle is inset by one
+ * texel from the cell border and two from the diagonal, so every point inside it has its whole bilinear footprint (the
+ * 2 x 2 texel centres around it) among its own face's texels.
+ *   - owner [T * T] int32: the owning face, or -1 for an unused texel (past the last face, in the columns and rows past
+ *     m c, or a face with a vertex index outside [0, V)).
+ *   - points [T * T][3]: b0 v[f0] + b1 v[f1] + b2 v[f2], the barycentrics of the texel centre in the owner's UV
+ *     triangle with negative weights set to 0 and the rest rescaled to sum 1 (a border texel holds a point of the
+ *     triangle); 0 for unused texels.
+ *   - uv: NULL, or [F][3][2] float32 the corner UVs ((cell origin + corner) / T, v = 0 at the top row, as glTF's
+ *     TEXCOORD_0).
+ *   - AVC_E_BADCFG / AVC_E_SIZE as avc_bake_atlas_grid; V >= 1.
+ *
+ * avc_bake_vertex_normals: normals [V][3], per vertex the sum over its faces, in the CSR order of avc_video_adjacency
+ * (offsets / vf of the same faces), of the un-normalised (v1 - v0) x (v2 - v0), normalised; (0, 1, 0) where the sum
+ * is zero.  No float atomics: bitwise reproducible.  1 <= V, 1 <= F <= 2^29.
+ * ------------------------------------------------------------------------------------------ */
+int avc_bake_atlas_grid(int32_t F, int32_t T, int32_t* m, int32_t* c);
+int avc_bake_texel_points(const float* verts, const int32_t* faces, int32_t V, int32_t F, int32_t T, int32_t* owner,
+                          float* points, float* uv, avc_stream_t stream);
+int avc_bake_vertex_normals(const float* verts, const int32_t* faces, const int32_t* offsets, const int32_t* vf,
+                            int32_t V, int32_t F, float* normals, avc_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
