@@ -12,7 +12,9 @@
 //   pass 1 (emit = false): triangles per cube -> counts[cube]
 //   host: exclusive scan of counts (torch.cumsum: plumbing)
 //   pass 2 (emit = true):  vertices [3 T][3] in index coordinates + a 64-bit key of the grid edge each vertex lies on
-//                          (min point index * 8 + edge direction code) for welding (torch.unique on the keys)
+//                          (min point index * 8 + edge direction code 1..7) for welding (torch.unique on the keys); a
+//                          crossing whose outside corner equals iso is that grid point and takes the point's key
+//                          (point index * 8 + code 0), so the caller welds it once and drops the triangles it collapses
 #include "avc_common.cuh"
 
 using namespace avc;
@@ -65,8 +67,9 @@ __global__ void k_march_tets(const float* __restrict__ u, Grid g, int* __restric
     // crossing points: every (inside, outside) pair of the tetrahedron is a cut edge
     float P[4][3];
     long long K[4];
+    int M[4][3];                                          // twice the cut edge's midpoint, cube-local
     int np = 0;
-    float cin[3] = {0, 0, 0}, cout[3] = {0, 0, 0};
+    int cin[3] = {0, 0, 0}, cout[3] = {0, 0, 0};
     for (int a = 0; a < ni; ++a) { int3 o = corner(in_idx[a]); cin[0] += o.x; cin[1] += o.y; cin[2] += o.z; }
     for (int b = 0; b < no; ++b) { int3 o = corner(out_idx[b]); cout[0] += o.x; cout[1] += o.y; cout[2] += o.z; }
     for (int a = 0; a < ni; ++a)
@@ -77,8 +80,12 @@ __global__ void k_march_tets(const float* __restrict__ u, Grid g, int* __restric
         P[np][0] = cx + pi.x + tt * (po.x - pi.x);
         P[np][1] = cy + pi.y + tt * (po.y - pi.y);
         P[np][2] = cz + pi.z + tt * (po.z - pi.z);
-        // key: the grid edge {p, q}: lower point's linear index and the direction code (bits of |q - p|)
-        int lo = min(ci, co), hi = max(ci, co);       // corner bit patterns: lo is componentwise <= hi inside one tet path
+        M[np][0] = pi.x + po.x; M[np][1] = pi.y + po.y; M[np][2] = pi.z + po.z;
+        // key: the grid edge {p, q}: lower point's linear index and the direction code (bits of |q - p|); an outside
+        // corner equal to iso puts the crossing on that grid point (tt == 1), keyed by the point itself with code 0
+        // so that every edge ending there welds to one vertex
+        const bool on_point = val[co] == g.iso;
+        int lo = on_point ? co : min(ci, co), hi = on_point ? co : max(ci, co);   // lo is componentwise <= hi
         int3 pl = corner(lo);
         long long base = ((long long)(cx + pl.x) * g.ny + (cy + pl.y)) * g.nz + (cz + pl.z);
         K[np] = base * 8 + (hi - lo);
@@ -87,13 +94,18 @@ __global__ void k_march_tets(const float* __restrict__ u, Grid g, int* __restric
     // ni == 1 or 3: np == 3 (one triangle); ni == 2: np == 4, ordered (a0b0, a0b1, a1b0, a1b1) -> quad a0b0,a0b1,a1b1,a1b0
     int tri[2][3] = {{0, 1, 2}, {0, 0, 0}};
     if (ni == 2) { tri[0][0] = 0; tri[0][1] = 1; tri[0][2] = 3; tri[1][0] = 0; tri[1][1] = 3; tri[1][2] = 2; }
-    const float dir[3] = {cin[0] / ni - cout[0] / no, cin[1] / ni - cout[1] / no, cin[2] / ni - cout[2] / no};   // towards inside
+    // orientation: the normal must leave the body, i.e. n . (inside centroid - outside centroid) < 0.  The triangle's
+    // plane separates the inside corners from the outside ones for every crossing strictly inside its edge, so the sign
+    // is the same for all of them: it is taken exactly, in integers, with the crossings at the edge midpoints (ni * no
+    // times the centroid difference), rather than from the fp32 positions, whose sign is arbitrary on triangles that
+    // fp32 index coordinates (2^-15 apart at 512) make degenerate
+    const int dir[3] = {no * cin[0] - ni * cout[0], no * cin[1] - ni * cout[1], no * cin[2] - ni * cout[2]};
     for (int q = 0; q < nt; ++q) {
       int i0 = tri[q][0], i1 = tri[q][1], i2 = tri[q][2];
-      float e1[3] = {P[i1][0] - P[i0][0], P[i1][1] - P[i0][1], P[i1][2] - P[i0][2]};
-      float e2[3] = {P[i2][0] - P[i0][0], P[i2][1] - P[i0][1], P[i2][2] - P[i0][2]};
-      float n[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2], e1[0] * e2[1] - e1[1] * e2[0]};
-      if (n[0] * dir[0] + n[1] * dir[1] + n[2] * dir[2] > 0.f) { int s = i1; i1 = i2; i2 = s; }   // normal must leave the body
+      int e1[3] = {M[i1][0] - M[i0][0], M[i1][1] - M[i0][1], M[i1][2] - M[i0][2]};
+      int e2[3] = {M[i2][0] - M[i0][0], M[i2][1] - M[i0][1], M[i2][2] - M[i0][2]};
+      int n[3] = {e1[1] * e2[2] - e1[2] * e2[1], e1[2] * e2[0] - e1[0] * e2[2], e1[0] * e2[1] - e1[1] * e2[0]};
+      if (n[0] * dir[0] + n[1] * dir[1] + n[2] * dir[2] > 0) { int s = i1; i1 = i2; i2 = s; }
       int idx[3] = {i0, i1, i2};
 #pragma unroll
       for (int k = 0; k < 3; ++k) {

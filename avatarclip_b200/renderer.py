@@ -360,17 +360,23 @@ class NeuSRenderer:
         T = int(incl[-1].item()) if incl.numel() else 0
         if T == 0:
             return np.zeros((0, 3), dtype=np.float64), np.zeros((0, 3), dtype=np.int64)
+        if T > 2 ** 31 - 1:              # avc_march_emit's offsets are int32
+            raise _lib.AvcError(f"extract_geometry: {T} triangles at resolution {N} exceed the int32 triangle offsets")
         offsets = (incl - counts).to(torch.int32)
         verts = torch.empty(T * 3, 3, dtype=torch.float32, device=dev)
         keys = torch.empty(T * 3, dtype=torch.int64, device=dev)
         _lib.check(L.avc_march_emit(_lib.ptr(u), N, N, N, float(threshold), _lib.ptr(offsets), _lib.ptr(verts),
                                     _lib.ptr(keys), _lib.stream_ptr()), "avc_march_emit")
-        uniq, inv = torch.unique(keys, return_inverse=True)                  # weld vertices that sit on the same grid edge
+        uniq, inv = torch.unique(keys, return_inverse=True)        # weld vertices on the same grid edge or grid point
         welded = torch.empty(uniq.numel(), 3, dtype=torch.float32, device=dev)
         welded[inv] = verts
         tri = inv.reshape(T, 3)
-        good = (tri[:, 0] != tri[:, 1]) & (tri[:, 1] != tri[:, 2]) & (tri[:, 0] != tri[:, 2])   # crossings exactly on a grid point
+        good = (tri[:, 0] != tri[:, 1]) & (tri[:, 1] != tri[:, 2]) & (tri[:, 0] != tri[:, 2])   # collapsed on a grid point
         tri = tri[good]
+        used = torch.zeros(uniq.numel(), dtype=torch.bool, device=dev)   # and the vertices only they referenced
+        used[tri.reshape(-1)] = True
+        welded = welded[used]
+        tri = (torch.cumsum(used, 0) - 1)[tri]
         b_min = torch.as_tensor(np.asarray(bound_min, dtype=np.float32), device=dev)
         b_max = torch.as_tensor(np.asarray(bound_max, dtype=np.float32), device=dev)
         vertices = welded / (N - 1.0) * (b_max - b_min)[None, :] + b_min[None, :]          # renderer.py:33-35

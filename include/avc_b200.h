@@ -563,8 +563,10 @@ int avc_uniform_fill(uint32_t seed, int32_t n, float lo, float hi, float* out, a
  * PyMCubes' marching_cubes, third-party, absent).  Marching tetrahedra over the [nx][ny][nz] field u (= -sdf):
  * avc_march_count writes the number of triangles of every grid cube ((nx-1)(ny-1)(nz-1) ints, x-major like the
  * field); the caller turns them into exclusive offsets; avc_march_emit writes 3 vertices per triangle in INDEX
- * coordinates (the caller rescales like renderer.py:33-35) and, per vertex, a 64-bit key of the grid edge it lies
- * on (for welding).  Triangles are oriented with normals towards decreasing u.
+ * coordinates (the caller rescales like renderer.py:33-35) and, per vertex, a 64-bit welding key: vertices with equal
+ * keys are the same point (the grid edge the crossing lies on, or the grid point itself when the outside corner equals
+ * iso; the encoding is internal to NeuSRenderer.extract_geometry, which drops the triangles two equal keys collapse).
+ * Triangles are oriented with normals towards decreasing u.
  * ------------------------------------------------------------------------------------------ */
 /* Profiling aid of the fused value-chain kernel: with AVC_CHAIN_DEBUG=1 in the environment block 0 records cycle
  * counters ([0] MMA warp waiting for its A operand, [1] for weight slabs, [2] MMA warp total, [3] tile-layers,
