@@ -8,8 +8,13 @@ to Autodesk's FBX SDK rigged to SMPL's 24 joints under Mixamo's bone names.  Her
 which Blender, three.js, Unity and Unreal import directly, with no SDK; optionally with the joint rotations of a motion
 ``.npy`` (the file ``avatarclip_b200.drive`` reads) as keyframes.
 
-Everything on the mesh runs in libavc_b200.so: ``avc_mesh_cluster``, ``avc_nearest_vertex_f32``, ``avc_lbs_fwd`` (the
-template), ``avc_lbs_rel_transforms`` and ``avc_inv_lbs``.
+Everything on the mesh runs in libavc_b200.so: ``avc_mesh_cluster``, ``avc_mesh_decimate``, ``avc_nearest_vertex_f32``,
+``avc_lbs_fwd`` (the template), ``avc_lbs_rel_transforms`` and ``avc_inv_lbs``.
+
+With ``--target_faces N``, when the clustering keeps more than N faces, the mesh as read is first decimated by
+quadric-error edge collapse (``decimate_mesh``) to N faces (or N - 1), keeping its topology, and then clustered
+(``reduce_mesh``): vertex clustering alone removes few faces from a finely tessellated mesh, and the texture atlas
+needs a few faces per texel cell.  The rig, the bake and the glTF then see the reduced mesh.
 
 The file:
   * Frame and units: the bind pose is SMPL's zero pose in SMPL's canonical frame, which is glTF's (+Y up, facing +Z);
@@ -39,7 +44,7 @@ Left out: FBX itself (it needs Autodesk's proprietary SDK; Blender converts the 
 blend shape, non-zero beta (Avatar2FBX fixes beta = 0) and ``cleanup_mesh`` (Avatar2FBX does not run it).
 
     python -m avatarclip_b200.export --mesh exp/.../meshes/00029500.ply --smpl smpl.npz \\
-        --stand_pose stand_pose.npy [--motion action.npy --fps 30] --out avatar.glb \\
+        --stand_pose stand_pose.npy [--motion action.npy --fps 30] [--target_faces 20000] --out avatar.glb \\
         [--conf confs/examples/hulk.conf [--case smpl] [--checkpoint ckpt_030000.pth] [--texture_size 2048]]
 """
 from __future__ import annotations
@@ -76,7 +81,10 @@ def _L():
         L.avc_nearest_vertex_f32.argtypes = [vp, i32, vp, i32, vp, vp]
         L.avc_mesh_cluster_workspace_bytes.argtypes = [i32, i32, C.POINTER(sz)]
         L.avc_mesh_cluster.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
-        for n in ("avc_nearest_vertex_f32", "avc_mesh_cluster_workspace_bytes", "avc_mesh_cluster"):
+        L.avc_mesh_decimate_workspace_bytes.argtypes = [i32, i32, C.POINTER(sz)]
+        L.avc_mesh_decimate.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+        for n in ("avc_nearest_vertex_f32", "avc_mesh_cluster_workspace_bytes", "avc_mesh_cluster",
+                  "avc_mesh_decimate_workspace_bytes", "avc_mesh_decimate"):
             getattr(L, n).restype = C.c_int
         _bound = L
     return L
@@ -110,6 +118,55 @@ def simplify_mesh(mesh: Mesh, resolution: int = DEFAULT_RESOLUTION) -> Mesh:
     return Mesh(v_out[:K], f_out[:T], None if c_out is None else c_out[:K].cpu().numpy())
 
 
+def decimate_mesh(mesh: Mesh, target_faces: int) -> Mesh:
+    """Quadric-error edge collapse to ``target_faces`` (semantics in include/avc_b200.h, ``avc_mesh_decimate``): the
+    result has target_faces - 1 or target_faces faces, or more when no edge can collapse without breaking the
+    topology or flipping a face.  Colours, when given, are float [N,3] in any scale and are interpolated along each
+    collapsed edge.  Vertices and faces keep their input order.  The ends of non-manifold edges never move, so a
+    mesh with many of them (a vertex-clustered one) stops early: ``reduce_mesh`` decimates before clustering."""
+    return _decimate(mesh, target_faces)[0]
+
+
+def _decimate(mesh: Mesh, target_faces: int):
+    """``decimate_mesh`` and the number of collapse rounds it ran."""
+    v, f = mesh.vertices, mesh.triangles
+    device = _cuda(v.device)
+    v = _f32(v, device).reshape(-1, 3)
+    f = f.to(device, torch.int32).contiguous().reshape(-1, 3)
+    V, F = v.shape[0], f.shape[0]
+    L = _L()
+    need = C.c_size_t()
+    _lib.check(L.avc_mesh_decimate_workspace_bytes(V, F, C.byref(need)), "avc_mesh_decimate_workspace_bytes")
+    ws = torch.empty(need.value, dtype=torch.uint8, device=device)
+    col = None if mesh.vertex_colors is None else _f32(torch.as_tensor(mesh.vertex_colors), device).reshape(-1, 3)
+    v_out = torch.empty(V, 3, dtype=torch.float32, device=device)
+    c_out = None if col is None else torch.empty(V, 3, dtype=torch.float32, device=device)
+    f_out = torch.empty(F, 3, dtype=torch.int32, device=device)
+    counts = torch.empty(3, dtype=torch.int32, device=device)
+    _lib.check(L.avc_mesh_decimate(_lib.ptr(v), _lib.ptr(col), V, _lib.ptr(f), F, int(target_faces), _lib.ptr(v_out),
+                                   _lib.ptr(c_out), _lib.ptr(f_out), _lib.ptr(counts), _lib.ptr(ws), ws.numel(),
+                                   _lib.stream_ptr()), "avc_mesh_decimate")
+    K, T, rounds = counts.tolist()
+    return Mesh(v_out[:K], f_out[:T], None if c_out is None else c_out[:K].cpu().numpy()), rounds
+
+
+def reduce_mesh(mesh: Mesh, resolution: int = DEFAULT_RESOLUTION, target_faces: int | None = None) -> Mesh:
+    """``simplify_mesh`` at ``resolution``; with ``target_faces``, when the clustering keeps more faces than that, the
+    input is first decimated to ``target_faces`` (``decimate_mesh``) and the result clustered.  Clustering a finely
+    tessellated mesh keeps most of its faces and leaves non-manifold edges (triangles beside their reverses) whose
+    ends the collapse must not move, so the decimation runs on the mesh as read; the clustering after it only merges
+    what falls in one voxel and keeps at most target_faces faces.  Colours are decimated on the 0-255 scale and rounded
+    to the nearest byte before the clustering.  When the clustering alone keeps at most ``target_faces`` faces, the
+    result is the clustering's, byte for byte."""
+    clustered = simplify_mesh(mesh, resolution)
+    if target_faces is None or clustered.triangles.shape[0] <= target_faces:
+        return clustered
+    col = None if mesh.vertex_colors is None else np.asarray(mesh.vertex_colors, dtype=np.float32)
+    dec = decimate_mesh(Mesh(mesh.vertices, mesh.triangles, col), target_faces)
+    c8 = None if dec.vertex_colors is None else np.clip(np.rint(dec.vertex_colors), 0, 255).astype(np.uint8)
+    return simplify_mesh(Mesh(dec.vertices, dec.triangles, c8), resolution)
+
+
 def _nearest_f32(query: torch.Tensor, ref: torch.Tensor) -> torch.Tensor:
     out = torch.empty(query.shape[0], dtype=torch.int32, device=query.device)
     _lib.check(_L().avc_nearest_vertex_f32(_lib.ptr(query), query.shape[0], _lib.ptr(ref), ref.shape[0],
@@ -127,19 +184,20 @@ def find_nearest_ind(new_vertices, template_object) -> torch.Tensor:
 
 # ---------------------------------------------------------------- export_fbx.py:44-109
 def rig_avatar(mesh_ply: str, smpl, stand_pose_npy: str, resolution: int = DEFAULT_RESOLUTION, device="cuda",
-               ply_frame: bool = False) -> dict:
+               ply_frame: bool = False, target_faces: int | None = None) -> dict:
     """export_fbx.py:50-109 for one PLY: the content of the reference's ``smpl_object``, in metres, as host arrays:
     ``vertices`` [N,3] T-pose (SMPL's zero pose), ``triangles`` [T,3], ``joints`` [24,3] (J_regressor . v_template),
     ``nearest`` [N] (template vertex whose weights each vertex takes), ``colors`` [N,3] float32 in [0, 1] or None,
     plus what the skin needs: ``lbs_weights`` [M,24] and ``parents`` [24] of the SMPL tensors, and ``name``.
     ``ply_frame`` adds ``vertices_ply`` [N,3] float32: the clustered vertices in the PLY (NeuS) frame, before the
-    rotation and the un-posing, where ``bake.bake_texture`` reads the colour field."""
+    rotation and the un-posing, where ``bake.bake_texture`` reads the colour field.  ``target_faces`` bounds the
+    faces (``reduce_mesh``)."""
     device = _cuda(device)
     s = drive.smpl_tensors(smpl, device)
     nj = s["J_regressor"].shape[0]
     if nj != len(JOINT_NAMES):
         raise ValueError(f"the skeleton has the {len(JOINT_NAMES)} SMPL joints; the SMPL tensors have {nj}")
-    mesh = simplify_mesh(drive.read_ply(mesh_ply, device), resolution)
+    mesh = reduce_mesh(drive.read_ply(mesh_ply, device), resolution, target_faces)
     v = mesh.vertices
     rot = torch.stack([v[:, 0], -v[:, 2], v[:, 1]], 1).contiguous()          # export_fbx.py:57-62
     template, pose_rot, _ = drive.load_template_smpl(s, stand_pose_npy, device)
@@ -319,16 +377,25 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
 
 def export_avatar(mesh_ply: str, out_glb: str, smpl, stand_pose_npy: str, motion_npy: str | None = None,
                   fps: float = 30, resolution: int = DEFAULT_RESOLUTION, device="cuda", conf: str | None = None,
-                  case: str = "smpl", checkpoint: str | None = None, texture_size: int | None = None) -> str:
+                  case: str = "smpl", checkpoint: str | None = None, texture_size: int | None = None,
+                  target_faces: int | None = None) -> str:
     """``rig_avatar`` + ``write_glb``: the .glb of one PLY, optionally animated by ``motion_npy``.  With ``conf`` (the
     NeuS run's conf) the mesh also gets a texture of ``texture_size`` (default ``bake.DEFAULT_TEXTURE_SIZE``) baked
     from the run's colour field: the Runner is built as ``--mode validate_mesh`` builds it (its last checkpoint), or
-    from ``checkpoint`` (a path, or a name under the run's checkpoints directory).  Returns the path."""
+    from ``checkpoint`` (a path, or a name under the run's checkpoints directory).  ``target_faces`` bounds the
+    faces (``reduce_mesh``); the texture atlas is then sized for the reduced mesh.  When decimation stops above the target, one line on stderr says how many faces it reached.  Returns the
+    path."""
+    if target_faces is not None and target_faces < 1:
+        raise ValueError(f"export_avatar: target_faces must be >= 1, got {target_faces}")
     if conf is None and (checkpoint is not None or texture_size is not None):
         raise ValueError("export_avatar: checkpoint and texture_size need conf (the NeuS run to bake from)")
     if motion_npy is not None:
         drive._motion_axis_angle(motion_npy)           # reject a bad motion before the GPU work
-    rig = rig_avatar(mesh_ply, smpl, stand_pose_npy, resolution, device, ply_frame=conf is not None)
+    rig = rig_avatar(mesh_ply, smpl, stand_pose_npy, resolution, device, ply_frame=conf is not None,
+                     target_faces=target_faces)
+    if target_faces is not None and len(rig["triangles"]) > target_faces:
+        print(f"export: decimation stopped at {len(rig['triangles'])} faces, above --target_faces {target_faces}: "
+              "no further edge collapse keeps the topology and the face orientations", file=sys.stderr)
     texture = None
     if conf is not None:
         from .runner import Runner
@@ -360,6 +427,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fps", type=float, default=30.0, help="keyframes per second of the motion")
     p.add_argument("--resolution", type=int, default=DEFAULT_RESOLUTION,
                    help="voxel = largest extent / resolution for the vertex clustering")
+    p.add_argument("--target_faces", type=int, default=None,
+                   help="at most this many faces: when the clustering keeps more, decimate the mesh by quadric-error "
+                        "edge collapse to this many, then cluster")
     p.add_argument("--out", required=True, help="the .glb to write")
     p.add_argument("--device", default="cuda")
     t = p.add_argument_group("texture", "bake a base-colour texture from the NeuS run that made the mesh")
@@ -379,6 +449,8 @@ def main(argv=None) -> int:
         for flag, val in (("--case", a.case), ("--checkpoint", a.checkpoint), ("--texture_size", a.texture_size)):
             if val is not None:
                 parser.error(f"{flag} needs --conf (the NeuS run to bake the texture from)")
+    if a.target_faces is not None and a.target_faces < 1:
+        parser.error("--target_faces must be >= 1")
     if a.texture_size is not None and not 1 <= a.texture_size <= bake.MAX_TEXTURE_SIZE:
         parser.error(f"--texture_size must be in [1, {bake.MAX_TEXTURE_SIZE}]")
     for flag, path in (("--mesh", a.mesh), ("--smpl", a.smpl), ("--stand_pose", a.stand_pose), ("--motion", a.motion),
@@ -402,11 +474,13 @@ def main(argv=None) -> int:
         except (ValueError, OSError) as e:
             parser.error(f"--motion: {e}")
     if a.conf is None:
-        print(export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device))
+        print(export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device,
+                            target_faces=a.target_faces))
         return 0
     try:
         out = export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device, conf=a.conf,
-                            case=a.case or "smpl", checkpoint=a.checkpoint, texture_size=a.texture_size)
+                            case=a.case or "smpl", checkpoint=a.checkpoint, texture_size=a.texture_size,
+                            target_faces=a.target_faces)
     except bake.AtlasTooSmall as e:
         parser.error(f"--texture_size: {e}")
     print(out)

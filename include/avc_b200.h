@@ -823,6 +823,67 @@ int avc_bake_texel_points(const float* verts, const int32_t* faces, int32_t V, i
 int avc_bake_vertex_normals(const float* verts, const int32_t* faces, const int32_t* offsets, const int32_t* vf,
                             int32_t V, int32_t F, float* normals, avc_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Mesh decimation (avatarclip_b200/export.py, decimate_mesh): quadric-error edge collapse (Garland & Heckbert 1997)
+ * to target_faces, in rounds of independent collapses.  oracle/decimate.py restates it in fp64 numpy.
+ *
+ * Arithmetic: positions are read as float32 and widened; every fp64 operation is rounded on its own (no contraction),
+ * sums left to right as written.  cross(e, f) = (e.y f.z - e.z f.y, e.z f.x - e.x f.z, e.x f.y - e.y f.x);
+ * dot(e, f) = (e.x f.x + e.y f.y) + e.z f.z.  A plane quadric of normal n through o with weight w: len = sqrt(dot(n, n));
+ * if len = 0 it is all +0, else u = n / len (three divisions), p = (u.x, u.y, u.z, -dot(u, o)) and its ten entries
+ * q = (00, 01, 02, 03, 11, 12, 13, 22, 23, 33) are q_ij = w (p_i p_j).
+ *
+ * Valid faces: indices in [0, V) and pairwise distinct; the others are dropped from the output.  Edge (f, k) of face
+ * f = (t0, t1, t2) joins t_k and t_(k+1 mod 3); its id is 3 f + k (f the input index), and an edge's id is the smallest
+ * over the live faces that name it.  n_f = cross(p1 - p0, p2 - p0).
+ *
+ * Quadrics: vertex v starts at +0 and, for each valid face f holding v in ascending f, adds (entrywise) the face
+ * quadric (n_f through p0, w = 0.5 len), then for k = 0, 1, 2 each edge (f, k) through v that lies on exactly one valid
+ * face adds the boundary quadric (normal cross(e, n_f) with e = p(t_(k+1)) - p(t_k), through p(t_k), weight
+ * 10 dot(e, e)).  A collapse of (a, b) leaves Q_a + Q_b on the survivor.
+ *
+ * Rounds.  Each round, over the live faces (valid and not removed), with nf(e) the live faces on edge e:
+ *   1. Flags.  Both ends of an edge with nf > 2 are locked for good; both ends of an edge with nf = 1 are boundary
+ *      vertices this round.  deg(v) = live faces holding v.
+ *   2. Candidates: edges (a, b), a < b, with nf in {1, 2}, neither end locked, deg(a), deg(b) <= 32 (the link
+ *      and flip tests cost O(deg^2) per edge; a vertex above 32 is rare and is retried every round), not interior
+ *      (nf = 2) with both ends boundary vertices, and
+ *      - link condition: the vertices other than a, b that share a live face with both a and b number exactly nf; for
+ *        nf = 2 the third vertices c, d of the two faces on ab differ, and there are not both a face {a, c, d} and a
+ *        face {b, c, d} (the tetrahedron);
+ *      - the point: q = Q_a + Q_b, cofactors c00 = q11 q22 - q12 q12, c01 = q12 q02 - q01 q22, c02 = q01 q12 - q11 q02,
+ *        c11 = q00 q22 - q02 q02, c12 = q01 q02 - q00 q12, c22 = q00 q11 - q01 q01, det = (q00 c00 + q01 c01) + q02 c02,
+ *        tr = (q00 + q11) + q22, r = (-q03, -q13, -q23).  If det > 1e-9 ((tr tr) tr): v* = ((r0 c00 + r1 c01) + r2 c02,
+ *        (r0 c01 + r1 c11) + r2 c12, (r0 c02 + r1 c12) + r2 c22) / det, kept if dot(v* - m, v* - m) <= dot(b - a, b - a)
+ *        with m = (a + b) 0.5.  Otherwise v* is the cheapest of a, b, m (ties in that order).  cost(v) = ((x s0 + y s1)
+ *        + z s2) + s3 with s_i = ((q_i0 x + q_i1 y) + q_i2 z) + q_i3, clamped below at 0 by fmax (a NaN
+ *        cost, which only non-finite coordinates give, becomes 0);
+ *      - no flip: every live face holding a but not b (or b but not a), with that corner moved to float32(v*), keeps
+ *        dot(n_old, n_new) > 0.25 (sqrt(dot(n_old, n_old)) sqrt(dot(n_new, n_new))).
+ *      Key = (float32(cost) bits << 32) | edge id.
+ *   3. Selection: a candidate whose key is <= the smallest candidate key at every vertex of every live face holding a or
+ *      b.  The selected edges' neighbourhoods are disjoint.
+ *   4. Cap: a collapse removes nf faces.  If the selection removes more than live - target_faces, only the longest
+ *      prefix in key order that removes at most that many is applied, and at least the smallest key.
+ *   5. Collapse: b is removed and a survives at float32(v*), its colour the fp64 c_a + t (c_b - c_a), t = dot(v* - a,
+ *      b - a) / dot(b - a, b - a) clamped to [0, 1] (0 when a = b), rounded to float32.  Faces holding a and b are
+ *      removed; b becomes a in the others.
+ * Rounds run while live > target_faces and the last round selected an edge, so the result has target_faces - 1 or
+ * target_faces faces, or more when no edge qualifies (counts[1] > target_faces).
+ *
+ * Outputs sized by the inputs: the vertices not removed by a collapse (unreferenced ones included) in input order,
+ * verts_out [V][3] and colors_out [V][3] (required when colors, float [V][3], is given); the live faces in input order,
+ * remapped, tris_out [F][3].  counts [3] (DEVICE): {vertices, faces, rounds}.  F <= target_faces: the input copied
+ * unchanged, rounds 0.  Bitwise deterministic, whatever the workspace held.  The host reads back two live counts per
+ * round to decide whether to run the next; nothing else returns to the host.
+ * AVC_E_NULL for a missing pointer, AVC_E_SIZE unless 1 <= V, F <= 2^29 or for a short workspace, AVC_E_BADCFG for
+ * target_faces < 1.  Workspace: avc_mesh_decimate_workspace_bytes(V, F) (about 136 V + 92 F bytes).
+ * ------------------------------------------------------------------------------------------ */
+int avc_mesh_decimate_workspace_bytes(int32_t V, int32_t F, size_t* bytes);
+int avc_mesh_decimate(const float* verts, const float* colors, int32_t V, const int32_t* tris, int32_t F,
+                      int32_t target_faces, float* verts_out, float* colors_out, int32_t* tris_out,
+                      int32_t* counts, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
