@@ -8,7 +8,8 @@ Two generators of models/pose_generation.py run here:
   * ``VPoserRealNVP`` (:176-285): per candidate ``num_batch`` x ``num_sample`` prior draws through the text-conditioned
     RealNVP and VPoser, each pose posed on SMPL, rendered with the UV texture from 5 cameras and scored by CLIP; the
     best of the batches is kept, then the candidates are sorted by a fresh score.
-The gradient-based ``PoseOptimizer`` / ``VPoserOptimizer`` are not available and are refused before any file is read;
+The gradient-based generators are refused before any file is read: ``PoseOptimizer`` runs as ``python -m
+avatarclip_b200.pose_optimizer``, and ``VPoserOptimizer`` is not available (the VPoser decoder's backward is not built);
 the motion stage (``general.mode = motion``) is ``python -m avatarclip_b200.motion``.
 
 Everything on the hot path runs in libavc_b200.so: ``avc_vposer_decode``, ``avc_realnvp_decode``,
@@ -41,10 +42,10 @@ SCORE_ORIENT = (math.pi / 2, 0.0, 0.0)  # get_pose_feature :71-72
 IMAGE_ORIENT = (math.pi, 0.0, 0.0)      # visualize.py:87-88
 IMAGE_SIZE, IMAGE_FOCAL, IMAGE_DEPTH, IMAGE_GREY = 512, 5000.0, 25.0, 0.4    # visualize.py:20-38
 IN_SCOPE = ("VPoserCodebook", "VPoserRealNVP")
-OUT_OF_SCOPE = {"PoseOptimizer": "optimises SMPL theta through the rasteriser's gradient, which this project's "
-                                 "textured rasteriser does not have",
-                "VPoserOptimizer": "optimises the VPoser latent through the rasteriser's gradient, which this "
-                                   "project's textured rasteriser does not have"}
+OUT_OF_SCOPE = {"PoseOptimizer": "optimises SMPL theta through the rasteriser's gradient, so it runs as its own "
+                                 "command: python -m avatarclip_b200.pose_optimizer",
+                "VPoserOptimizer": "optimises the VPoser latent through the rasteriser's gradient and the VPoser "
+                                   "decoder's, and the decoder's backward is not built"}
 DEFAULT_PATHS = {"vposer": "data/vposer", "codebook": "data/codebook.pth",      # BasePoseGenerator / the
                  "realnvp": "data/pose_realnvp.pth"}                           # generators' constructor defaults
 _RENDER_BYTES = 1 << 30                 # device bytes per chunk of renders (z-buffers, images, CLIP inputs)
@@ -305,7 +306,8 @@ class Assets:
         self.smpl = drive.smpl_tensors(smpl, self.device)
         self.faces = torch.as_tensor(np.asarray(smpl["faces"], dtype=np.int32)).to(self.device)
         self.clip = clip
-        self.vposer = {k: v.to(self.device) for k, v in load_vposer(vposer).items()}
+        # None: a generator that needs no VPoser (PoseOptimizer)
+        self.vposer = None if vposer is None else {k: v.to(self.device) for k, v in load_vposer(vposer).items()}
         tex = uv_obj if isinstance(uv_obj, torch.Tensor) else shapegen.load_obj_textures(uv_obj, 8, self.device)
         if tex.shape[0] != self.faces.shape[0]:
             raise ValueError(f"the UV texture has {tex.shape[0]} faces, the SMPL mesh {self.faces.shape[0]}")

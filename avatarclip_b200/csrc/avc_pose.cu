@@ -626,7 +626,617 @@ __global__ void k_group_best(const unsigned long long* __restrict__ keys, int n,
   if (g < n) best[g] = (int)(0xffffffffu - (unsigned)(keys[g] & 0xffffffffu));
 }
 
+// ================================================================ backward of the pose optimiser's chain
+// N values summed over the CTA in a fixed order: warp xor trees, then the warps in index order by thread i < N;
+// the totals land in red[i * 32] (red holds N * 32 floats)
+template <int N>
+__device__ __forceinline__ void block_sum_n(float (&v)[N], float* red) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int i = 0; i < N; ++i) v[i] = warp_sum(v[i]);
+  if (lane == 0)
+#pragma unroll
+    for (int i = 0; i < N; ++i) red[i * 32 + w] = v[i];
+  __syncthreads();
+  if (threadIdx.x < N) {
+    float s = 0.f;
+    for (int k = 0; k < nw; ++k) s += red[threadIdx.x * 32 + k];
+    red[threadIdx.x * 32] = s;
+  }
+  __syncthreads();
+}
+
+// ---------------------------------------------------------------- SMPL posing backward
+// thread per vertex, kSkinRows rows per CTA: k_pose_skin's p (pose-blended template) and blended transform T again,
+// then g_o = post_rot g_v (o @ post_rot is the output), and g_p = T_3x3^T g_o
+__global__ void __launch_bounds__(128)
+k_pose_skin_bwd(const float* __restrict__ v_template, const float* __restrict__ posedirs, const float* __restrict__ feat,
+                const float* __restrict__ A, const float* __restrict__ lbs_weights, int V, int NJ, int NF, int B,
+                PostRot pr, const float* __restrict__ g_verts, float* __restrict__ p_out, float* __restrict__ go_out,
+                float* __restrict__ gp_out) {
+  __shared__ float sA[kSkinRows][NJ_MAX * 12];
+  __shared__ float sF[kSkinRows][NJ_MAX * 9];
+  const int b0 = blockIdx.y * kSkinRows;
+  const int nr = min(kSkinRows, B - b0);
+  for (int i = threadIdx.x; i < kSkinRows * NJ * 12; i += blockDim.x) {
+    const int r = i / (NJ * 12), k = i - r * NJ * 12;
+    sA[r][k] = r < nr ? A[(size_t)(b0 + r) * NJ * 12 + k] : 0.f;
+  }
+  for (int i = threadIdx.x; i < kSkinRows * NF; i += blockDim.x) {
+    const int r = i / NF, k = i - r * NF;
+    sF[r][k] = r < nr ? feat[(size_t)(b0 + r) * NF + k] : 0.f;
+  }
+  __syncthreads();
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  float p[kSkinRows][3];
+  const float t0 = v_template[v * 3], t1 = v_template[v * 3 + 1], t2 = v_template[v * 3 + 2];
+#pragma unroll
+  for (int r = 0; r < kSkinRows; ++r) { p[r][0] = t0; p[r][1] = t1; p[r][2] = t2; }
+  const size_t ld = (size_t)V * 3;
+  for (int k = 0; k < NF; ++k) {
+    const float* pd = posedirs + (size_t)k * ld + (size_t)v * 3;
+    const float d0 = pd[0], d1 = pd[1], d2 = pd[2];
+#pragma unroll
+    for (int r = 0; r < kSkinRows; ++r) {
+      const float f = sF[r][k];
+      p[r][0] = fmaf(f, d0, p[r][0]); p[r][1] = fmaf(f, d1, p[r][1]); p[r][2] = fmaf(f, d2, p[r][2]);
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < kSkinRows; ++r) {
+    if (r >= nr) break;
+    float T[12];
+#pragma unroll
+    for (int i = 0; i < 12; ++i) T[i] = 0.f;
+    for (int j = 0; j < NJ; ++j) {
+      const float w = lbs_weights[(size_t)v * NJ + j];
+#pragma unroll
+      for (int i = 0; i < 12; ++i) T[i] = fmaf(w, sA[r][j * 12 + i], T[i]);
+    }
+    const size_t o = ((size_t)(b0 + r) * V + v) * 3;
+    float g0 = g_verts[o], g1 = g_verts[o + 1], g2 = g_verts[o + 2];
+    if (pr.on) {     // q = o @ m  ->  g_o = m g_q
+      const float h0 = pr.m[0] * g0 + pr.m[1] * g1 + pr.m[2] * g2;
+      const float h1 = pr.m[3] * g0 + pr.m[4] * g1 + pr.m[5] * g2;
+      const float h2 = pr.m[6] * g0 + pr.m[7] * g1 + pr.m[8] * g2;
+      g0 = h0; g1 = h1; g2 = h2;
+    }
+    p_out[o] = p[r][0]; p_out[o + 1] = p[r][1]; p_out[o + 2] = p[r][2];
+    go_out[o] = g0; go_out[o + 1] = g1; go_out[o + 2] = g2;
+    gp_out[o] = T[0] * g0 + T[4] * g1 + T[8] * g2;
+    gp_out[o + 1] = T[1] * g0 + T[5] * g1 + T[9] * g2;
+    gp_out[o + 2] = T[2] * g0 + T[6] * g1 + T[10] * g2;
+  }
+}
+
+// CTA (joint j, row b): dA[b][j] = sum_v w_vj g_o(v) [p(v); 1]^T, a 3 x 4 block
+__global__ void __launch_bounds__(256)
+k_pose_dA(const float* __restrict__ lbs_weights, const float* __restrict__ p, const float* __restrict__ go, int V,
+          int NJ, float* __restrict__ dA) {
+  __shared__ float red[12 * 32];
+  const int j = blockIdx.x, b = blockIdx.y;
+  float acc[12];
+#pragma unroll
+  for (int i = 0; i < 12; ++i) acc[i] = 0.f;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) {
+    const float w = lbs_weights[(size_t)v * NJ + j];
+    if (w == 0.f) continue;
+    const size_t o = ((size_t)b * V + v) * 3;
+    const float q[4] = {p[o], p[o + 1], p[o + 2], 1.f};
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const float wg = w * go[o + r];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) acc[r * 4 + c] = fmaf(wg, q[c], acc[r * 4 + c]);
+    }
+  }
+  block_sum_n<12>(acc, red);
+  if (threadIdx.x < 12) dA[((size_t)b * NJ + j) * 12 + threadIdx.x] = red[threadIdx.x * 32];
+}
+
+// CTA (pose feature k, kSkinRows rows): g_feat[b][k] = posedirs[k] . g_p[b] over the 3V entries
+__global__ void __launch_bounds__(256)
+k_pose_gfeat(const float* __restrict__ posedirs, const float* __restrict__ gp, int V3, int NF, int B,
+             float* __restrict__ gfeat) {
+  __shared__ float red[kSkinRows * 32];
+  const int k = blockIdx.x, b0 = blockIdx.y * kSkinRows;
+  const int nr = min(kSkinRows, B - b0);
+  float acc[kSkinRows];
+#pragma unroll
+  for (int r = 0; r < kSkinRows; ++r) acc[r] = 0.f;
+  const float* pd = posedirs + (size_t)k * V3;
+  for (int i = threadIdx.x; i < V3; i += blockDim.x) {
+    const float d = pd[i];
+#pragma unroll
+    for (int r = 0; r < kSkinRows; ++r)
+      if (r < nr) acc[r] = fmaf(d, gp[(size_t)(b0 + r) * V3 + i], acc[r]);
+  }
+  block_sum_n<kSkinRows>(acc, red);
+  if (threadIdx.x < nr) gfeat[(size_t)(b0 + threadIdx.x) * NF + k] = red[threadIdx.x * 32];
+}
+
+// one warp per pose row, lane j = joint j: the kinematic chain in reverse (children before parents, each parent
+// adding its children's terms in lane order), then batch_rodrigues' backward (the +1e-8 inside the norm included)
+__global__ void __launch_bounds__(128)
+k_pose_chain_bwd(const float* __restrict__ body_pose, int P, int B, const float* __restrict__ Jg,
+                 const int* __restrict__ parents, int NJ, const float* __restrict__ A, const float* __restrict__ feat,
+                 const float* __restrict__ dA, const float* __restrict__ gfeat, float* __restrict__ g_pose) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;                        // warp-uniform
+  const int j = lane;
+  const bool act = j < NJ;
+  const int NF = (NJ - 1) * 9;
+  const int par = act ? parents[j] : -1;
+  int depth = 0;
+  {
+    int p = par;
+    for (int it = 0; it < NJ_MAX; ++it) {
+      int pp = __shfl_sync(0xffffffffu, par, p < 0 ? 0 : p);
+      if (p >= 0) { ++depth; p = pp; }
+    }
+  }
+  int maxd = depth;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) maxd = max(maxd, __shfl_xor_sync(0xffffffffu, act ? maxd : 0, o));
+  // forward values: R_j = feat_j + I, t_j = J_j - J_par, the parent's world rotation P3 = A[par][:, :3]
+  float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, t[3] = {0.f, 0.f, 0.f}, P3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  const float Jx = act ? Jg[j * 3] : 0.f, Jy = act ? Jg[j * 3 + 1] : 0.f, Jz = act ? Jg[j * 3 + 2] : 0.f;
+  if (act && j >= 1) {
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = feat[(size_t)b * NF + (j - 1) * 9 + i] + ((i % 4 == 0) ? 1.f : 0.f);
+    t[0] = Jx - Jg[par * 3]; t[1] = Jy - Jg[par * 3 + 1]; t[2] = Jz - Jg[par * 3 + 2];
+    const float* ap = A + ((size_t)b * NJ + par) * 12;
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) P3[r * 3 + c] = ap[r * 4 + c];
+  }
+  // A = G - [0 | G_3x3 J]:  g_G3 = dA3 - dA_t J^T, g_Gt = dA_t
+  float gG[12];
+  if (act) {
+    const float* d = dA + ((size_t)b * NJ + j) * 12;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const float dt = d[r * 4 + 3];
+      gG[r * 4 + 0] = d[r * 4 + 0] - dt * Jx;
+      gG[r * 4 + 1] = d[r * 4 + 1] - dt * Jy;
+      gG[r * 4 + 2] = d[r * 4 + 2] - dt * Jz;
+      gG[r * 4 + 3] = dt;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 12; ++i) gG[i] = 0.f;
+  }
+  // G_j = G_par [R_j | t_j]:  g_Gpar3 += g_G3 R^T + g_Gt t^T, g_Gpar_t += g_Gt
+  for (int d = maxd; d >= 1; --d) {
+    float cP[12];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        cP[r * 4 + c] = gG[r * 4] * R[c * 3] + gG[r * 4 + 1] * R[c * 3 + 1] + gG[r * 4 + 2] * R[c * 3 + 2] +
+                        gG[r * 4 + 3] * t[c];
+      cP[r * 4 + 3] = gG[r * 4 + 3];
+    }
+    const bool send = act && depth == d;
+    for (int src = 0; src < 32; ++src) {
+      const int ps = __shfl_sync(0xffffffffu, send ? par : -1, src);
+      float add[12];
+#pragma unroll
+      for (int i = 0; i < 12; ++i) add[i] = __shfl_sync(0xffffffffu, cP[i], src);
+      if (ps == j)
+#pragma unroll
+        for (int i = 0; i < 12; ++i) gG[i] += add[i];
+    }
+  }
+  if (!act || j == 0) return;
+  // G3 = P3 R:  g_R = P3^T g_G3, plus the pose feature's (feat = R - I)
+  float gR[9];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      gR[k * 3 + c] = P3[k] * gG[c] + P3[3 + k] * gG[4 + c] + P3[6 + k] * gG[8 + c] +
+                      gfeat[(size_t)b * NF + (j - 1) * 9 + k * 3 + c];
+  float rv[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int q = (j - 1) * 3 + c;
+    rv[c] = q < P ? body_pose[(size_t)b * P + q] : 0.f;
+  }
+  const float eps = 1e-8f;
+  const float ang = sqrtf((rv[0] + eps) * (rv[0] + eps) + (rv[1] + eps) * (rv[1] + eps) + (rv[2] + eps) * (rv[2] + eps));
+  const float x = rv[0] / ang, y = rv[1] / ang, z = rv[2] / ang;
+  float s, c;
+  sincosf(ang, &s, &c);
+  const float K[9] = {0, -z, y, z, 0, -x, -y, x, 0};
+  float KK[9];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int bb = 0; bb < 3; ++bb) KK[a * 3 + bb] = K[a * 3] * K[bb] + K[a * 3 + 1] * K[3 + bb] + K[a * 3 + 2] * K[6 + bb];
+  // R = I + s K + (1 - c) K K
+  float gs = 0.f, gc = 0.f;
+#pragma unroll
+  for (int i = 0; i < 9; ++i) { gs += gR[i] * K[i]; gc -= gR[i] * KK[i]; }
+  const float omc = 1.f - c;
+  float gK[9];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int bb = 0; bb < 3; ++bb) {
+      // d(KK) -> g_K += g_KK K^T + K^T g_KK with g_KK = (1 - c) g_R
+      float m = 0.f;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) m += gR[a * 3 + k] * K[bb * 3 + k] + K[k * 3 + a] * gR[k * 3 + bb];
+      gK[a * 3 + bb] = s * gR[a * 3 + bb] + omc * m;
+    }
+  const float gx = gK[7] - gK[5], gy = gK[2] - gK[6], gz = gK[3] - gK[1];
+  const float gang = gs * c - gc * s - (gx * rv[0] + gy * rv[1] + gz * rv[2]) / (ang * ang);
+  const float ga[3] = {gx, gy, gz};
+#pragma unroll
+  for (int cc = 0; cc < 3; ++cc) {
+    const int q = (j - 1) * 3 + cc;
+    if (q < P) g_pose[(size_t)b * P + q] = ga[cc] / ang + gang * (rv[cc] + eps) / ang;
+  }
+}
+
+// ---------------------------------------------------------------- textured render backward
+// per supersample of image img: the lit colour the forward averaged (ss_rgb) and dl = g_ss . unlit sample, this
+// supersample's share of the gradient of its face's light (g_ss = g_pixel / ss^2, avg-pool's backward); background 0
+__global__ void k_rb_samples(const unsigned long long* __restrict__ zbuf, const int* __restrict__ faces,
+                             const float* __restrict__ verts, const float4* __restrict__ proj,
+                             const float* __restrict__ tex, int R, int V, int B, int G, int A,
+                             const LookAtCam* __restrict__ cams, int n, int ss, const float* __restrict__ g_rgb,
+                             float* __restrict__ ss_rgb, float* __restrict__ dl) {
+  const int img = blockIdx.y, a = img / B, b = img - a * B;
+  const LookAtCam c = cams[(b / G) * A + a];
+  const int is = c.is;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= is * is) return;
+  const int row = q / is, xi = q - row * is;
+  const size_t o = (size_t)img * is * is + q;
+  const unsigned long long zb = zbuf[o];
+  float* out = ss_rgb + o * 3;
+  if (zb == ~0ull) {
+    out[0] = 0.f; out[1] = 0.f; out[2] = 0.f;
+    dl[o] = 0.f;
+    return;
+  }
+  const int f = (int)(zb & 0xffffffffu);
+  const float zp = __uint_as_float((unsigned)(zb >> 32));
+  float col[3], light;
+  textured_sample(row, xi, f, zp, faces, verts + (size_t)b * V * 3, proj + (size_t)img * V, tex, R, c, col, &light);
+  out[0] = col[0] * light; out[1] = col[1] * light; out[2] = col[2] * light;
+  const float* g = g_rgb + ((size_t)img * n * n + (size_t)(row / ss) * n + xi / ss) * 3;
+  const float inv = 1.f / (float)(ss * ss);
+  dl[o] = (g[0] * inv) * col[0] + (g[1] * inv) * col[1] + (g[2] * inv) * col[2];
+}
+
+__device__ __forceinline__ int face_at(const unsigned long long* zbuf, size_t i) {
+  return (int)(unsigned)(zbuf[i] & 0xffffffffu);      // background ~0 -> -1
+}
+
+// neural_renderer's backward_pixel_map of face f in one image (rgb only, fp32), its corners in the winding of the
+// drawn copy: pxy [3][2] their NDC x, y; adds d loss / d (x, y) of each corner to gxy.  Pixel coordinates and the
+// crossings are rounded op by op (no contraction), so an fp32 restatement makes the same pixel choices.
+__device__ __forceinline__ void edge_sweep(const float (&pxy)[3][2], int f, const unsigned long long* __restrict__ zbuf,
+                           const float* __restrict__ rgb, const float* __restrict__ g_rgb, int is, int n, int ss,
+                           float (&gxy)[3][2]) {
+  const float eps = 1e-4f;                   // neural_renderer's DEFAULT_EPS
+  const float inv = 1.f / (float)(ss * ss);
+  const float fis = (float)is;
+  float pp[3][2];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int d = 0; d < 2; ++d) pp[k][d] = __fmul_rn(0.5f, __fadd_rn(__fadd_rn(__fmul_rn(pxy[k][d], fis), fis), -1.f));
+  auto gpix = [&](size_t i) {                // g at supersample i = (row, col)
+    const int row = (int)(i / is), col = (int)(i - (size_t)row * is);
+    return g_rgb + ((size_t)(row / ss) * n + col / ss) * 3;
+  };
+  // unrolled, so that every index into pp and gxy is a constant (no local memory)
+#pragma unroll
+  for (int e = 0; e < 3; ++e) {
+    const int pi[3] = {e, (e + 1) % 3, (e + 2) % 3};
+#pragma unroll
+    for (int axis = 0; axis < 2; ++axis) {
+      float p[3][2];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { p[k][0] = pp[pi[k]][axis]; p[k][1] = pp[pi[k]][1 - axis]; }
+      if (p[0][0] == p[1][0]) continue;      // neural_renderer divides 0 by 0 here
+      int direction = p[0][0] < p[1][0] ? -1 : 1;
+      if (axis == 1) direction = -direction;
+      const float span = __fadd_rn(p[1][0], -p[0][0]);
+      const float slope = __fdiv_rn(__fadd_rn(p[1][1], -p[0][1]), span);
+      const int d0_from = max((int)ceilf(fminf(p[0][0], p[1][0])), 0);
+      const int d0_to = min((int)floorf(fmaxf(p[0][0], p[1][0])), is - 1);
+      for (int d0 = d0_from; d0 <= d0_to; ++d0) {
+        const float fd0 = (float)d0;
+        const float d1_cross = __fadd_rn(__fmul_rn(slope, __fadd_rn(fd0, -p[0][0])), p[0][1]);
+        const int d1_in = direction > 0 ? (int)floorf(d1_cross) : (int)ceilf(d1_cross);
+        const int d1_out = d1_in + direction;
+        if (d1_in < 0 || d1_in >= is || d1_out < 0 || d1_out >= is) continue;
+        auto pix = [&](int d1) {
+          return axis == 0 ? (size_t)(is - 1 - d1) * is + d0 : (size_t)(is - 1 - d0) * is + d1;
+        };
+        const float* rin = rgb + pix(d1_in) * 3;
+        const float* rout = rgb + pix(d1_out) * 3;
+        // the two distance factors of the edge's end points
+        const bool use0 = p[1][0] != fd0, use1 = p[0][0] != fd0;
+        const float f0 = use0 ? span / (p[1][0] - fd0) : 0.f;
+        const float f1 = use1 ? span / (fd0 - p[0][0]) : 0.f;
+        auto add = [&](int d1, float diff) {
+          const float base = (d1 - d1_cross) * 2.f / fis;
+          if (use0) {
+            float dist = f0 * base;
+            dist = dist > 0.f ? dist + eps : dist - eps;
+            gxy[pi[0]][1 - axis] -= diff / dist;
+          }
+          if (use1) {
+            float dist = f1 * base;
+            dist = dist > 0.f ? dist + eps : dist - eps;
+            gxy[pi[1]][1 - axis] -= diff / dist;
+          }
+        };
+        // out: the in-pixel is f's, sweep the pixels beyond the edge up to the border
+        if (face_at(zbuf, pix(d1_in)) == f) {
+          const int lim = direction > 0 ? is - 1 : 0;
+          const int lo = min(d1_out, lim), hi = max(d1_out, lim);
+          for (int d1 = lo; d1 <= hi; ++d1) {
+            const size_t i = pix(d1);
+            const float* r = rgb + i * 3;
+            const float* g = gpix(i);
+            const float diff = (r[0] - rin[0]) * (g[0] * inv) + (r[1] - rin[1]) * (g[1] * inv) +
+                               (r[2] - rin[2]) * (g[2] * inv);
+            if (diff > 0.f) add(d1, diff);
+          }
+        }
+        // in: f's pixels from the edge to the face's opposite edge
+        {
+          float cross2;
+          if ((fd0 - p[0][0]) * (fd0 - p[2][0]) < 0.f)
+            cross2 = __fadd_rn(__fmul_rn(__fdiv_rn(__fadd_rn(p[2][1], -p[0][1]), __fadd_rn(p[2][0], -p[0][0])),
+                                         __fadd_rn(fd0, -p[0][0])), p[0][1]);
+          else
+            cross2 = __fadd_rn(__fmul_rn(__fdiv_rn(__fadd_rn(p[1][1], -p[2][1]), __fadd_rn(p[1][0], -p[2][0])),
+                                         __fadd_rn(fd0, -p[2][0])), p[2][1]);
+          int lim = d1_in;                   // a vertical opposite edge through the column: only d1_in
+          if (isfinite(cross2)) {
+            const float l = direction > 0 ? ceilf(cross2) : floorf(cross2);
+            lim = (int)fminf(fmaxf(l, -1.f), (float)is);
+          }
+          const int lo = max(min(d1_in, lim), 0), hi = min(max(d1_in, lim), is - 1);
+          for (int d1 = lo; d1 <= hi; ++d1) {
+            const size_t i = pix(d1);
+            if (face_at(zbuf, i) != f) continue;
+            const float* r = rgb + i * 3;
+            const float* g = gpix(i);
+            const float diff = (r[0] - rout[0]) * (g[0] * inv) + (r[1] - rout[1]) * (g[1] * inv) +
+                               (r[2] - rout[2]) * (g[2] * inv);
+            if (diff > 0.f) add(d1, diff);
+          }
+        }
+      }
+    }
+  }
+}
+
+// thread per (image, face): the edge sweep of the drawn copy, the projection's backward, and the light's backward,
+// written per corner: gface [A B][F][3][3] (world frame of the vertices as given to the forward)
+// (128, 4): with one block per SM as the target ptxas held the kernel to 96 registers and spilled 12 bytes
+__global__ void __launch_bounds__(128, 4)
+k_rb_faces(const unsigned long long* __restrict__ zbuf, const int* __restrict__ faces, int F,
+           const float* __restrict__ verts, const float4* __restrict__ proj, int V, int B, int G, int A,
+           const LookAtCam* __restrict__ cams, int n, int ss, const float* __restrict__ ss_rgb,
+           const float* __restrict__ dl, const float* __restrict__ g_rgb, float* __restrict__ gface) {
+  const int img = blockIdx.y, a = img / B, b = img - a * B;
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  const LookAtCam c = cams[(b / G) * A + a];
+  const int is = c.is;
+  const size_t npix = (size_t)is * is;
+  const unsigned long long* zb = zbuf + (size_t)img * npix;
+  const float4* pj = proj + (size_t)img * V;
+  const float* vb = verts + (size_t)b * V * 3;
+  const int idx[3] = {faces[f * 3], faces[f * 3 + 1], faces[f * 3 + 2]};
+  const float4 q[3] = {pj[idx[0]], pj[idx[1]], pj[idx[2]]};
+  float g[3][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+  float* out = gface + ((size_t)img * F + f) * 9;
+  if (q[0].z <= 0.f || q[1].z <= 0.f || q[2].z <= 0.f) {       // never drawn
+#pragma unroll
+    for (int i = 0; i < 9; ++i) out[i] = 0.f;
+    return;
+  }
+  // (b) the edge sweep of the drawn copy: the face as given when it faces the camera (neural_renderer's backside
+  // test), else fill_back's reversed copy (v2, v1, v0)
+  const bool front = (q[2].y - q[0].y) * (q[1].x - q[0].x) >= (q[1].y - q[0].y) * (q[2].x - q[0].x);
+  const float4 o[3] = {front ? q[0] : q[2], q[1], front ? q[2] : q[0]};     // corners in the drawn winding
+  float pxy[3][2], gxy[3][2];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    pxy[k][0] = o[k].x; pxy[k][1] = o[k].y;
+    gxy[k][0] = 0.f; gxy[k][1] = 0.f;
+  }
+  edge_sweep(pxy, f, zb, ss_rgb + (size_t)img * npix * 3, g_rgb + (size_t)img * n * n * 3, is, n, ss, gxy);
+  // (a) light: the sum of dl over f's supersamples, in raster_face's bounding box, row-major
+  float dlight = 0.f;
+  {
+    const float xmin = fminf(q[0].x, fminf(q[1].x, q[2].x)), xmax = fmaxf(q[0].x, fmaxf(q[1].x, q[2].x));
+    const float ymin = fminf(q[0].y, fminf(q[1].y, q[2].y)), ymax = fmaxf(q[0].y, fmaxf(q[1].y, q[2].y));
+    // one pixel wider than raster_face's box: f's supersamples lie inside however the bounds round
+    const int xi0 = max(0, (int)ceilf((xmin * is + is - 1.f) * 0.5f) - 1);
+    const int xi1 = min(is - 1, (int)floorf((xmax * is + is - 1.f) * 0.5f) + 1);
+    const int yi0 = max(0, (int)ceilf((ymin * is + is - 1.f) * 0.5f) - 1);
+    const int yi1 = min(is - 1, (int)floorf((ymax * is + is - 1.f) * 0.5f) + 1);
+    const float* d = dl + (size_t)img * npix;
+    for (int yi = yi1; yi >= yi0; --yi)
+      for (int xi = xi0; xi <= xi1; ++xi) {
+        const size_t i = (size_t)(is - 1 - yi) * is + xi;
+        if (face_at(zb, i) == f) dlight += d[i];
+      }
+  }
+  if (dlight != 0.f) {
+    const float* v0 = vb + 3 * idx[0];
+    const float* v1 = vb + 3 * idx[1];
+    const float* v2 = vb + 3 * idx[2];
+    const float ea[3] = {v0[0] - v1[0], v0[1] - v1[1], v0[2] - v1[2]};
+    const float eb[3] = {v2[0] - v1[0], v2[1] - v1[1], v2[2] - v1[2]};
+    const float nx = ea[1] * eb[2] - ea[2] * eb[1], ny = ea[2] * eb[0] - ea[0] * eb[2], nz = ea[0] * eb[1] - ea[1] * eb[0];
+    const float len = sqrtf(nx * nx + ny * ny + nz * nz);
+    const float nl = fmaxf(len, 1e-5f);
+    const float s = (nx * (c.eye[0] - v1[0]) + ny * (c.eye[1] - v1[1]) + nz * (c.eye[2] - v1[2])) >= 0.f ? 1.f : -1.f;
+    if (s * ny / nl > 0.f) {                 // relu's gradient is 0 at <= 0
+      // light = 0.5 + 0.5 s n_y / max(|n|, 1e-5)
+      const float k = 0.5f * s * dlight;
+      float gn[3] = {0.f, k / nl, 0.f};
+      if (len > 1e-5f) {
+        const float m = k * ny / (len * len * len);
+        gn[0] -= m * nx; gn[1] -= m * ny; gn[2] -= m * nz;
+      }
+      // n = ea x eb:  g_ea = eb x g_n, g_eb = g_n x ea
+      const float ga[3] = {eb[1] * gn[2] - eb[2] * gn[1], eb[2] * gn[0] - eb[0] * gn[2], eb[0] * gn[1] - eb[1] * gn[0]};
+      const float gb[3] = {gn[1] * ea[2] - gn[2] * ea[1], gn[2] * ea[0] - gn[0] * ea[2], gn[0] * ea[1] - gn[1] * ea[0]};
+#pragma unroll
+      for (int k3 = 0; k3 < 3; ++k3) {
+        g[0][k3] += ga[k3];
+        g[2][k3] += gb[k3];
+        g[1][k3] -= ga[k3] + gb[k3];
+      }
+    }
+  }
+  // (c) projection: x' = x_c / z_c / tan 30, y' likewise; c = R (v - eye)
+  float gw[3][3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float gx = gxy[k][0], gy = gxy[k][1];
+    const float iz = 1.f / o[k].z;
+    const float gcx = gx * c.inv_width * iz, gcy = gy * c.inv_width * iz, gcz = -(gx * o[k].x + gy * o[k].y) * iz;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) gw[k][d] = c.rx[d] * gcx + c.ry[d] * gcy + c.rz[d] * gcz;
+  }
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    g[0][d] += front ? gw[0][d] : gw[2][d];
+    g[1][d] += gw[1][d];
+    g[2][d] += front ? gw[2][d] : gw[0][d];
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int d = 0; d < 3; ++d) out[k * 3 + d] = g[k][d];
+}
+
+// thread per (row b, vertex v): g_verts[b][v] = sum over the angles, then over v's faces in ascending order, of the
+// corners of those faces that are v
+__global__ void k_rb_gather(const float* __restrict__ gface, const int* __restrict__ faces, int F,
+                            const int* __restrict__ offsets, const int* __restrict__ vf, int V, int B, int A,
+                            float* __restrict__ g_verts) {
+  const int b = blockIdx.y;
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+  const int e0 = offsets[v], e1 = offsets[v + 1];
+  for (int a = 0; a < A; ++a) {
+    const float* gf = gface + (size_t)(a * B + b) * F * 9;
+    int prev = -1;
+    for (int e = e0; e < e1; ++e) {
+      const int f = vf[e];
+      if (f == prev) continue;               // a face naming v twice is listed twice
+      prev = f;
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (faces[f * 3 + k] == v) {
+          const float* x = gf + (size_t)f * 9 + k * 3;
+          s0 += x[0]; s1 += x[1]; s2 += x[2];
+        }
+    }
+  }
+  float* o = g_verts + ((size_t)b * V + v) * 3;
+  o[0] = s0; o[1] = s1; o[2] = s2;
+}
+
+// ---------------------------------------------------------------- CLIP prep and loss
+// thread per (row b, source pixel): avc_clip_prep_nearest's backward, the output pixels that read it summed in
+// row-major order, each divided by its channel's std
+__global__ void k_clip_prep_nearest_bwd(const float* __restrict__ g_out, int B, int n, int S, float* __restrict__ g_img) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)B * n * n) return;
+  const int sx = (int)(i % n), sy = (int)((i / n) % n), b = (int)(i / ((long long)n * n));
+  const float scale = (float)n / (float)S;
+  const int y0 = max(0, (int)((float)sy / scale) - 2), y1 = min(S - 1, (int)((float)(sy + 1) / scale) + 2);
+  const int x0 = max(0, (int)((float)sx / scale) - 2), x1 = min(S - 1, (int)((float)(sx + 1) / scale) + 2);
+  float acc[3] = {0.f, 0.f, 0.f};
+  for (int y = y0; y <= y1; ++y) {
+    if (min((int)floorf(y * scale), n - 1) != sy) continue;
+    for (int x = x0; x <= x1; ++x) {
+      if (min((int)floorf(x * scale), n - 1) != sx) continue;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const double stdv = ch == 0 ? 0.26862954 : (ch == 1 ? 0.26130258 : 0.27577711);
+        acc[ch] += (float)((double)g_out[(((size_t)b * 3 + ch) * S + y) * S + x] / stdv);
+      }
+    }
+  }
+  float* o = g_img + (size_t)i * 3;
+  o[0] = acc[0]; o[1] = acc[1]; o[2] = acc[2];
+}
+
+// one CTA per pose b: loss[b] = 1 - cos(mean_a emb[a][b], text) as k_pose_score computes the cosine, and
+// g_emb[a][b] = d loss[b] / d emb[a][b]
+__global__ void k_pose_clip_loss(const float* __restrict__ emb, int A, int B, int Dm, const float* __restrict__ text,
+                                 float* __restrict__ loss, float* __restrict__ g_emb) {
+  __shared__ double red[32];
+  const int b = blockIdx.x;
+  double xx = 0.0, xy = 0.0, yy = 0.0;
+  for (int j = threadIdx.x; j < Dm; j += blockDim.x) {
+    double s = 0.0;
+    for (int a = 0; a < A; ++a) s += emb[((size_t)a * B + b) * Dm + j];
+    const double f = (float)(s / A), t = text[j];
+    xx += f * f; xy += f * t; yy += t * t;
+  }
+  xx = block_sum_d(xx, red);
+  xy = block_sum_d(xy, red);
+  yy = block_sum_d(yy, red);
+  const double lf = sqrt(xx), nf = fmax(lf, 1e-8), nt = fmax(sqrt(yy), 1e-8);
+  const double cs = xy / (nf * nt);
+  if (threadIdx.x == 0 && loss) loss[b] = (float)(1.0 - (double)(float)cs);
+  for (int j = threadIdx.x; j < Dm; j += blockDim.x) {
+    double s = 0.0;
+    for (int a = 0; a < A; ++a) s += emb[((size_t)a * B + b) * Dm + j];
+    const double f = (float)(s / A);
+    double dc = text[j] / (nf * nt);
+    if (lf > 1e-8) dc -= cs * f / (nf * lf);
+    const float gv = (float)(-dc / A);
+    for (int a = 0; a < A; ++a) g_emb[((size_t)a * B + b) * Dm + j] = gv;
+  }
+}
+
 }  // namespace
+
+// the batched render's passes with its cameras copied (kind: from host or device memory) into the workspace
+static int raster_batch_run(const float* verts, int B, int group, const int* faces, const float* textures, int V,
+                            int F, int R, const void* cams_src, cudaMemcpyKind kind, int A, int image_size,
+                            int supersample, float* rgb_out, void* workspace, avc_stream_t stream) {
+  const int ngroups = (B + group - 1) / group;
+  const int is = image_size * supersample;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver c(workspace);
+  LookAtCam* cams = c.take<LookAtCam>((size_t)ngroups * A);
+  float4* proj = c.take<float4>((size_t)A * B * V);
+  unsigned long long* zbuf = c.take<unsigned long long>((size_t)A * B * is * is);
+  AVC_CUDA_TRY(cudaMemcpyAsync(cams, cams_src, sizeof(LookAtCam) * (size_t)ngroups * A, kind, st));
+  AVC_CUDA_TRY(cudaMemsetAsync(zbuf, 0xff, sizeof(unsigned long long) * (size_t)A * B * is * is, st));
+  const unsigned nimg = (unsigned)(A * B);
+  k_project_batch<<<dim3((V + 255) / 256, nimg), 256, 0, st>>>(verts, V, B, group, A, cams, proj);
+  k_raster_batch<<<dim3((F + 127) / 128, nimg), 128, 0, st>>>(proj, V, faces, F, is, zbuf);
+  k_resolve_batch<<<dim3((image_size * image_size + 255) / 256, nimg), 256, 0, st>>>(
+      zbuf, faces, verts, proj, textures, R, V, B, group, A, cams, image_size, supersample, rgb_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
 
 extern "C" {
 
@@ -822,19 +1432,163 @@ int avc_raster_textured_batch(const float* verts, int32_t B, int32_t group, cons
   std::vector<LookAtCam> hc((size_t)ngroups * A);
   for (int i = 0; i < ngroups * A; ++i)
     if (!make_look_at_cam(eyes + 3 * i, at, up, is, &hc[i])) return AVC_E_BADCFG;
-  cudaStream_t st = (cudaStream_t)stream;
-  Carver c(workspace);
-  LookAtCam* cams = c.take<LookAtCam>((size_t)ngroups * A);
-  float4* proj = c.take<float4>((size_t)A * B * V);
-  unsigned long long* zbuf = c.take<unsigned long long>((size_t)A * B * is * is);
   // from pageable memory: the call returns once hc is staged, so it may be freed on return
-  AVC_CUDA_TRY(cudaMemcpyAsync(cams, hc.data(), sizeof(LookAtCam) * hc.size(), cudaMemcpyHostToDevice, st));
-  AVC_CUDA_TRY(cudaMemsetAsync(zbuf, 0xff, sizeof(unsigned long long) * (size_t)A * B * is * is, st));
+  return raster_batch_run(verts, B, group, faces, textures, V, F, R, hc.data(), cudaMemcpyHostToDevice, A, image_size,
+                          supersample, rgb_out, workspace, stream);
+}
+
+int avc_look_at_cam_bytes(size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  *bytes = sizeof(LookAtCam);
+  return 0;
+}
+
+int avc_look_at_cams(const float* eyes, int32_t n, const float* at, const float* up, int32_t image_size,
+                     int32_t supersample, void* cams_out, avc_stream_t stream) {
+  if (!eyes || !at || !up || !cams_out) return AVC_E_NULL;
+  if (n < 1 || image_size < 1 || image_size > 4096 || supersample < 1 || supersample > 4) return AVC_E_SIZE;
+  std::vector<LookAtCam> hc((size_t)n);
+  for (int i = 0; i < n; ++i)
+    if (!make_look_at_cam(eyes + 3 * i, at, up, image_size * supersample, &hc[i])) return AVC_E_BADCFG;
+  AVC_CUDA_TRY(cudaMemcpyAsync(cams_out, hc.data(), sizeof(LookAtCam) * hc.size(), cudaMemcpyHostToDevice,
+                               (cudaStream_t)stream));
+  return 0;
+}
+
+int avc_raster_textured_batch_dev(const float* verts, int32_t B, int32_t group, const int32_t* faces,
+                                  const float* textures, int32_t V, int32_t F, int32_t R, const void* cams, int32_t A,
+                                  int32_t image_size, int32_t supersample, float* rgb_out, void* workspace,
+                                  size_t workspace_bytes, avc_stream_t stream) {
+  if (!verts || !faces || !textures || !cams || !rgb_out || !workspace) return AVC_E_NULL;
+  if (B < 1 || group < 1 || A < 1 || A > kMaxCams || F < 1 || R < 2 || R > 64) return AVC_E_SIZE;
+  const int ngroups = (B + group - 1) / group;
+  size_t need = 0;
+  AVC_TRY(avc_raster_textured_batch_workspace_bytes(V, A * B, ngroups * A, image_size, supersample, &need));
+  if (workspace_bytes < need) return AVC_E_SIZE;
+  return raster_batch_run(verts, B, group, faces, textures, V, F, R, cams, cudaMemcpyDeviceToDevice, A, image_size,
+                          supersample, rgb_out, workspace, stream);
+}
+
+int avc_raster_textured_batch_bwd_workspace_bytes(int32_t F, int32_t n_images, int32_t image_size,
+                                                  int32_t supersample, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (F < 1 || n_images < 1 || n_images > 65535 || image_size < 1 || image_size > 4096 || supersample < 1 ||
+      supersample > 4)
+    return AVC_E_SIZE;
+  const size_t npix = (size_t)image_size * supersample * image_size * supersample;
+  Carver c(nullptr);
+  c.take<float>((size_t)n_images * npix * 3);
+  c.take<float>((size_t)n_images * npix);
+  c.take<float>((size_t)n_images * F * 9);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_raster_textured_batch_bwd(const float* verts, int32_t B, int32_t group, const int32_t* faces,
+                                  const float* textures, int32_t V, int32_t F, int32_t R, int32_t A,
+                                  int32_t image_size, int32_t supersample, const int32_t* offsets, const int32_t* vf,
+                                  const float* g_rgb, float* g_verts, const void* fwd_workspace,
+                                  size_t fwd_workspace_bytes, void* workspace, size_t workspace_bytes,
+                                  avc_stream_t stream) {
+  if (!verts || !faces || !textures || !offsets || !vf || !g_rgb || !g_verts || !fwd_workspace || !workspace)
+    return AVC_E_NULL;
+  if (B < 1 || group < 1 || A < 1 || A > kMaxCams || F < 1 || R < 2 || R > 64) return AVC_E_SIZE;
+  const int ngroups = (B + group - 1) / group;
+  size_t need_f = 0, need = 0;
+  AVC_TRY(avc_raster_textured_batch_workspace_bytes(V, A * B, ngroups * A, image_size, supersample, &need_f));
+  AVC_TRY(avc_raster_textured_batch_bwd_workspace_bytes(F, A * B, image_size, supersample, &need));
+  if (fwd_workspace_bytes < need_f || workspace_bytes < need) return AVC_E_SIZE;
+  const int is = image_size * supersample;
+  const size_t npix = (size_t)is * is;
+  Carver cf(const_cast<void*>(fwd_workspace));
+  const LookAtCam* cams = cf.take<LookAtCam>((size_t)ngroups * A);
+  const float4* proj = cf.take<float4>((size_t)A * B * V);
+  const unsigned long long* zbuf = cf.take<unsigned long long>((size_t)A * B * npix);
+  Carver c(workspace);
+  float* ss_rgb = c.take<float>((size_t)A * B * npix * 3);
+  float* dl = c.take<float>((size_t)A * B * npix);
+  float* gface = c.take<float>((size_t)A * B * F * 9);
+  cudaStream_t st = (cudaStream_t)stream;
   const unsigned nimg = (unsigned)(A * B);
-  k_project_batch<<<dim3((V + 255) / 256, nimg), 256, 0, st>>>(verts, V, B, group, A, cams, proj);
-  k_raster_batch<<<dim3((F + 127) / 128, nimg), 128, 0, st>>>(proj, V, faces, F, is, zbuf);
-  k_resolve_batch<<<dim3((image_size * image_size + 255) / 256, nimg), 256, 0, st>>>(
-      zbuf, faces, verts, proj, textures, R, V, B, group, A, cams, image_size, supersample, rgb_out);
+  k_rb_samples<<<dim3((unsigned)((npix + 255) / 256), nimg), 256, 0, st>>>(
+      zbuf, faces, verts, proj, textures, R, V, B, group, A, cams, image_size, supersample, g_rgb, ss_rgb, dl);
+  k_rb_faces<<<dim3((F + 127) / 128, nimg), 128, 0, st>>>(zbuf, faces, F, verts, proj, V, B, group, A, cams,
+                                                          image_size, supersample, ss_rgb, dl, g_rgb, gface);
+  k_rb_gather<<<dim3((V + 127) / 128, B), 128, 0, st>>>(gface, faces, F, offsets, vf, V, B, A, g_verts);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_smpl_pose_batch_bwd_workspace_bytes(int32_t B, int32_t V, int32_t n_joints, size_t* bytes) {
+  if (!bytes) return AVC_E_NULL;
+  if (B < 1 || V < 1 || n_joints < 2 || n_joints > NJ_MAX) return AVC_E_SIZE;
+  Carver c(nullptr);
+  c.take<float>((size_t)n_joints * 3);
+  c.take<float>((size_t)B * n_joints * 12);
+  c.take<float>((size_t)B * (n_joints - 1) * 9);
+  for (int i = 0; i < 3; ++i) c.take<float>((size_t)B * V * 3);
+  c.take<float>((size_t)B * n_joints * 12);
+  c.take<float>((size_t)B * (n_joints - 1) * 9);
+  *bytes = c.used();
+  return 0;
+}
+
+int avc_smpl_pose_batch_bwd(const float* v_template, const float* J_regressor, const int32_t* parents,
+                            const float* posedirs, const float* lbs_weights, int32_t V, int32_t n_joints,
+                            const float* body_pose, int32_t pose_dim, int32_t B, const float* global_orient,
+                            const float* post_rot, const float* g_verts, float* g_body_pose, void* workspace,
+                            size_t workspace_bytes, avc_stream_t stream) {
+  if (!v_template || !J_regressor || !parents || !posedirs || !lbs_weights || !body_pose || !global_orient ||
+      !g_verts || !g_body_pose || !workspace)
+    return AVC_E_NULL;
+  size_t need = 0;
+  AVC_TRY(avc_smpl_pose_batch_bwd_workspace_bytes(B, V, n_joints, &need));
+  if (pose_dim < 1 || pose_dim > (n_joints - 1) * 3 || workspace_bytes < need) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int NF = (n_joints - 1) * 9;
+  Carver c(workspace);
+  float* J = c.take<float>((size_t)n_joints * 3);
+  float* A = c.take<float>((size_t)B * n_joints * 12);
+  float* feat = c.take<float>((size_t)B * NF);
+  float* p = c.take<float>((size_t)B * V * 3);
+  float* go = c.take<float>((size_t)B * V * 3);
+  float* gp = c.take<float>((size_t)B * V * 3);
+  float* dA = c.take<float>((size_t)B * n_joints * 12);
+  float* gfeat = c.take<float>((size_t)B * NF);
+  Orient o{{global_orient[0], global_orient[1], global_orient[2]}};
+  PostRot pr{};
+  pr.on = post_rot != nullptr;
+  if (post_rot)
+    for (int i = 0; i < 9; ++i) pr.m[i] = post_rot[i];
+  k_pose_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, J);
+  k_pose_chain<<<(B + 3) / 4, 128, 0, st>>>(body_pose, pose_dim, B, o, J, parents, n_joints, A, feat);
+  const unsigned rows = (unsigned)((B + kSkinRows - 1) / kSkinRows);
+  k_pose_skin_bwd<<<dim3((V + 127) / 128, rows), 128, 0, st>>>(v_template, posedirs, feat, A, lbs_weights, V, n_joints,
+                                                               NF, B, pr, g_verts, p, go, gp);
+  k_pose_dA<<<dim3(n_joints, B), 256, 0, st>>>(lbs_weights, p, go, V, n_joints, dA);
+  k_pose_gfeat<<<dim3(NF, rows), 256, 0, st>>>(posedirs, gp, V * 3, NF, B, gfeat);
+  k_pose_chain_bwd<<<(B + 3) / 4, 128, 0, st>>>(body_pose, pose_dim, B, J, parents, n_joints, A, feat, dA, gfeat,
+                                                g_body_pose);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_clip_prep_nearest_bwd(const float* g_out, int32_t B, int32_t n, int32_t out_size, float* g_images,
+                              avc_stream_t stream) {
+  if (!g_out || !g_images) return AVC_E_NULL;
+  if (B < 1 || n < 1 || out_size < 1) return AVC_E_SIZE;
+  const long long total = (long long)B * n * n;
+  k_clip_prep_nearest_bwd<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(g_out, B, n, out_size,
+                                                                                              g_images);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_pose_clip_loss(const float* emb, int32_t A, int32_t B, int32_t dim, const float* text, float* loss_out,
+                       float* g_emb, avc_stream_t stream) {
+  if (!emb || !text || !g_emb) return AVC_E_NULL;
+  if (A < 1 || B < 1 || dim < 1) return AVC_E_SIZE;
+  k_pose_clip_loss<<<B, 128, 0, (cudaStream_t)stream>>>(emb, A, B, dim, text, loss_out, g_emb);
   AVC_LAUNCH_TRY();
   return 0;
 }

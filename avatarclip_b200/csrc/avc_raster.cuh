@@ -75,6 +75,59 @@ __global__ void k_project_look_at(const float* __restrict__ v, int V, LookAtCam 
   project_look_at(i, v, c, proj);
 }
 
+// the supersample (row, xi) won by face f at depth zp: the unlit trilinear sample col of f's R^3 cube at the
+// perspective-corrected barycentrics, and f's light
+__device__ __forceinline__ void textured_sample(int row, int xi, int f, float zp, const int* __restrict__ faces,
+                                                const float* __restrict__ verts, const float4* __restrict__ proj,
+                                                const float* __restrict__ tex, int R, const LookAtCam& c, float* col,
+                                                float* light_out) {
+  const int is = c.is;
+  const int i0 = faces[f * 3], i1 = faces[f * 3 + 1], i2 = faces[f * 3 + 2];
+  // lighting in the world frame: n = normalize((v0 - v1) x (v2 - v1)), the copy facing the eye is the one drawn
+  const float* v0 = verts + 3 * i0;
+  const float* v1 = verts + 3 * i1;
+  const float* v2 = verts + 3 * i2;
+  float a[3] = {v0[0] - v1[0], v0[1] - v1[1], v0[2] - v1[2]}, b[3] = {v2[0] - v1[0], v2[1] - v1[1], v2[2] - v1[2]};
+  float nx = a[1] * b[2] - a[2] * b[1], ny = a[2] * b[0] - a[0] * b[2], nz = a[0] * b[1] - a[1] * b[0];
+  float nl = fmaxf(sqrtf(nx * nx + ny * ny + nz * nz), 1e-5f);
+  float s = (nx * (c.eye[0] - v1[0]) + ny * (c.eye[1] - v1[1]) + nz * (c.eye[2] - v1[2])) >= 0.f ? 1.f : -1.f;
+  const float light = 0.5f + 0.5f * fmaxf(s * ny / nl, 0.f);
+  // screen barycentrics at the supersample centre, then w_k (R - 1) z_pixel / z_k
+  const float4 pa = proj[i0], pb = proj[i1], pc = proj[i2];
+  const int yi = is - 1 - row;
+  const float xp = (2.f * xi + 1.f - is) / is, yp = (2.f * yi + 1.f - is) / is;
+  const float det = (pb.y - pc.y) * (pa.x - pc.x) + (pc.x - pb.x) * (pa.y - pc.y);
+  const float w0 = ((pb.y - pc.y) * (xp - pc.x) + (pc.x - pb.x) * (yp - pc.y)) / det;
+  const float w1 = ((pc.y - pa.y) * (xp - pc.x) + (pa.x - pc.x) * (yp - pc.y)) / det;
+  const float w2 = 1.f - w0 - w1;
+  const float wz[3] = {w0 * zp / pa.z, w1 * zp / pb.z, w2 * zp / pc.z};
+  float ti[3];
+  int tb[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    ti[k] = fminf(fmaxf(wz[k] * (R - 1), 0.f), (float)(R - 1) - 1e-5f);
+    tb[k] = (int)ti[k];
+    ti[k] -= (float)tb[k];
+  }
+  const float* cube = tex + (size_t)f * R * R * R * 3;
+  col[0] = 0.f; col[1] = 0.f; col[2] = 0.f;
+#pragma unroll
+  for (int corner = 0; corner < 8; ++corner) {
+    float w = 1.f;
+    int idx = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const int hi = (corner >> k) & 1;
+      w *= hi ? ti[k] : 1.f - ti[k];
+      idx = idx * R + min(tb[k] + hi, R - 1);
+    }
+    col[0] += w * cube[idx * 3];
+    col[1] += w * cube[idx * 3 + 1];
+    col[2] += w * cube[idx * 3 + 2];
+  }
+  *light_out = light;
+}
+
 // resolve pixel p: per supersample the winning face's colour -- trilinear sample of its R^3 cube at the perspective-
 // corrected barycentrics, times the face's light -- then the ss x ss average.  No flip (neural_renderer's image).
 __device__ __forceinline__ void resolve_textured(int p, const unsigned long long* __restrict__ zbuf,
@@ -91,49 +144,8 @@ __device__ __forceinline__ void resolve_textured(int p, const unsigned long long
       if (zb == ~0ull) continue;
       const int f = (int)(zb & 0xffffffffu);
       const float zp = __uint_as_float((unsigned)(zb >> 32));
-      const int i0 = faces[f * 3], i1 = faces[f * 3 + 1], i2 = faces[f * 3 + 2];
-      // lighting in the world frame: n = normalize((v0 - v1) x (v2 - v1)), the copy facing the eye is the one drawn
-      const float* v0 = verts + 3 * i0;
-      const float* v1 = verts + 3 * i1;
-      const float* v2 = verts + 3 * i2;
-      float a[3] = {v0[0] - v1[0], v0[1] - v1[1], v0[2] - v1[2]}, b[3] = {v2[0] - v1[0], v2[1] - v1[1], v2[2] - v1[2]};
-      float nx = a[1] * b[2] - a[2] * b[1], ny = a[2] * b[0] - a[0] * b[2], nz = a[0] * b[1] - a[1] * b[0];
-      float nl = fmaxf(sqrtf(nx * nx + ny * ny + nz * nz), 1e-5f);
-      float s = (nx * (c.eye[0] - v1[0]) + ny * (c.eye[1] - v1[1]) + nz * (c.eye[2] - v1[2])) >= 0.f ? 1.f : -1.f;
-      const float light = 0.5f + 0.5f * fmaxf(s * ny / nl, 0.f);
-      // screen barycentrics at the supersample centre, then w_k (R - 1) z_pixel / z_k
-      const float4 pa = proj[i0], pb = proj[i1], pc = proj[i2];
-      const int yi = is - 1 - row;
-      const float xp = (2.f * xi + 1.f - is) / is, yp = (2.f * yi + 1.f - is) / is;
-      const float det = (pb.y - pc.y) * (pa.x - pc.x) + (pc.x - pb.x) * (pa.y - pc.y);
-      const float w0 = ((pb.y - pc.y) * (xp - pc.x) + (pc.x - pb.x) * (yp - pc.y)) / det;
-      const float w1 = ((pc.y - pa.y) * (xp - pc.x) + (pa.x - pc.x) * (yp - pc.y)) / det;
-      const float w2 = 1.f - w0 - w1;
-      const float wz[3] = {w0 * zp / pa.z, w1 * zp / pb.z, w2 * zp / pc.z};
-      float ti[3];
-      int tb[3];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        ti[k] = fminf(fmaxf(wz[k] * (R - 1), 0.f), (float)(R - 1) - 1e-5f);
-        tb[k] = (int)ti[k];
-        ti[k] -= (float)tb[k];
-      }
-      const float* cube = tex + (size_t)f * R * R * R * 3;
-      float col[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-      for (int corner = 0; corner < 8; ++corner) {
-        float w = 1.f;
-        int idx = 0;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const int hi = (corner >> k) & 1;
-          w *= hi ? ti[k] : 1.f - ti[k];
-          idx = idx * R + min(tb[k] + hi, R - 1);
-        }
-        col[0] += w * cube[idx * 3];
-        col[1] += w * cube[idx * 3 + 1];
-        col[2] += w * cube[idx * 3 + 2];
-      }
+      float col[3], light;
+      textured_sample(row, xi, f, zp, faces, verts, proj, tex, R, c, col, &light);
       acc[0] += col[0] * light;
       acc[1] += col[1] * light;
       acc[2] += col[2] * light;

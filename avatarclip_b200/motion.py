@@ -7,8 +7,8 @@ Two generators of models/motion_generation.py run here:
     anchor frames by the reference's sequential fp32 accumulation, decoded by ``avc_vposer_decode``;
   * ``MotionOptimizer`` (:249-358) with ``clip_coef = 0``: the motion VAE decoder's latent optimised by Adam against
     the reconstruction (and delta) loss, ``avc_motion_optimize``.
-A ``MotionOptimizer`` with ``clip_coef > 0`` is refused: its CLIP term needs the textured rasteriser's gradient, which
-this project does not have.  So are the pose generators ``animate`` refuses, and any optimiser other than Adam.
+A ``MotionOptimizer`` with ``clip_coef > 0`` is refused: its CLIP term (one camera at 150 degrees on every 30th frame)
+is not built.  So are the pose generators ``animate`` refuses, and any optimiser other than Adam.
 
     python -m avatarclip_b200.motion --conf confs/motion_ablation/baseline/walk.conf --smpl smpl.npz \\
         --clip_model ViT-B-32.pt --bpe bpe_simple_vocab_16e6.txt.gz
@@ -290,29 +290,37 @@ class MotionOptimizer:
         return pose_padding(motion)
 
 
+def adam_refusal(mg: Mapping, who: str, default_cfg: Mapping) -> Optional[str]:
+    """Why the optimiser settings (optim_name, optim_cfg) of ``who``'s conf block cannot run here, or None: only plain
+    torch.optim.Adam runs (avc_adam_step_dev)."""
+    name = mg.get("optim_name", "Adam")
+    if name != "Adam":
+        return f"{who} optim_name = {name} is not available: only Adam runs"
+    cfg = dict(mg.get("optim_cfg", default_cfg))
+    bad = sorted(set(cfg) - set(ADAM_KEYS))
+    if bad:
+        return f"{who} optim_cfg keys {bad} are not Adam's"
+    if cfg.get("weight_decay", 0) or cfg.get("amsgrad", False) or cfg.get("maximize", False):
+        return f"{who} optim_cfg: weight_decay, amsgrad and maximize are not available (plain Adam runs)"
+    return None
+
+
 def optimizer_refusal(mg: Mapping) -> Optional[str]:
     """Why a MotionOptimizer block cannot run here, or None."""
     clip_coef = float(mg.get("clip_coef", OPTIMIZER_DEFAULTS["clip_coef"]))
     if clip_coef > 0:
-        return (f"MotionOptimizer with clip_coef = {clip_coef} is not available: its CLIP term needs the rasteriser's "
-                "gradient, which this project's textured rasteriser does not have (clip_coef = 0 runs)")
-    name = mg.get("optim_name", "Adam")
-    if name != "Adam":
-        return f"MotionOptimizer optim_name = {name} is not available: only Adam runs"
-    cfg = dict(mg.get("optim_cfg", OPTIMIZER_DEFAULTS["optim_cfg"]))
-    bad = sorted(set(cfg) - set(ADAM_KEYS))
-    if bad:
-        return f"MotionOptimizer optim_cfg keys {bad} are not Adam's"
-    if cfg.get("weight_decay", 0) or cfg.get("amsgrad", False) or cfg.get("maximize", False):
-        return "MotionOptimizer optim_cfg: weight_decay, amsgrad and maximize are not available (plain Adam runs)"
-    return None
+        return (f"MotionOptimizer with clip_coef = {clip_coef} is not available: its CLIP term is not built (the "
+                "rasteriser's gradient exists, python -m avatarclip_b200.pose_optimizer uses it, but the term's "
+                "backward into the motion latent does not; clip_coef = 0 runs)")
+    return adam_refusal(mg, "MotionOptimizer", OPTIMIZER_DEFAULTS["optim_cfg"])
 
 
 def refusal(conf) -> Optional[str]:
     """Why ``conf`` cannot run as a motion, or None."""
     mode = conf.get_string("general.mode", "pose")
     if mode != "motion":
-        return f"general.mode = {mode}: this command runs the motion stage; run python -m avatarclip_b200.animate"
+        return (f"general.mode = {mode}: this command runs the motion stage; run python -m avatarclip_b200.animate "
+                "(PoseOptimizer confs: python -m avatarclip_b200.pose_optimizer)")
     why = animate.pose_generator_refusal(conf)
     if why:
         return why

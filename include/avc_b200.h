@@ -690,6 +690,65 @@ int avc_pose_suppress(const float* poses, int32_t P, int32_t dim, float threshol
 int avc_pose_score(const float* emb, int32_t A, int32_t B, int32_t dim, const float* text, int32_t group,
                    float* score_out, int32_t* best_out, void* workspace, size_t workspace_bytes, avc_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * AvatarAnimate's PoseOptimizer (models/pose_generation.py:102-135): the gradient of the CLIP loss with respect to
+ * the body pose, pose -> SMPL vertices -> textured render -> nearest resize -> CLIP image tower -> cosine.  All fp32.
+ *
+ * avc_look_at_cams writes the cameras of n eyes (HOST [n][3], at / up HOST [3]) for images of image_size x
+ * supersample pixels into cams_out (DEVICE, n avc_look_at_cam_bytes bytes), as avc_raster_textured_batch makes them.
+ * avc_raster_textured_batch_dev is avc_raster_textured_batch with those cameras read from DEVICE memory (cams:
+ * [ceil(B / group)][A] records), so that it can be captured in a CUDA graph and replayed with new cameras; same
+ * workspace, same images bit for bit.
+ *
+ * avc_raster_textured_batch_bwd: g_verts [B][V][3] = d loss / d verts (the vertices as given to the forward) from
+ * g_rgb [A][B][n][n][3], restating neural_renderer's backward (Kato et al. 2018) per image:
+ *   (a) light: per face, d light = sum over its supersamples of g_rgb / ss^2 . the unlit trilinear sample, through
+ *       light = 0.5 + 0.5 relu(s n_y / max(|n|, 1e-5)), n = (v0 - v1) x (v2 - v1) (relu's gradient 0 at <= 0);
+ *   (b) backward_pixel_map on the supersampled colour map (background 0, face index -1) of the drawn copy of each
+ *       face (the face as given when it faces the camera, else fill_back's (v2, v1, v0)), eps 1e-4; an edge whose
+ *       end points share the swept coordinate contributes nothing (neural_renderer divides 0 by 0 there);
+ *   (c) the screen gradient through x' = x_c / (z_c tan 30), y' likewise, and look_at's rotation (no depth term).
+ * Per-face contributions are gathered to vertices over offsets / vf (avc_video_adjacency of faces) in a fixed order
+ * over the angles and the faces: no float atomics, so the result is bitwise reproducible.  fwd_workspace is the
+ * workspace the forward (either entry point) just used with the same arguments (it holds the cameras, projections
+ * and z-buffers).  Workspace: avc_raster_textured_batch_bwd_workspace_bytes(F, A B, n, supersample), about
+ * A B (16 (n ss)^2 + 36 F) bytes.
+ *
+ * avc_smpl_pose_batch_bwd: g_body_pose [B][pose_dim] = the reverse-mode derivative of avc_smpl_pose_batch (same
+ * arguments) given g_verts [B][V][3]; global_orient gets none.  pose_dim >= 1.  Workspace:
+ * avc_smpl_pose_batch_bwd_workspace_bytes(B, V, n_joints).  Deterministic (fixed-order reductions).
+ * avc_clip_prep_nearest_bwd: g_images [B][n][n][3] from g_out [B][3][S][S] of avc_clip_prep_nearest: each source
+ * pixel sums, in row-major order, g_out / std over the output pixels that read it (zero when none do).
+ * avc_pose_clip_loss: loss_out[b] = 1 - F.cosine_similarity(mean_a emb[a][b], text) (eps 1e-8, computed as
+ * avc_pose_score does; loss_out may be NULL) and g_emb [A][B][dim] = d loss_out[b] / d emb[a][b]: each row's
+ * gradient is that of its own loss.
+ * ------------------------------------------------------------------------------------------ */
+int avc_look_at_cam_bytes(size_t* bytes);
+int avc_look_at_cams(const float* eyes, int32_t n, const float* at, const float* up, int32_t image_size,
+                     int32_t supersample, void* cams_out, avc_stream_t stream);
+int avc_raster_textured_batch_dev(const float* verts, int32_t B, int32_t group, const int32_t* faces,
+                                  const float* textures, int32_t V, int32_t F, int32_t R, const void* cams, int32_t A,
+                                  int32_t image_size, int32_t supersample, float* rgb_out, void* workspace,
+                                  size_t workspace_bytes, avc_stream_t stream);
+int avc_raster_textured_batch_bwd_workspace_bytes(int32_t F, int32_t n_images, int32_t image_size,
+                                                  int32_t supersample, size_t* bytes);
+int avc_raster_textured_batch_bwd(const float* verts, int32_t B, int32_t group, const int32_t* faces,
+                                  const float* textures, int32_t V, int32_t F, int32_t R, int32_t A,
+                                  int32_t image_size, int32_t supersample, const int32_t* offsets, const int32_t* vf,
+                                  const float* g_rgb, float* g_verts, const void* fwd_workspace,
+                                  size_t fwd_workspace_bytes, void* workspace, size_t workspace_bytes,
+                                  avc_stream_t stream);
+int avc_smpl_pose_batch_bwd_workspace_bytes(int32_t B, int32_t V, int32_t n_joints, size_t* bytes);
+int avc_smpl_pose_batch_bwd(const float* v_template, const float* J_regressor, const int32_t* parents,
+                            const float* posedirs, const float* lbs_weights, int32_t V, int32_t n_joints,
+                            const float* body_pose, int32_t pose_dim, int32_t B, const float* global_orient,
+                            const float* post_rot, const float* g_verts, float* g_body_pose, void* workspace,
+                            size_t workspace_bytes, avc_stream_t stream);
+int avc_clip_prep_nearest_bwd(const float* g_out, int32_t B, int32_t n, int32_t out_size, float* g_images,
+                              avc_stream_t stream);
+int avc_pose_clip_loss(const float* emb, int32_t A, int32_t B, int32_t dim, const float* text, float* loss_out,
+                       float* g_emb, avc_stream_t stream);
+
 /* avc_vposer_encode is VPoser 2.x encode(x).mean in eval mode: encoder_net = BatchNorm1d(n_in) (running statistics,
  * eps 1e-5), Linear(n_in, hidden) W1, LeakyReLU(0.01), BatchNorm1d(hidden), Dropout (identity), Linear W2 [hidden]
  * [hidden], Linear W3 [hidden][hidden], then the NormalDistDecoder's mu head Wmu [latent][hidden].  Each batch norm
