@@ -41,7 +41,8 @@ struct Args {
   int64_t P;
 };
 
-// true when the fused kernel covers this network shape (hidden widths <= 256 and multiples of 16, L <= kMaxHidden)
+// true when the fused kernel covers this network shape: 1 <= L <= kMaxHidden; every hidden linear has 1 <= N, K <= 256
+// and ldw % 8 == 0; the widths chain (N_l + next_skip_cols_l = K_{l+1}, N_{L-1} + head_skip_cols = K_head); ld0 % 8 == 0
 bool supported(const Args& a);
 int launch(const Args& a, cudaStream_t st);
 

@@ -305,11 +305,12 @@ int assemble_sdf_feat(const NeusPlan& pl, const float* sdf, const float* feat, i
 // Leaves in[L] ready; writes sdf[Pn] (thin) and, when want_feat, feat[Pn][Fp].
 // wgmma engine, no stash, no features (sample placement, sdf queries): the whole chain of a 128-point tile in ONE
 // kernel (avc_chain.cu), activations resident in shared memory.  Returns 1 when the fused kernel does not cover this
-// network shape (the caller then runs the layer-by-layer launches), 0 on success.
+// network shape (the caller then runs the layer-by-layer launches), 0 on success.  The in0 and skip pairs are read at
+// their own pitch (Split16::ld): the render's separate [P][Kp] halves, or one [P][2 Kp] buffer (kind 27 of
+// avc_neus_kernel_test).
 int value_chain_fused(const NeusPlan& pl, const NeusWs& w, int64_t Pn, float* sdf_out, cudaStream_t st, int sdf_nz,
                       int sdf_pitch) {
-  const char* env = getenv("AVC_FUSED_CHAIN");      // 0: layer-by-layer launches (A-B knob, read on every call)
-  if ((env && atoi(env) == 0) || pl.L > chain::kMaxHidden) return 1;
+  if (pl.L > chain::kMaxHidden) return 1;
   chain::Args a;
   memset(&a, 0, sizeof(a));
   a.L = pl.L;
@@ -325,9 +326,9 @@ int value_chain_fused(const NeusPlan& pl, const NeusWs& w, int64_t Pn, float* sd
     y.oscale = pl.sdf[l + 1].skip ? kSqrtHalf : 1.f;
     y.next_skip_cols = (l + 1 < pl.L && pl.sdf[l + 1].skip) ? pl.E : 0;
   }
-  a.a0_hi = w.in16[0].hi; a.a0_lo = w.in16[0].lo; a.ld0 = pl.sdf[0].Kp;
+  a.a0_hi = w.in16[0].hi; a.a0_lo = w.in16[0].lo; a.ld0 = w.in16[0].ld;
   if (ls >= 0) {
-    a.skip_hi = w.in16[ls].hi; a.skip_lo = w.in16[ls].lo; a.skip_ld = pl.sdf[ls].Kp; a.skip_col0 = pl.sdf[ls].K - pl.E;
+    a.skip_hi = w.in16[ls].hi; a.skip_lo = w.in16[ls].lo; a.skip_ld = w.in16[ls].ld; a.skip_col0 = pl.sdf[ls].K - pl.E;
   }
   a.w_sdf = w.pack + pl.pk_wsdf; a.b_sdf = w.pack + pl.pk_bsdf; a.K_head = pl.sdf[pl.L].K;
   a.head_skip_cols = pl.sdf[pl.L].skip ? pl.E : 0;
@@ -339,7 +340,8 @@ int value_chain_fused(const NeusPlan& pl, const NeusWs& w, int64_t Pn, float* sd
 
 int value_chain(const NeusPlan& pl, const NeusWs& w, int64_t Pn, bool stash, bool want_feat, float* sdf_out,
                 cudaStream_t st, int sdf_nz = 0, int sdf_pitch = 0) {
-  if (pl.cfg.engine == 1 && !stash && !want_feat) {
+  const char* env = getenv("AVC_FUSED_CHAIN");      // 0: layer-by-layer launches (A-B knob, read on every call)
+  if (pl.cfg.engine == 1 && !stash && !want_feat && !(env && atoi(env) == 0)) {
     int r = value_chain_fused(pl, w, Pn, sdf_out, st, sdf_nz, sdf_pitch);
     if (r != 1) return r;
   }
@@ -983,7 +985,7 @@ int avc_neus_kernel_test(int32_t kind, const int64_t* d, const float* fs, const 
       return points_to_cin(F32(in[0]), d[0], O32(out[0]), st);
     }
   }
-  if (kind < 9 || kind > 26) return AVC_E_BADCFG;
+  if (kind < 9 || kind > 27) return AVC_E_BADCFG;
   if (kind >= 12 && kind <= 14) {
     // EncodeTargets: out[0] in0 or NULL, out[1..4] skip fp32 targets or NULL, out[5] the in0 pair, out[6..9] the skip
     // pairs (bf16 [P][2 ld]: hi in columns [0, ld), lo in [ld, 2 ld) of each row; NULL: none)
@@ -1058,6 +1060,25 @@ int avc_neus_kernel_test(int32_t kind, const int64_t* d, const float* fs, const 
       return fill_gebar(pl, l, F32(in[1]), d[0], O32(out[0]), pair(out[1], pl.sdf[l].Kp), st);
     }
     case 26: return assemble_sdf_feat(pl, F32(in[1]), F32(in[2]), d[0], O32(out[0]), st);
+    case 27: {
+      // the fused value chain alone, whatever AVC_FUSED_CHAIN says: AVC_E_BADCFG where it does not cover the network
+      const int nz = (int)d[1], pitch = (int)d[2];
+      if (nz < 0 || (nz > 0 && pitch < nz)) return AVC_E_SIZE;
+      if (pl.cfg.engine != 1) return AVC_E_BADCFG;
+      if (!in[1] || !in[2] || !in[3] || !out[0]) return AVC_E_NULL;
+      NeusWs w;
+      memset(&w, 0, sizeof(w));
+      w.pack = const_cast<float*>(F32(in[1]));
+      w.pk_hi = (__nv_bfloat16*)const_cast<void*>(in[2]); w.pk_lo = w.pk_hi + pl.pack_floats;
+      w.in16[0] = pair(const_cast<void*>(in[3]), pl.sdf[0].Kp);
+      for (int l = 1; l <= pl.L; ++l) {
+        if (!pl.sdf[l].skip) continue;
+        if (!in[4]) return AVC_E_NULL;
+        w.in16[l] = pair(const_cast<void*>(in[4]), pl.sdf[l].Kp);
+      }
+      const int r = value_chain_fused(pl, w, d[0], O32(out[0]), st, nz, pitch);
+      return r == 1 ? AVC_E_BADCFG : r;
+    }
   }
   return AVC_E_BADCFG;
 }

@@ -473,7 +473,7 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
  *   8 k_merge          dims {n (<= 256), pitch, Rc, per (<= 64), pitch_o >= n + per};  in {z[Rc][pitch], sdf[Rc][pitch],
  *     newz[Rc][per], news[Rc][per] or NULL};  out {zo[Rc][pitch_o], so[Rc][pitch_o] (unused when news is NULL)}
  * A "pair" output is the two-term bf16 split of a [rows][ld] activation as ONE bf16 buffer [rows][2 ld]: hi in columns
- * [0, ld), lo in [ld, 2 ld) of each row; NULL where the render passes no split.  Kinds 9..11, 15..17, 20..24 and 26 run
+ * [0, ld), lo in [ld, 2 ld) of each row; NULL where the render passes no split.  Kinds 9..11, 15..17, 20..24, 26 and 27 run
  * on a whole configuration: in[0] is a HOST avc_neus_cfg, the widths and pitches below are those of its plan (K_l, Kp_l,
  * Np_l of SDF linear l; E, EP the encoded width and its pitch; Hc, F), pack is what kind 10 writes.  dims[0] = P.
  *   9 pack layout       out {HOST int64 [16 + 11 (L + Lc + 3)]}: {L, Lc, E, EP, F, Fp, Hc, pack_floats, n_params,
@@ -497,7 +497,11 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
  *  23 k_dge             in {cfg, cin[P][8], nbar[P][4]};  out {ubar0[P][Kp_0] or NULL, gebar[P][EP], pair or NULL}
  *  24 k_fill_gebar      dims {P, l (a skip layer)};  in {cfg, gebar[P][EP]};  out {ubar_l[P][Kp_l], pair or NULL}
  *  25 k_points_to_cin   dims {P};  in {pts[P][3]};  out {cin[P][8]}
- *  26 k_assemble_sdf_feat  in {cfg, sdf[P], feat[P][Fp]};  out {[P][F + 1]} */
+ *  26 k_assemble_sdf_feat  in {cfg, sdf[P], feat[P][Fp]};  out {[P][F + 1]}
+ *  27 k_sdf_chain (the fused value chain, engine 1)  dims {P, nz, pitch};  in {cfg, pack[pack_floats], pk pair
+ *     [2 pack_floats] (hi, then lo), in0 pair [P][2 Kp_0], skip pair [P][2 Kp_ls] of the skip linear ls or NULL (no
+ *     skip)};  out {sdf ([P], or [P / nz][pitch] when nz > 0: point p at (p / nz) pitch + p % nz)}.  Always the fused
+ *     kernel (AVC_FUSED_CHAIN is not read): AVC_E_BADCFG where it does not cover the configuration */
 int avc_neus_kernel_test(int32_t kind, const int64_t* dims, const float* fscal, const void* const* in, void* const* out,
                          avc_stream_t stream);
 /* One kernel of the CLIP towers (avc_clip.cu) on caller buffers, launched by the host code the towers use (the GEMMs

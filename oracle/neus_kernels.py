@@ -1,5 +1,6 @@
 """float64 references of the NeuS kernels outside the GEMM tiles (avc_neus_kernels.cuh): compositing, scalars,
-placement, weight packing and its backward, the encoding, the thin contractions and the ends of the gradient chain.
+placement, weight packing and its backward, the encoding, the thin contractions and the ends of the gradient chain; and
+of the fused value-chain kernel (avc_chain.cu), which holds its own tiles.
 One function per kernel, taking the fp32 inputs the kernel reads.  They run on whatever device the inputs live on.
 
 The compositing forward is oracle.neus.composite itself; its backward is fp64 autograd through it, so the kernels'
@@ -311,9 +312,40 @@ def heads_dgrad(y6bar, W6, h, dtype=F64) -> torch.Tensor:
     return (y6bar[:, 0:6].to(dtype) @ W6[0:6].to(dtype)) * (h > 0).to(dtype)
 
 
-# --------------------------------------------------------------------------- gradient chain
+# --------------------------------------------------------------------------- value chain
 SQRT_HALF = 0.70710678118654752440
 
+
+def value_chain(x0, skip, weights, biases, w_sdf, b_sdf, skip_layer: Optional[int], scale: float, dtype=F64,
+                split_acts: bool = False, pre: Optional[list] = None) -> torch.Tensor:
+    """k_sdf_chain (avc_chain.cu) on its own inputs: the SDF value chain of models/fields.py:72-91 from the encoded
+    points to the sdf.  x0 [P, K_0] is the layer-0 input, skip [P, E] the skip linear's encoding columns as the kernel
+    reads them (already times sqrt(1/2)) or None, weights / biases the L hidden linears ([N_l, K_l], [N_l]), w_sdf [K_L]
+    and b_sdf the sdf row of the last linear, skip_layer the index (1..L) of the linear that takes cat([h, enc]) / sqrt(2)
+    or None.  Per hidden linear: z = h W^T + b, softplus with beta 100 and threshold 20, times sqrt(1/2) when the next
+    linear takes the skip concat, then the concat.  sdf = (h . w_sdf + b_sdf) / scale.
+    ``split_acts`` rounds every activation that feeds another hidden linear to fp32 and then to its two-term bf16 split
+    (split_bf16), as the kernel's epilogue stores it; the last hidden activation meets the head unsplit, as in the kernel.
+    ``pre`` (a list) receives each linear's pre-activation z."""
+    h = x0.to(dtype)
+    L = len(weights)
+    for l in range(L):
+        z = h @ weights[l].to(dtype).T + biases[l].to(dtype)
+        if pre is not None:
+            pre.append(z)
+        a = neus.softplus100(z)
+        if skip_layer == l + 1:
+            a = a * SQRT_HALF
+        if split_acts and l + 1 < L:
+            hi, lo = split_bf16(a.float())
+            a = hi.to(dtype) + lo.to(dtype)
+        if skip_layer == l + 1:
+            a = torch.cat([a, skip.to(dtype)], -1)
+        h = a
+    return (h @ w_sdf.to(dtype) + b_sdf.to(dtype).reshape(())) / scale
+
+
+# --------------------------------------------------------------------------- gradient chain
 
 def chain_start(wsdf, zprev, n_prev: int, K_last: int, skip_last: bool, E: int, dtype=F64):
     """k_chain_start: qt_{L-1} = sp'(z_{L-1}) * w_sdf[0:N_{L-1}] (times sqrt(1/2) when the last linear takes the skip

@@ -368,3 +368,32 @@ def test_gradient_chain_references_match_sdf_gradient(skip_in, multires, scale):
     got = nk.normal(ge, x, scale, multires)
     assert (got - want).abs().max().item() <= 1e-12 * max(1.0, want.abs().max().item())
 
+
+
+
+@pytest.mark.parametrize("H,L,skip_in,multires,scale", [(256, 4, (4,), 6, 1.0), (64, 8, (4,), 6, 1.0),
+                                                        (48, 1, (), 6, 1.0), (64, 10, (1,), 6, 1.0),
+                                                        (64, 3, (2,), 10, 2.5), (16, 3, (2,), 0, 0.5)])
+def test_value_chain_matches_sdf_value(H, L, skip_in, multires, scale):
+    """value_chain (k_sdf_chain) in fp64 on exact fp32 inputs -- points and parameters held in fp32, the encoding, the
+    effective weights and the skip columns (the encoding times sqrt(1/2)) computed from them -- equals sdf_value of the
+    fp64 network: the skip concat inside the chain, at the head, right after linear 0 (25 wide), one hidden linear, a
+    one-column linear (64 - 63), multires 0 and 10, scale != 1.  Splitting the stored activations moves it by less than
+    2^-14 of its largest entry (measured up to 8.4e-6); with one hidden linear nothing is split."""
+    conf = neus.SDFConf(d_in=3, d_out=9, d_hidden=H, n_layers=L, skip_in=skip_in, multires=multires, scale=scale)
+    g = torch.Generator().manual_seed(H + L)
+    p32 = {k: v + 0.05 * torch.randn(v.shape, generator=g) for k, v in neus.init_sdf_params(conf, g).items()}
+    p = {k: v.double() for k, v in p32.items()}
+    x = ((torch.rand(257, 3, generator=g) - 0.5) * 2).double()
+    want = neus.sdf_value(p, conf, x)[:, 0]
+    enc = neus.positional_encode(x * scale, multires)
+    W = [neus.effective_weight(p, f"lin{l}") for l in range(L + 1)]
+    b = [p[f"lin{l}.bias"] for l in range(L + 1)]
+    ls = skip_in[0] if skip_in else None
+    args = (enc, enc * nk.SQRT_HALF if ls else None, W[:L], b[:L], W[L][0], b[L][0:1], ls, scale)
+    got = nk.value_chain(*args)
+    m = want.abs().max().item()
+    assert (got - want).abs().max().item() <= 1e-12 * m
+    d = (nk.value_chain(*args, split_acts=True) - got).abs().max().item() / m
+    print(f"split activations move the sdf by {d:.1e}")
+    assert (d > 0.0) == (L > 1) and d < 2.0 ** -14, d
