@@ -526,6 +526,60 @@ k_motion_loss(const float* __restrict__ out, int T, int n_out, const float* __re
   }
 }
 
+// ---------------------------------------------------------------- the CLIP term (:333-343)
+// Row r scores frame st + r P (P = clip_num_part, st = *st_idx) with weight clip_coef (st + r P) / T.  Rows past the
+// motion get weight 0 and frame st, so that every row renders a valid pose.  One thread per (row, pose column).
+__global__ void k_motion_clip_select(const float* __restrict__ motion, int T, int P, float clip_coef,
+                                     const int32_t* __restrict__ st_idx, int R, float* __restrict__ pose,
+                                     int32_t* __restrict__ frame, float* __restrict__ weight) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= R * kPose) return;
+  const int r = e / kPose, c = e - r * kPose, st = *st_idx, t = st + r * P;
+  const int f = t < T ? t : st;
+  pose[e] = motion[(size_t)f * kPose + c];
+  if (c == 0) {
+    frame[r] = f;
+    weight[r] = t < T ? clip_coef * ((float)t / (float)T) : 0.f;
+  }
+}
+
+// dout[frame[r]] += J^T (weight[r] g[r]) per joint, J = d rot6d_to_aa / d (the 6D output), by the forward-mode duals
+// k_motion_loss uses; loss_out[state[0]] += sum_r weight[r] loss[r].  Rows of weight 0 are skipped, and the rows of
+// non-zero weight score distinct frames, so each thread owns its 6 entries of dout.
+__global__ void k_motion_clip_grad(const float* __restrict__ out, int n_out, const int32_t* __restrict__ frame,
+                                   const float* __restrict__ weight, int R, const float* __restrict__ g,
+                                   const float* __restrict__ loss, float* __restrict__ dout,
+                                   float* __restrict__ loss_out, const float* __restrict__ state) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e == 0 && loss_out) {
+    float s = 0.f;
+    bool any = false;
+    for (int r = 0; r < R; ++r)
+      if (weight[r] != 0.f) {
+        any = true;
+        s = fmaf(weight[r], loss[r], s);
+      }
+    if (any) loss_out[(int)state[0]] += s;
+  }
+  if (e >= R * kJoints) return;
+  const int r = e / kJoints, j = e - r * kJoints;
+  const float w = weight[r];
+  if (w == 0.f) return;
+  const size_t o = (size_t)frame[r] * n_out + (j + 1) * 6;
+  const float ga[3] = {w * g[r * kPose + j * 3], w * g[r * kPose + j * 3 + 1], w * g[r * kPose + j * 3 + 2]};
+#pragma unroll 1
+  for (int i = 0; i < 6; ++i) {
+    Dual xd[6], aa[3];
+#pragma unroll
+    for (int c = 0; c < 6; ++c) xd[c] = Dual{out[o + c], c == i ? 1.f : 0.f};
+    rot6d_to_aa(xd, aa);
+    float s = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s = fmaf(ga[c], aa[c].d, s);
+    dout[o + i] += s;
+  }
+}
+
 // ---------------------------------------------------------------- host side
 struct Dims {
   int D, L, H, F, T, O, dh;
@@ -774,6 +828,84 @@ done:
   if (ev_out) cudaEventDestroy(ev_out);
   if (st) cudaStreamDestroy(st);
   return rc;
+}
+
+int avc_motion_clip_init(const avc_motion_dims* dims, const float* params, const float* pe, const float* latent_init,
+                         float lr, void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!latent_init) return AVC_E_NULL;
+  Net n;
+  AVC_TRY(prepare(dims, params, pe, workspace, workspace_bytes, &n));
+  cudaStream_t st = (cudaStream_t)stream;
+  const float lr_state[4] = {0.f, lr, 0.f, 0.f};
+  AVC_CUDA_TRY(cudaMemcpyAsync(n.w.lat, latent_init, sizeof(float) * n.d.D, cudaMemcpyDeviceToDevice, st));
+  AVC_CUDA_TRY(cudaMemsetAsync(n.w.m1, 0, sizeof(float) * n.d.D, st));
+  AVC_CUDA_TRY(cudaMemsetAsync(n.w.m2, 0, sizeof(float) * n.d.D, st));
+  AVC_CUDA_TRY(cudaMemsetAsync(n.w.dout, 0, sizeof(float) * n.d.T * n.d.O, st));
+  AVC_CUDA_TRY(cudaMemcpyAsync(n.w.state, lr_state, sizeof(lr_state), cudaMemcpyHostToDevice, st));
+  self_attn_fwd(st, n, 0, pe);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_motion_clip_forward(const avc_motion_dims* dims, const float* params, const float* pe, float* motion_out,
+                            void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!motion_out) return AVC_E_NULL;
+  Net n;
+  AVC_TRY(prepare(dims, params, pe, workspace, workspace_bytes, &n));
+  cudaStream_t st = (cudaStream_t)stream;
+  forward(st, n);
+  k_motion_loss<<<1, 1024, 0, st>>>(n.w.out, n.d.T, n.d.O, nullptr, 0, Coef{}, 0.f, motion_out, nullptr, nullptr,
+                                    nullptr, nullptr);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_motion_clip_select(const float* motion, int32_t n_frames, int32_t clip_num_part, float clip_coef,
+                           const int32_t* st_idx, int32_t n_rows, float* pose_out, int32_t* frame_out,
+                           float* weight_out, avc_stream_t stream) {
+  if (!motion || !st_idx || !pose_out || !frame_out || !weight_out) return AVC_E_NULL;
+  if (n_frames < 1 || clip_num_part < 1 || clip_num_part > n_frames || n_rows < 1 || n_rows > kMaxT ||
+      !(clip_coef >= 0.f))
+    return AVC_E_BADCFG;
+  k_motion_clip_select<<<ceil_div(n_rows * kPose, 256), 256, 0, (cudaStream_t)stream>>>(
+      motion, n_frames, clip_num_part, clip_coef, st_idx, n_rows, pose_out, frame_out, weight_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_motion_clip_backward(const avc_motion_dims* dims, const float* params, const float* pe, const float* poses,
+                             int32_t n_poses, const float* recon_coef, float delta_coef, int32_t n_rows,
+                             const int32_t* frame, const float* weight, const float* pose_grad, const float* pose_loss,
+                             float beta1, float beta2, float eps, float* motion_out, float* loss_out, float* grad_out,
+                             void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!poses || !recon_coef || !frame || !weight || !pose_grad || !pose_loss || !motion_out) return AVC_E_NULL;
+  if (n_poses < 1 || n_poses > kMaxCand || n_rows < 1 || n_rows > kMaxT || !(delta_coef >= 0.f)) return AVC_E_BADCFG;
+  Net n;
+  AVC_TRY(prepare(dims, params, pe, workspace, workspace_bytes, &n));
+  Coef coef{};
+  for (int k = 0; k < n_poses; ++k) coef.c[k] = recon_coef[k];
+  cudaStream_t st = (cudaStream_t)stream;
+  k_motion_loss<<<1, 1024, 0, st>>>(n.w.out, n.d.T, n.d.O, poses, n_poses, coef, delta_coef, motion_out, n.w.g6,
+                                    n.w.dout, loss_out, n.w.state);
+  k_motion_clip_grad<<<ceil_div(n_rows * kJoints, 128), 128, 0, st>>>(n.w.out, n.d.O, frame, weight, n_rows,
+                                                                      pose_grad, pose_loss, n.w.dout, loss_out,
+                                                                      n.w.state);
+  backward(st, n);
+  if (grad_out)
+    AVC_CUDA_TRY(cudaMemcpyAsync(grad_out, n.w.grad, sizeof(float) * n.d.D, cudaMemcpyDeviceToDevice, st));
+  AVC_TRY(avc_adam_step_dev(n.w.lat, n.w.grad, n.w.m1, n.w.m2, n.d.D, n.w.state, beta1, beta2, eps, 1.f, st));
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_motion_clip_latent(const avc_motion_dims* dims, const float* params, const float* pe, float* latent_out,
+                           void* workspace, size_t workspace_bytes, avc_stream_t stream) {
+  if (!latent_out) return AVC_E_NULL;
+  Net n;
+  AVC_TRY(prepare(dims, params, pe, workspace, workspace_bytes, &n));
+  AVC_CUDA_TRY(cudaMemcpyAsync(latent_out, n.w.lat, sizeof(float) * n.d.D, cudaMemcpyDeviceToDevice,
+                               (cudaStream_t)stream));
+  return 0;
 }
 
 }  // extern "C"

@@ -8,7 +8,8 @@ Two generators of models/motion_generation.py run here:
   * ``MotionOptimizer`` (:249-358) with ``clip_coef = 0``: the motion VAE decoder's latent optimised by Adam against
     the reconstruction (and delta) loss, ``avc_motion_optimize``.
 A ``MotionOptimizer`` with ``clip_coef > 0`` is refused: its CLIP term (one camera at 150 degrees on every 30th frame)
-is not built.  So are the pose generators ``animate`` refuses, and any optimiser other than Adam.
+runs as its own command, ``python -m avatarclip_b200.motion_clip``.  So are the pose generators ``animate`` refuses,
+and any optimiser other than Adam.
 
     python -m avatarclip_b200.motion --conf confs/motion_ablation/baseline/walk.conf --smpl smpl.npz \\
         --clip_model ViT-B-32.pt --bpe bpe_simple_vocab_16e6.txt.gz
@@ -309,9 +310,9 @@ def optimizer_refusal(mg: Mapping) -> Optional[str]:
     """Why a MotionOptimizer block cannot run here, or None."""
     clip_coef = float(mg.get("clip_coef", OPTIMIZER_DEFAULTS["clip_coef"]))
     if clip_coef > 0:
-        return (f"MotionOptimizer with clip_coef = {clip_coef} is not available: its CLIP term is not built (the "
-                "rasteriser's gradient exists, python -m avatarclip_b200.pose_optimizer uses it, but the term's "
-                "backward into the motion latent does not; clip_coef = 0 runs)")
+        return (f"MotionOptimizer with clip_coef = {clip_coef} does not run on this command: its CLIP term needs the "
+                "rasteriser's gradient, so it runs as its own command, python -m avatarclip_b200.motion_clip "
+                "(clip_coef = 0 runs here)")
     return adam_refusal(mg, "MotionOptimizer", OPTIMIZER_DEFAULTS["optim_cfg"])
 
 

@@ -813,6 +813,43 @@ int avc_motion_optimize(const avc_motion_dims* dims, const float* params, const 
                         float* loss_out, float* grad_out, void* workspace, size_t workspace_bytes,
                         avc_stream_t stream);
 
+/* MotionOptimizer with its CLIP term (clip_coef > 0, :333-343), as entry points that a caller strings into one
+ * iteration around the pose stage's render-and-score chain, so that the whole iteration can be captured as a CUDA graph:
+ *
+ *   avc_motion_clip_forward -> avc_motion_clip_select -> (SMPL, textured render, CLIP tower, loss and their backward
+ *   on the selected rows) -> avc_motion_clip_backward
+ *
+ * All calls of one run share one workspace of avc_motion_workspace_bytes, which holds the latent, Adam's moments and
+ * counter between the calls.  Every pointer is DEVICE memory except recon_coef (HOST).
+ * avc_motion_clip_init: the latent := latent_init [latent], Adam's moments and step count := 0, Adam's lr := lr, and
+ *   layer 0's self-attention block (it reads only pe).  Call it once, before the iterations.
+ * avc_motion_clip_forward: decode the current latent -> motion_out [n_frames][63] (avc_motion_decode's path).
+ * avc_motion_clip_select: with st = *st_idx (0 <= st < clip_num_part), row r < n_rows scores frame st + r clip_num_part
+ *   with weight clip_coef (st + r clip_num_part) / n_frames; a row past the motion gets weight 0 and frame st.  Writes
+ *   pose_out [n_rows][63] (the frames' poses), frame_out [n_rows], weight_out [n_rows].  n_rows <= 64;
+ *   ceil(n_frames / clip_num_part) rows cover every st.
+ * avc_motion_clip_backward: avc_motion_optimize's loss (recon and delta) of the current latent, plus
+ *   sum_r weight[r] pose_loss[r], where pose_loss [n_rows] is each row's CLIP loss and pose_grad [n_rows][63] its
+ *   gradient with respect to the row's pose; then the gradient with respect to the latent and the Adam step.  The loss
+ *   goes to loss_out[step] (step = Adam's count before the call) when loss_out is not NULL, the latent gradient to
+ *   grad_out [latent] when it is not NULL, and the motion (the same values as the forward's) to motion_out.  Rows of
+ *   weight 0 contribute nothing, so with clip_coef = 0 every value is bitwise avc_motion_optimize's.
+ * avc_motion_clip_latent: the current latent -> latent_out [latent]. */
+int avc_motion_clip_init(const avc_motion_dims* dims, const float* params, const float* pe, const float* latent_init,
+                         float lr, void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_motion_clip_forward(const avc_motion_dims* dims, const float* params, const float* pe, float* motion_out,
+                            void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_motion_clip_select(const float* motion, int32_t n_frames, int32_t clip_num_part, float clip_coef,
+                           const int32_t* st_idx, int32_t n_rows, float* pose_out, int32_t* frame_out,
+                           float* weight_out, avc_stream_t stream);
+int avc_motion_clip_backward(const avc_motion_dims* dims, const float* params, const float* pe, const float* poses,
+                             int32_t n_poses, const float* recon_coef, float delta_coef, int32_t n_rows,
+                             const int32_t* frame, const float* weight, const float* pose_grad, const float* pose_loss,
+                             float beta1, float beta2, float eps, float* motion_out, float* loss_out, float* grad_out,
+                             void* workspace, size_t workspace_bytes, avc_stream_t stream);
+int avc_motion_clip_latent(const avc_motion_dims* dims, const float* params, const float* pe, float* latent_out,
+                           void* workspace, size_t workspace_bytes, avc_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Video frames of a generated avatar (avatarclip_b200/video.py): one vertex-coloured mesh, smooth-shaded, over many
  * frames per launch.  The reference has no renderer for its results (render_novel_image / interpolate_view cannot
