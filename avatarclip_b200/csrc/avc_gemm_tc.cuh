@@ -832,6 +832,13 @@ gemm_tc_nt_kernel(const __grid_constant__ CUtensorMap mapAhi, const __grid_const
   })
 }
 
+// 1: the last NT launch of this host thread stored its outputs through the ring, 0: from registers (read by the tests)
+inline thread_local int g_nt_last_ring = -1;
+// Test hooks (avc_tc_nt_set_max_ctas, avc_tc_nt_last_grid): a cap on the persistent grid of this host thread's NT
+// launches (0: none), so that a small launch walks many row tiles per CTA, and the grid of its last NT launch (-1: none)
+inline thread_local int g_nt_max_ctas = 0;
+inline thread_local int g_nt_last_grid = -1;
+
 template <int BN, int NPROD, bool RESB, typename Epi, bool RING>
 static inline int launch_gemm_tc_nt_kern(cudaStream_t st, int64_t M, int N, int K, const CUtensorMap (&mab)[4],
                                          const Epi& epi, bool b_const, const EpiMaps<EpiStage<Epi>::kN>& emaps,
@@ -854,15 +861,17 @@ static inline int launch_gemm_tc_nt_kern(cudaStream_t st, int64_t M, int N, int 
   int g = ntiles < num_sms ? ntiles : num_sms;         // persistent: at most one CTA per SM ...
   g = (g / tiles_n) * tiles_n;                         // ... and a whole number of CTAs per column tile
   if (g < tiles_n) return AVC_E_BADCFG;
+  if (g_nt_max_ctas > 0) {                             // the test cap, in whole CTAs per column tile, at least one
+    const int cap = g_nt_max_ctas / tiles_n > 1 ? g_nt_max_ctas / tiles_n * tiles_n : tiles_n;
+    g = cap < g ? cap : g;
+  }
+  g_nt_last_grid = g;
   dim3 grid(g);
   AVC_CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(kNtThreads), (size_t)Cfg::SMEM_BYTES, st, mab[0], mab[1], mab[2], mab[3],
                           (int)M, N, K, epi, b_const ? 1 : 0, emaps, omaps, omask));
   AVC_LAUNCH_TRY();
   return 0;
 }
-
-// 1: the last NT launch of this host thread stored its outputs through the ring, 0: from registers (read by the tests)
-inline thread_local int g_nt_last_ring = -1;
 
 template <int BN, int NPROD, bool RESB, typename Epi>
 static inline int launch_gemm_tc_nt_bn(cudaStream_t st, int64_t M, int N, int K, const SplitPtr& A, const SplitPtr& B,

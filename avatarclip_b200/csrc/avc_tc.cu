@@ -72,4 +72,15 @@ int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, i
 // registers, -1: none yet.
 int avc_tc_nt_last_ring(void) { return tc::g_nt_last_ring; }
 
+// Caps the persistent grid of the calling host thread's wgmma NT launches at n CTAs, rounded down to whole CTAs per
+// column tile and at least one per column tile (0: no cap); returns the previous cap.
+int avc_tc_nt_set_max_ctas(int32_t n) {
+  const int prev = tc::g_nt_max_ctas;
+  tc::g_nt_max_ctas = n > 0 ? n : 0;
+  return prev;
+}
+
+// gridDim.x of the calling host thread's last wgmma NT launch, -1: none yet.
+int avc_tc_nt_last_grid(void) { return tc::g_nt_last_grid; }
+
 }  // extern "C"

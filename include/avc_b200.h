@@ -442,6 +442,12 @@ int avc_tc_gemm_tn_test(const float* A, const float* B, int64_t P, int32_t N1, i
 /* 1: the last wgmma NT launch of the calling host thread stored its outputs with TMA bulk stores through the epilogue
  * ring, 0: from registers, -1: no launch yet (the tests check which path a shape takes). */
 int avc_tc_nt_last_ring(void);
+/* For tests only: cap the persistent grid of the calling host thread's wgmma NT launches at n CTAs, rounded down to a
+ * whole number of CTAs per column tile and never below one per column tile (0: no cap, the default), so that a small
+ * launch walks many row tiles per CTA; returns the previous cap.  The library itself never sets it. */
+int avc_tc_nt_set_max_ctas(int32_t n);
+/* gridDim.x of the calling host thread's last wgmma NT launch, -1: none yet (the tests check the placement they claim). */
+int avc_tc_nt_last_grid(void);
 /* The backward epilogue functors of the NeuS path through the NT tiles on caller data: kind 0 second-order sweep,
  * 1 / 2 value backward without / with the sdf term, 3 gradient chain, 4 ReLU-mask dgrad, 5 encoding-gradient
  * accumulation; and with the bf16 split of their output: 6 value chain, 7 feature bias, 8 colour lin0, 9 ReLU,

@@ -100,6 +100,13 @@ def _check_f32(OUT, M, N, ref):
 SHAPES = [(1000, 217, 256), (300, 64, 39), (4133, 256, 256), (129, 39, 256), (513, 128, 39)]
 
 
+def _chain_bwd_ref(D1, QT, acc, s):
+    """EpiChainBwd: (zbar, ubar_next) from the sp' stash D1 and qt read as its two-term split."""
+    M, N = acc.shape
+    d = D1.double()[:M, :N]
+    return BETA * (1.0 - d) * _split_value(QT[:M])[:, :N] * acc, d * acc * s
+
+
 def _chain_bwd_inputs(M, N, ldx):
     g = torch.Generator().manual_seed(1)
     return _stash(M, N, ldx, g), _stash(M, N, ldx, g, -1.0, 1.0)
@@ -116,9 +123,9 @@ def test_chain_bwd_split(M, N, K):
     s = math.sqrt(0.5)
     acc, ring = _run(12, M, N, K, ldx, D1, QT, s=s, OUT=Z, OUT2=U16, ld2=ld2)
     assert ring == 1
-    d = D1.double()[:, :N]
-    ez = _check_f32(Z, M, N, BETA * (1.0 - d) * _split_value(QT)[:, :N] * acc)
-    eu = _check_split(U16, before, M, N, ldx, ld2, d * acc * s)
+    z_ref, u_ref = _chain_bwd_ref(D1, QT, acc, s)
+    ez = _check_f32(Z, M, N, z_ref)
+    eu = _check_split(U16, before, M, N, ldx, ld2, u_ref)
     print(M, N, K, "zbar", ez, "ubar split", eu)
 
 
@@ -131,9 +138,9 @@ def test_chain_bwd_f32(M, N, K):
     s = math.sqrt(0.5)
     acc, ring = _run(0, M, N, K, ldx, D1, QT, s=s, OUT=Z, OUT2=U, ld2=ldx)
     assert ring == 1
-    d = D1.double()[:, :N]
-    ez = _check_f32(Z, M, N, BETA * (1.0 - d) * _split_value(QT)[:, :N] * acc)
-    eu = _check_f32(U, M, N, d * acc * s)
+    z_ref, u_ref = _chain_bwd_ref(D1, QT, acc, s)
+    ez = _check_f32(Z, M, N, z_ref)
+    eu = _check_f32(U, M, N, u_ref)
     print(M, N, K, "zbar", ez, "ubar", eu)
 
 
@@ -150,8 +157,9 @@ def _dgrad_inputs(M, N, ldx, sdf):
 
 
 def _dgrad_ref(D1, ZB, acc, sdfbar, wsdf, M, N, s, inv):
-    ab = acc + (sdfbar.double()[:, None] * inv * wsdf.double()[None, :N] if sdfbar is not None else 0.0)
-    return D1.double()[:, :N] * ab * s + ZB.double()[:M, :N]
+    """EpiDgrad: the new zbar_prev from the sp' stash D1, the old zbar_prev ZB and the sdf term (sdfbar None: none)."""
+    ab = acc + (sdfbar.double()[:M, None] * inv * wsdf.double()[None, :N] if sdfbar is not None else 0.0)
+    return D1.double()[:M, :N] * ab * s + ZB.double()[:M, :N]
 
 
 @pytest.mark.parametrize("sdf", [False, True])
@@ -193,6 +201,12 @@ def test_dgrad_in_place(M, N, K, sdf):
 CHAIN_SHAPES = [(1000, 217, 39, 256), (300, 64, 0, 39), (4133, 256, 0, 256), (129, 25, 39, 39)]
 
 
+def _chain_ref(D1, acc, Nv, s):
+    """EpiChain: qt_prev of the hidden columns < Nv, and what the columns >= Nv add to ge (u / sqrt(2))."""
+    M = acc.shape[0]
+    return D1.double()[:M, :Nv] * acc[:, :Nv] * s, acc[:, Nv:] * math.sqrt(0.5)
+
+
 def _chain_inputs(M, Nv, E):
     ldx = max(r8(Nv), r8(E))
     g = torch.Generator().manual_seed(3)
@@ -209,10 +223,11 @@ def test_chain_split(M, Nv, E, K):
     s = math.sqrt(0.5)
     acc, ring = _run(15, M, Nv + E, K, ldx, D1, s=s, OUT=GE, OUT2=Q16, ld2=ldx, Nv=Nv)
     assert ring == 1
-    eq = _check_split(Q16, before, M, Nv, ldx, ldx, D1.double()[:, :Nv] * acc[:, :Nv] * s)
+    qt_ref, dge = _chain_ref(D1, acc, Nv, s)
+    eq = _check_split(Q16, before, M, Nv, ldx, ldx, qt_ref)
     print(M, Nv, E, K, "qt_prev split", eq)
     if E:
-        ege = _err(GE[:M, :E], ge0[:M, :E].double() + acc[:, Nv:] * math.sqrt(0.5))
+        ege = _err(GE[:M, :E], ge0[:M, :E].double() + dge)
         print("ge", ege)
         assert ege < BAR
     assert torch.equal(GE[:M, E:], ge0[:M, E:]) and torch.equal(GE[M:], ge0[M:])
@@ -227,8 +242,9 @@ def test_chain_f32(M, Nv, E, K):
     s = math.sqrt(0.5)
     acc, ring = _run(3, M, Nv + E, K, ldx, D1, s=s, OUT=Q, OUT2=GE, ld2=ldx, Nv=Nv)
     assert ring == 1
-    eq = _check_f32(Q, M, Nv, D1.double()[:, :Nv] * acc[:, :Nv] * s)
+    qt_ref, dge = _chain_ref(D1, acc, Nv, s)
+    eq = _check_f32(Q, M, Nv, qt_ref)
     print(M, Nv, E, K, "qt_prev", eq)
     if E:
-        assert _err(GE[:M, :E], ge0[:M, :E].double() + acc[:, Nv:] * math.sqrt(0.5)) < BAR
+        assert _err(GE[:M, :E], ge0[:M, :E].double() + dge) < BAR
     assert torch.equal(GE[M:], ge0[M:])

@@ -55,14 +55,23 @@ def _ptr(t):
 
 def _sentinel_split(M, ld2):
     """[M + EXTRA][ld2] fp32 buffer holding bf16 pairs: known finite values everywhere (hi then lo halves of a row)."""
-    pat = (torch.arange((M + EXTRA) * 2 * ld2, dtype=torch.float32) % 97 - 48.0).bfloat16()
-    return pat.view(torch.float32).reshape(M + EXTRA, ld2).cuda()
+    pat = (torch.arange((M + EXTRA) * 2 * ld2, device="cuda") % 97 - 48).bfloat16()
+    return pat.view(torch.float32).reshape(M + EXTRA, ld2)
 
 
 def _split(x):
     hi = x.bfloat16()
     lo = (x - hi.float()).bfloat16()
     return hi.double(), lo.double()
+
+
+def _split_acc(A, B, nprod):
+    """The fp64 accumulator of the tiles (up to their fp32 sums): the hi product, or the three of the two-term split
+    (sp' = sigmoid(100 z) would turn the split's own ~1e-5 error into ~1e-4)."""
+    (ah, al), (bh, bl) = _split(A), _split(B)
+    if nprod == 1:
+        return ah @ bh.t()
+    return ah @ bh.t() + ah @ bl.t() + al @ bh.t()
 
 
 def _run(kind, M, N, K, ldx, ld2, X=None, Y=None, v1=None, v2=None, s=1.0, seed=0, OUT2=None):
@@ -82,13 +91,7 @@ def _run(kind, M, N, K, ldx, ld2, X=None, Y=None, v1=None, v2=None, s=1.0, seed=
     L.check(f(kind, A.data_ptr(), B.data_ptr(), M, N, K, 0, _ptr(X), _ptr(Y), ldx, _ptr(v1), _ptr(v2), s, 1.0,
               OUT.data_ptr(), OUT2.data_ptr(), ld2, ws.data_ptr(), ws.numel(), L.stream_ptr()), "avc_tc_epi_test")
     torch.cuda.synchronize()
-    ring = _last_ring()
-    (ah, al), (bh, bl) = _split(A), _split(B)
-    if kind >= 100:      # one product of the hi halves
-        return ah @ bh.t(), OUT, OUT2, before, ring
-    # the three products of the two-term split in fp64 (sp' = sigmoid(100 z) would turn the split's own ~1e-5 error
-    # into ~1e-4)
-    return ah @ bh.t() + ah @ bl.t() + al @ bh.t(), OUT, OUT2, before, ring
+    return _split_acc(A, B, 1 if kind >= 100 else 3), OUT, OUT2, before, _last_ring()
 
 
 def _err(got, ref):
@@ -124,6 +127,24 @@ def _softplus(z):
     return sp, d1
 
 
+def _value_ref(acc, bias, s):
+    """EpiValue: the scaled softplus of acc + bias and its sp' stash."""
+    sp, d1 = _softplus(acc + bias.double()[None, :])
+    return sp * s, d1
+
+
+def _color0_ref(acc, bias, cin, WxT):
+    """EpiColor0: relu(acc + bias + cin[:, :6] . WxT)."""
+    M, N = acc.shape
+    return torch.relu(acc + bias.double()[None, :] + cin.double()[:M, :6] @ WxT.double()[:, :N])
+
+
+def _relu_mask_ref(acc, H):
+    """EpiDgradRelu: acc where the bf16 hi half of the activation H is not zero."""
+    M, N = acc.shape
+    return acc * (H[:M, :N].bfloat16() != 0).double()
+
+
 # (M, N, K, ldx, ld2): ld2 = 256 at N = 217 is the skip-layer input, whose columns 217..255 hold the encoding
 VALUE_SHAPES = [(1000, 217, 256, 224, 256), (300, 64, 39, 64, 64), (4133, 256, 256, 256, 256), (129, 39, 256, 40, 40),
                 (513, 128, 39, 128, 136), (777, 200, 256, 224, 208), (700, 128, 320, 128, 128)]
@@ -141,8 +162,8 @@ def test_value(M, N, K, ldx, ld2):
     s = 0.7071067811865476
     acc, OUT, OUT2, before, ring = _run(6, M, N, K, ldx, ld2, Y=D1, v1=bias, s=s, seed=1)
     assert ring == int(ring_expected)
-    sp, d1 = _softplus(acc + bias.double()[None, :])
-    eo, ed = _err(OUT[:M, :N], sp * s), _err(D1[:M, :N], d1)
+    out_ref, d1_ref = _value_ref(acc, bias, s)
+    eo, ed = _err(OUT[:M, :N], out_ref), _err(D1[:M, :N], d1_ref)
     print(M, N, K, "ring", ring, "out", eo, "sp'", ed)
     # sp' = sigmoid(100 z) has a slope of up to 25 in z: the fp32 sums of z (~3e-6 off at K = 256) move it by up to ~1e-4
     assert eo < BAR and ed < BAR_D1
@@ -211,8 +232,7 @@ def test_color0(M, N, K, nprod):
     WxT = WxT.cuda()
     acc, OUT, OUT2, before, ring = _run(8 if nprod == 3 else 108, M, N, K, ldx, ldx, X=cin, v1=bias, v2=WxT, seed=5)
     assert ring == 0             # colour lin0 keeps register stores
-    ref = torch.relu(acc + bias.double()[None, :] + cin.double()[:, :6] @ WxT.double()[:, :N])
-    e = _err(OUT[:M, :N], ref)
+    e = _err(OUT[:M, :N], _color0_ref(acc, bias, cin, WxT))
     print(M, N, K, nprod, "color0", e)
     assert e < (BAR if nprod == 3 else BAR_NP1)
     _check_store(OUT, OUT2, before, M, N, N, ldx)
@@ -228,8 +248,7 @@ def test_dgrad_relu_split(M, N, K, nprod):
     H = H.cuda()
     acc, OUT, OUT2, before, ring = _run(11 if nprod == 3 else 111, M, N, K, ldx, ldx, X=H, seed=6)
     assert ring == int(_aligned(2 * r4(N)))
-    mask = (H[:, :N].bfloat16() != 0).double()
-    e = _err(OUT[:M, :N], acc * mask)
+    e = _err(OUT[:M, :N], _relu_mask_ref(acc, H))
     print(M, N, K, nprod, "ring", ring, "dgrad relu", e)
     assert e < (BAR if nprod == 3 else BAR_NP1)
     _check_store(OUT, OUT2, before, M, r4(N), r4(N), ldx)
@@ -269,9 +288,7 @@ def test_plain_store(M, N, K, nprod):
             "avc_tc_gemm_nt_test")
     torch.cuda.synchronize()
     assert _last_ring() == int(_aligned(4 * N))
-    (ah, al), (bh, bl) = _split(A), _split(B)
-    ref = ah @ bh.t() if nprod == 1 else ah @ bh.t() + ah @ bl.t() + al @ bh.t()
-    e = _err(Cm[:M], ref)
+    e = _err(Cm[:M], _split_acc(A, B, nprod))
     print(M, N, K, nprod, "plain", e)
     assert e < BAR
     assert torch.isnan(Cm[M:]).all()

@@ -1,6 +1,7 @@
-"""wgmma NT tiles at shapes where every CTA runs many 64-row tiles per consumer warpgroup: the persistent row loop, the
-wrap-around of the operand ring and the consumers' turn handoff, against an fp64 matmul on the device.  The last shape
-(K > 256) takes the variant that streams B through the ring."""
+"""wgmma NT tiles with the GEMM self-test's plain store at shapes where every CTA runs many 64-row tiles per consumer
+warpgroup: the persistent row loop, the wrap-around of the operand ring and the consumers' turn handoff, against an fp64
+matmul on the device.  The last shape (K > 256) takes the variant that streams B through the ring.  The epilogue
+functors at many tiles per CTA: test_nt_persistent_epilogue_gpu.py."""
 import pytest
 
 from test_tc_gemm_gpu import _run
