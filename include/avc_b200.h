@@ -579,9 +579,16 @@ int avc_uniform_fill(uint32_t seed, int32_t n, float lo, float hi, float* out, a
  * Triangles are oriented with normals towards decreasing u.
  * ------------------------------------------------------------------------------------------ */
 /* Profiling aid of the fused value-chain kernel: with AVC_CHAIN_DEBUG=1 in the environment block 0 records cycle
- * counters ([0] MMA warp waiting for its A operand, [1] for weight slabs, [2] MMA warp total, [3] tile-layers,
- * [4] epilogue waiting for the accumulator, [5] epilogue work); this call synchronises the device and copies them. */
+ * counters (consumer warpgroup 0: [0] waiting for its layer-0 input, [1] for weight slabs, [2] total, [3] tile-layers,
+ * [4] waiting for its turn at the MMAs, [5] epilogue work, [6] MMAs from the turn to the accumulator, [1] included;
+ * [7] the weight producer waiting for a free ring stage); this call synchronises the device and copies them. */
 int avc_chain_debug_read(long long* out8);
+/* For tests only: cap the persistent grid of the calling host thread's fused value-chain launches at n CTAs (0: no cap,
+ * the default), so that a small launch walks many 64-point tiles per CTA on both consumer warpgroups; returns the
+ * previous cap.  The library itself never sets it. */
+int avc_chain_set_max_ctas(int32_t n);
+/* gridDim.x of the calling host thread's last fused value-chain launch, -1: none yet. */
+int avc_chain_last_grid(void);
 /* Stall probe of the wgmma NT tiles: only in a diagnostic build (-DAVC_NT_PROBE=1, tools/nt_probe.py); a regular
  * build returns AVC_E_BADCFG.  host_out[16][10]: per epilogue functor the summed cycles {producer waiting for a free
  * stage, producer loop, consumers waiting for operands, consumers waiting for their turn, consumers' MMAs, consumers'

@@ -1,5 +1,6 @@
 """Times SDFNetwork.sdf (value chain without a stash) on the wgmma engine, fused kernel vs layer-by-layer launches,
-for the point counts of the placement passes and of a mesh grid.  Run on the GPU box: python tools/chain_probe.py"""
+for the point counts of the placement passes and of a mesh grid, and reads the fused kernel's cycle counters
+(AVC_CHAIN_DEBUG=1) at the placement passes' point counts.  Run on the GPU box: python tools/chain_probe.py"""
 import json
 import os
 import sys
@@ -42,8 +43,13 @@ def main():
             L.avc_chain_debug_read.argtypes = [C.POINTER(C.c_longlong)]
             if L.avc_chain_debug_read(buf) == 0:
                 n = max(1, buf[3])
-                row["block0_cycles_per_tile_layer"] = {"mma_wait_A": buf[0] / n, "mma_wait_W": buf[1] / n, "mma_total": buf[2] / n,
-                                                       "epi_wait_acc": buf[4] / n, "epi_work": buf[5] / n, "tile_layers": n}
+                # consumer warpgroup 0 of block 0 per tile-layer: waits for its layer-0 input, for weight slabs, for
+                # the MMA turn; MMAs (turn taken to accumulator ready, weight waits included); epilogue; loop total;
+                # and the weight producer's waits for a free ring stage
+                row["block0_cycles_per_tile_layer"] = {
+                    "wait_A": buf[0] / n, "wait_W": buf[1] / n, "wait_turn": buf[4] / n, "mma": buf[6] / n,
+                    "epi_work": buf[5] / n, "total": buf[2] / n, "producer_wait_free_stage": buf[7] / n,
+                    "tile_layers": n, "epi_share": buf[5] / max(1, buf[2])}
             os.environ["AVC_CHAIN_DEBUG"] = "0"
         out[str(P)] = row
     print(json.dumps(out))
