@@ -6,17 +6,16 @@
 //   k_cc_*              connected components of the triangle-edge graph: lock-free union-find (hook the larger root
 //                       under the smaller by CAS, path halving), flatten + atomicAdd sizes, one 64-bit atomicMax picks
 //                       the largest component (ties: smallest minimum vertex index, the reference's discovery order)
-//   k_drive_joints      J = J_regressor . v_template (one warp per joint, warp-shuffle sums)
-//   k_drive_chain       one warp per frame: rotations (or batch_rodrigues of axis-angle), kinematic chain, A[f][j][3x4]
+//   k_smpl_joints       J = J_regressor . v_template (avc_smpl.cuh)
+//   k_drive_chain       one warp per frame: rotations (or batch_rodrigues of axis-angle), then avc_smpl.cuh's kinematic
+//                       chain, A[f][j][3x4]
 //   k_inv_lbs           T = sum_j w_j A_j (fp64), p_T = M^-1 (p - t / s) in fp64 (torch.inverse(T) . [p; 1], rows 0-2)
 //   k_skin_frames       out[f][v] = (sum_j w_j A[f]_j) . [p_T; 1] for a range of frames, in the PC2 payload layout
-#include "avc_common.cuh"
+#include "avc_smpl.cuh"
 
 using namespace avc;
 
 namespace {
-
-constexpr int NJ_MAX = 32;
 
 // ---------------------------------------------------------------- nearest vertex (drive.py:235-240)
 constexpr int NN_THREADS = 128, NN_QPT = 4, NN_TILE = 256;
@@ -153,24 +152,6 @@ __global__ void k_cc_kept(const unsigned long long* __restrict__ key, int32_t* _
 }
 
 // ---------------------------------------------------------------- rigid transforms (drive.py:93-148, batched)
-__global__ void __launch_bounds__(256)
-k_drive_joints(const float* __restrict__ v_template, const float* __restrict__ J_regressor, int V, int NJ,
-               float* __restrict__ joints) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int j = warp; j < NJ; j += nw) {     // vertices2joints (drive.py:51-68)
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-    const float* jr = J_regressor + (size_t)j * V;
-    for (int v = lane; v < V; v += 32) {
-      const float w = jr[v];
-      a0 = fmaf(w, v_template[(size_t)v * 3 + 0], a0);
-      a1 = fmaf(w, v_template[(size_t)v * 3 + 1], a1);
-      a2 = fmaf(w, v_template[(size_t)v * 3 + 2], a2);
-    }
-    a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
-    if (lane == 0) { joints[j * 3 + 0] = a0; joints[j * 3 + 1] = a1; joints[j * 3 + 2] = a2; }
-  }
-}
-
 constexpr int CHAIN_WARPS = 4;
 
 __global__ void __launch_bounds__(CHAIN_WARPS * 32)
@@ -182,22 +163,9 @@ k_drive_chain(const float* __restrict__ joints, const float* __restrict__ pose, 
   const bool act = j < NJ;
   float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   if (act) {
-    if (pose2rot) {   // batch_rodrigues (drive.py:13-49)
+    if (pose2rot) {
       const float* r = pose + ((size_t)f * NJ + j) * 3;
-      const float rx = r[0], ry = r[1], rz = r[2];
-      const float eps = 1e-8f;
-      const float ang = sqrtf((rx + eps) * (rx + eps) + (ry + eps) * (ry + eps) + (rz + eps) * (rz + eps));
-      const float x = rx / ang, y = ry / ang, z = rz / ang;
-      float s, c;
-      sincosf(ang, &s, &c);
-      const float K[9] = {0, -z, y, z, 0, -x, -y, x, 0};
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) {
-          const float kk = K[a * 3] * K[b] + K[a * 3 + 1] * K[3 + b] + K[a * 3 + 2] * K[6 + b];
-          R[a * 3 + b] = ((a == b) ? 1.f : 0.f) + s * K[a * 3 + b] + (1.f - c) * kk;
-        }
+      rodrigues(r[0], r[1], r[2], R);
     } else {
       const float* r = pose + ((size_t)f * NJ + j) * 9;
 #pragma unroll
@@ -206,49 +174,9 @@ k_drive_chain(const float* __restrict__ joints, const float* __restrict__ pose, 
   }
   const int par = act ? parents[j] : -1;
   const float Jx = act ? joints[j * 3] : 0.f, Jy = act ? joints[j * 3 + 1] : 0.f, Jz = act ? joints[j * 3 + 2] : 0.f;
-  float tx = Jx, ty = Jy, tz = Jz;    // rel_joints (drive.py:123-124)
-  {
-    const int p = par < 0 ? 0 : par;
-    const float px = __shfl_sync(0xffffffffu, Jx, p), py = __shfl_sync(0xffffffffu, Jy, p),
-                pz = __shfl_sync(0xffffffffu, Jz, p);
-    if (act && j >= 1) { tx -= px; ty -= py; tz -= pz; }
-  }
-  float T[12] = {R[0], R[1], R[2], tx, R[3], R[4], R[5], ty, R[6], R[7], R[8], tz};
-  int depth = 0;
-  {   // depth in the tree (root 0) by pointer chasing through shuffles
-    int p = par;
-    for (int it = 0; it < NJ_MAX; ++it) {
-      const int pp = __shfl_sync(0xffffffffu, par, p < 0 ? 0 : p);
-      if (p >= 0) { ++depth; p = pp; }
-    }
-  }
-  int maxd = act ? depth : 0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) maxd = max(maxd, __shfl_xor_sync(0xffffffffu, maxd, o));
-  for (int d = 1; d <= maxd; ++d) {   // a joint's world transform once its parent's is final (drive.py:130-136)
-    float P[12];
-#pragma unroll
-    for (int i = 0; i < 12; ++i) P[i] = __shfl_sync(0xffffffffu, T[i], par < 0 ? 0 : par);
-    if (act && depth == d) {
-      float Nw[12];
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) Nw[r * 4 + c] = P[r * 4] * T[c] + P[r * 4 + 1] * T[4 + c] + P[r * 4 + 2] * T[8 + c];
-        Nw[r * 4 + 3] = P[r * 4] * T[3] + P[r * 4 + 1] * T[7] + P[r * 4 + 2] * T[11] + P[r * 4 + 3];
-      }
-#pragma unroll
-      for (int i = 0; i < 12; ++i) T[i] = Nw[i];
-    }
-  }
-  if (act) {   // rel_transforms: A = T - [0 | T_rot J]   (drive.py:143-146)
-    float* a = A_out + ((size_t)f * NJ + j) * 12;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      a[r * 4 + 0] = T[r * 4]; a[r * 4 + 1] = T[r * 4 + 1]; a[r * 4 + 2] = T[r * 4 + 2];
-      a[r * 4 + 3] = T[r * 4 + 3] - (T[r * 4] * Jx + T[r * 4 + 1] * Jy + T[r * 4 + 2] * Jz);
-    }
-  }
+  float T[12];
+  chain_world(R, j, par, act, Jx, Jy, Jz, T);
+  if (act) rel_transform(T, Jx, Jy, Jz, A_out + ((size_t)f * NJ + j) * 12);
 }
 
 // ---------------------------------------------------------------- inverse LBS (drive.py:242-253)
@@ -387,7 +315,7 @@ int avc_lbs_rel_transforms(const float* v_template, const float* J_regressor, co
   if (n_joints < 1 || n_joints > NJ_MAX) return AVC_E_BADCFG;
   if (V < 1 || n_frames < 1) return AVC_E_SIZE;
   cudaStream_t st = (cudaStream_t)stream;
-  k_drive_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, joints_out);
+  k_smpl_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, joints_out);
   k_drive_chain<<<blocks(n_frames, CHAIN_WARPS), CHAIN_WARPS * 32, 0, st>>>(joints_out, pose, pose2rot, parents,
                                                                             n_joints, n_frames, A_out);
   AVC_LAUNCH_TRY();

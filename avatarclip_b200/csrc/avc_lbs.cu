@@ -2,17 +2,22 @@
 // (AvatarGen/AppearanceGen/models/utils.py:72-106,176-224) with smplx's vertices2joints / batch_rigid_transform
 // (in-tree copies: drive.py:51-160).  Two launches:
 //   k_lbs_joints_chain  one CTA: joint regression by warp-shuffle reductions (one warp per joint at a time), then
-//                       warp 0 walks the kinematic tree level by level, lane j owning joint j and pulling its
-//                       parent's 3x4 transform with warp shuffles
+//                       warp 0 walks the kinematic tree (both from avc_smpl.cuh)
 //   k_lbs_skin          one thread per vertex: pose blend shapes (207-term dot against coalesced posedirs columns),
 //                       blended 3x4 transform from the 24 joint transforms held in shared memory, skinned vertex
-#include "avc_common.cuh"
+// Also defines k_smpl_joints (declared in avc_smpl.cuh), the joint regression that avc_lbs_rel_transforms and
+// avc_smpl_pose_batch launch.
+#include "avc_smpl.cuh"
 
 using namespace avc;
 
-namespace {
+__global__ void __launch_bounds__(256)
+avc::k_smpl_joints(const float* __restrict__ v_template, const float* __restrict__ J_regressor, int V, int NJ,
+                   float* __restrict__ J) {
+  regress_joints(v_template, J_regressor, V, NJ, J);
+}
 
-constexpr int NJ_MAX = 32;
+namespace {
 
 __global__ void __launch_bounds__(256)
 k_lbs_joints_chain(const float* __restrict__ v_shaped, const float* __restrict__ pose, int pose2rot,
@@ -20,37 +25,16 @@ k_lbs_joints_chain(const float* __restrict__ v_shaped, const float* __restrict__
                    float* __restrict__ A_out /*[NJ][12]*/, float* __restrict__ joints_out /*[NJ][3]*/,
                    float* __restrict__ feat_out /*[(NJ-1)*9]*/) {
   __shared__ float sJ[NJ_MAX][3];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  // ---- J = J_regressor @ v_shaped   (vertices2joints, drive.py:51-70)
-  for (int j = warp; j < NJ; j += nw) {
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-    const float* jr = J_regressor + (size_t)j * V;
-    for (int v = lane; v < V; v += 32) {
-      float w = jr[v];
-      a0 = fmaf(w, v_shaped[v * 3 + 0], a0); a1 = fmaf(w, v_shaped[v * 3 + 1], a1); a2 = fmaf(w, v_shaped[v * 3 + 2], a2);
-    }
-    a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
-    if (lane == 0) { sJ[j][0] = a0; sJ[j][1] = a1; sJ[j][2] = a2; }
-  }
+  regress_joints(v_shaped, J_regressor, V, NJ, &sJ[0][0]);
   __syncthreads();
-  if (warp != 0) return;
+  if ((threadIdx.x >> 5) != 0) return;
   // ---- lane j <-> joint j
-  const int j = lane;
+  const int j = threadIdx.x & 31;
   const bool act = j < NJ;
   float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   if (act) {
-    if (pose2rot) {   // batch_rodrigues, models/utils.py:72-106
-      float rx = pose[j * 3], ry = pose[j * 3 + 1], rz = pose[j * 3 + 2];
-      const float eps = 1e-8f;
-      float ang = sqrtf((rx + eps) * (rx + eps) + (ry + eps) * (ry + eps) + (rz + eps) * (rz + eps));
-      float x = rx / ang, y = ry / ang, z = rz / ang;
-      float s, c;
-      sincosf(ang, &s, &c);
-      float K[9] = {0, -z, y, z, 0, -x, -y, x, 0};
-      float KK[9];
-      for (int a = 0; a < 3; ++a)
-        for (int b = 0; b < 3; ++b) KK[a * 3 + b] = K[a * 3] * K[b] + K[a * 3 + 1] * K[3 + b] + K[a * 3 + 2] * K[6 + b];
-      for (int i = 0; i < 9; ++i) R[i] = ((i % 4 == 0) ? 1.f : 0.f) + s * K[i] + (1.f - c) * KK[i];
+    if (pose2rot) {
+      rodrigues(pose[j * 3], pose[j * 3 + 1], pose[j * 3 + 2], R);
     } else {
       for (int i = 0; i < 9; ++i) R[i] = pose[j * 9 + i];
     }
@@ -58,52 +42,12 @@ k_lbs_joints_chain(const float* __restrict__ v_shaped, const float* __restrict__
       for (int i = 0; i < 9; ++i) feat_out[(j - 1) * 9 + i] = R[i] - ((i % 4 == 0) ? 1.f : 0.f);   // pose_feature (:193)
   }
   const int par = act ? parents[j] : -1;
-  float Jx = act ? sJ[j][0] : 0.f, Jy = act ? sJ[j][1] : 0.f, Jz = act ? sJ[j][2] : 0.f;
-  // rel_joints (drive.py:122-123)
-  float tx = Jx, ty = Jy, tz = Jz;
-  {
-    int p = par < 0 ? 0 : par;
-    float px = __shfl_sync(0xffffffffu, Jx, p), py = __shfl_sync(0xffffffffu, Jy, p), pz = __shfl_sync(0xffffffffu, Jz, p);
-    if (act && j >= 1) { tx -= px; ty -= py; tz -= pz; }
-  }
-  // local transform M = [R | t]; world transform T, filled level by level (a joint's parent always has a smaller index)
-  float T[12] = {R[0], R[1], R[2], tx, R[3], R[4], R[5], ty, R[6], R[7], R[8], tz};
-  int depth = 0;
-  {   // depth of each joint (root 0), computed by pointer chasing through shuffles
-    int p = par;
-    for (int it = 0; it < NJ_MAX; ++it) {
-      int pp = __shfl_sync(0xffffffffu, par, p < 0 ? 0 : p);
-      if (p >= 0) { ++depth; p = pp; }
-    }
-  }
-  int maxd = depth;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) maxd = max(maxd, __shfl_xor_sync(0xffffffffu, act ? maxd : 0, o));
-  for (int d = 1; d <= maxd; ++d) {
-    float P[12];
-#pragma unroll
-    for (int i = 0; i < 12; ++i) P[i] = __shfl_sync(0xffffffffu, T[i], par < 0 ? 0 : par);
-    if (act && depth == d) {     // T = T_parent @ M   (drive.py:130-135)
-      float Nw[12];
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) Nw[r * 4 + c] = P[r * 4] * T[c] + P[r * 4 + 1] * T[4 + c] + P[r * 4 + 2] * T[8 + c];
-        Nw[r * 4 + 3] = P[r * 4] * T[3] + P[r * 4 + 1] * T[7] + P[r * 4 + 2] * T[11] + P[r * 4 + 3];
-      }
-#pragma unroll
-      for (int i = 0; i < 12; ++i) T[i] = Nw[i];
-    }
-  }
+  const float Jx = act ? sJ[j][0] : 0.f, Jy = act ? sJ[j][1] : 0.f, Jz = act ? sJ[j][2] : 0.f;
+  float T[12];
+  chain_world(R, j, par, act, Jx, Jy, Jz, T);
   if (act) {
     joints_out[j * 3 + 0] = T[3]; joints_out[j * 3 + 1] = T[7]; joints_out[j * 3 + 2] = T[11];   // posed joints (:140)
-    // rel_transforms: A = T - [0 | T_rot J]   (drive.py:144-145)
-    float* a = A_out + j * 12;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      a[r * 4 + 0] = T[r * 4]; a[r * 4 + 1] = T[r * 4 + 1]; a[r * 4 + 2] = T[r * 4 + 2];
-      a[r * 4 + 3] = T[r * 4 + 3] - (T[r * 4] * Jx + T[r * 4 + 1] * Jy + T[r * 4 + 2] * Jz);
-    }
+    rel_transform(T, Jx, Jy, Jz, A_out + j * 12);
   }
 }
 

@@ -8,7 +8,7 @@
 //   avc_realnvp_decode         VPoserRealNVP.decode (:233-240): the 8 conditional coupling blocks, the text feature folded
 //                              into each first linear's bias once per call, the whole chain in one kernel per tile of rows
 //   avc_smpl_pose_batch        smplx SMPL with zero betas for B body poses: pose blend shapes, kinematic chain, skinning;
-//                              each row is what avc_lbs_fwd computes for it (same arithmetic, same order)
+//                              each row is what avc_lbs_fwd computes for it (both pose through avc_smpl.cuh)
 //   avc_raster_textured_batch  render.py:10-39's renders of B meshes from A eyes per group of rows, one launch per pass
 //                              for the whole batch; each image is what avc_raster_textured makes of it
 //   avc_cosine_topk            F.cosine_similarity of N rows against one vector + torch.topk (VPoserCodebook :322-324)
@@ -20,6 +20,7 @@
 
 #include "avc_common.cuh"
 #include "avc_raster.cuh"
+#include "avc_smpl.cuh"
 
 using namespace avc;
 
@@ -37,7 +38,6 @@ constexpr int kNvpMaxBlocks = 16;
 constexpr int kMaxCams = 16;
 constexpr int kSupMax = 64;
 constexpr int kSupMaxD = 96;
-constexpr int NJ_MAX = 32;
 
 // Wt[k][n] = W[n][col0 + k] for k < K  (W row-major with leading dimension ldw)
 __global__ void k_transpose(const float* __restrict__ W, int N, int K, int ldw, int col0, float* __restrict__ Wt) {
@@ -297,28 +297,12 @@ k_realnvp_decode(const float* __restrict__ z, int B, int D, int E, int H, int nb
 }
 
 // ---------------------------------------------------------------- SMPL for a batch of body poses
-// J = J_regressor . v_template: the joint regression of k_lbs_joints_chain (avc_lbs.cu), same reduction order
-__global__ void __launch_bounds__(256)
-k_pose_joints(const float* __restrict__ v, const float* __restrict__ J_regressor, int V, int NJ, float* __restrict__ J) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int j = warp; j < NJ; j += nw) {
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-    const float* jr = J_regressor + (size_t)j * V;
-    for (int i = lane; i < V; i += 32) {
-      float w = jr[i];
-      a0 = fmaf(w, v[i * 3 + 0], a0); a1 = fmaf(w, v[i * 3 + 1], a1); a2 = fmaf(w, v[i * 3 + 2], a2);
-    }
-    a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
-    if (lane == 0) { J[j * 3] = a0; J[j * 3 + 1] = a1; J[j * 3 + 2] = a2; }
-  }
-}
-
 struct Orient {
   float r[3];
 };
 
 // one warp per pose row, lane j = joint j: batch_rodrigues of (global_orient, body_pose, zeros), the pose feature and
-// the kinematic chain of k_lbs_joints_chain, written per row: A [B][NJ][12], feat [B][(NJ-1)*9]
+// avc_smpl.cuh's kinematic chain, written per row: A [B][NJ][12], feat [B][(NJ-1)*9]
 __global__ void __launch_bounds__(128)
 k_pose_chain(const float* __restrict__ body_pose, int P, int B, Orient go, const float* __restrict__ Jg,
              const int* __restrict__ parents, int NJ, float* __restrict__ A_out, float* __restrict__ feat_out) {
@@ -336,68 +320,16 @@ k_pose_chain(const float* __restrict__ body_pose, int P, int B, Orient go, const
       const int q = (j - 1) * 3 + c;
       rv[c] = j == 0 ? go.r[c] : (q < P ? body_pose[(size_t)b * P + q] : 0.f);
     }
-    float rx = rv[0], ry = rv[1], rz = rv[2];
-    const float eps = 1e-8f;
-    float ang = sqrtf((rx + eps) * (rx + eps) + (ry + eps) * (ry + eps) + (rz + eps) * (rz + eps));
-    float x = rx / ang, y = ry / ang, z = rz / ang;
-    float s, c;
-    sincosf(ang, &s, &c);     // its Payne-Hanek path for |ang| > 105615 is the kernel's 32-byte stack frame
-    float K[9] = {0, -z, y, z, 0, -x, -y, x, 0};
-    float KK[9];
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-#pragma unroll
-      for (int bb = 0; bb < 3; ++bb) KK[a * 3 + bb] = K[a * 3] * K[bb] + K[a * 3 + 1] * K[3 + bb] + K[a * 3 + 2] * K[6 + bb];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) R[i] = ((i % 4 == 0) ? 1.f : 0.f) + s * K[i] + (1.f - c) * KK[i];
+    rodrigues(rv[0], rv[1], rv[2], R);
     if (j >= 1)
 #pragma unroll
       for (int i = 0; i < 9; ++i) feat[(j - 1) * 9 + i] = R[i] - ((i % 4 == 0) ? 1.f : 0.f);
   }
   const int par = act ? parents[j] : -1;
-  float Jx = act ? Jg[j * 3] : 0.f, Jy = act ? Jg[j * 3 + 1] : 0.f, Jz = act ? Jg[j * 3 + 2] : 0.f;
-  float tx = Jx, ty = Jy, tz = Jz;
-  {
-    int p = par < 0 ? 0 : par;
-    float px = __shfl_sync(0xffffffffu, Jx, p), py = __shfl_sync(0xffffffffu, Jy, p), pz = __shfl_sync(0xffffffffu, Jz, p);
-    if (act && j >= 1) { tx -= px; ty -= py; tz -= pz; }
-  }
-  float T[12] = {R[0], R[1], R[2], tx, R[3], R[4], R[5], ty, R[6], R[7], R[8], tz};
-  int depth = 0;
-  {
-    int p = par;
-    for (int it = 0; it < NJ_MAX; ++it) {
-      int pp = __shfl_sync(0xffffffffu, par, p < 0 ? 0 : p);
-      if (p >= 0) { ++depth; p = pp; }
-    }
-  }
-  int maxd = depth;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) maxd = max(maxd, __shfl_xor_sync(0xffffffffu, act ? maxd : 0, o));
-  for (int d = 1; d <= maxd; ++d) {
-    float Pm[12];
-#pragma unroll
-    for (int i = 0; i < 12; ++i) Pm[i] = __shfl_sync(0xffffffffu, T[i], par < 0 ? 0 : par);
-    if (act && depth == d) {
-      float Nw[12];
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) Nw[r * 4 + c] = Pm[r * 4] * T[c] + Pm[r * 4 + 1] * T[4 + c] + Pm[r * 4 + 2] * T[8 + c];
-        Nw[r * 4 + 3] = Pm[r * 4] * T[3] + Pm[r * 4 + 1] * T[7] + Pm[r * 4 + 2] * T[11] + Pm[r * 4 + 3];
-      }
-#pragma unroll
-      for (int i = 0; i < 12; ++i) T[i] = Nw[i];
-    }
-  }
-  if (act) {
-    float* a = A_out + ((size_t)b * NJ + j) * 12;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      a[r * 4 + 0] = T[r * 4]; a[r * 4 + 1] = T[r * 4 + 1]; a[r * 4 + 2] = T[r * 4 + 2];
-      a[r * 4 + 3] = T[r * 4 + 3] - (T[r * 4] * Jx + T[r * 4 + 1] * Jy + T[r * 4 + 2] * Jz);
-    }
-  }
+  const float Jx = act ? Jg[j * 3] : 0.f, Jy = act ? Jg[j * 3 + 1] : 0.f, Jz = act ? Jg[j * 3 + 2] : 0.f;
+  float T[12];
+  chain_world(R, j, par, act, Jx, Jy, Jz, T);
+  if (act) rel_transform(T, Jx, Jy, Jz, A_out + ((size_t)b * NJ + j) * 12);
 }
 
 constexpr int kSkinRows = 8;
@@ -417,42 +349,16 @@ k_pose_skin(const float* __restrict__ v_template, const float* __restrict__ pose
   __shared__ float sF[kSkinRows][NJ_MAX * 9];
   const int b0 = blockIdx.y * kSkinRows;
   const int nr = min(kSkinRows, B - b0);
-  for (int i = threadIdx.x; i < kSkinRows * NJ * 12; i += blockDim.x) {
-    const int r = i / (NJ * 12), k = i - r * NJ * 12;
-    sA[r][k] = r < nr ? A[(size_t)(b0 + r) * NJ * 12 + k] : 0.f;
-  }
-  for (int i = threadIdx.x; i < kSkinRows * NF; i += blockDim.x) {
-    const int r = i / NF, k = i - r * NF;
-    sF[r][k] = r < nr ? feat[(size_t)(b0 + r) * NF + k] : 0.f;
-  }
-  __syncthreads();
+  stage_rows<kSkinRows>(sA, sF, A, feat, b0, nr, NJ, NF);
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= V) return;
   float p[kSkinRows][3];
-  const float t0 = v_template[v * 3], t1 = v_template[v * 3 + 1], t2 = v_template[v * 3 + 2];
-#pragma unroll
-  for (int r = 0; r < kSkinRows; ++r) { p[r][0] = t0; p[r][1] = t1; p[r][2] = t2; }
-  const size_t ld = (size_t)V * 3;
-  for (int k = 0; k < NF; ++k) {
-    const float* pd = posedirs + (size_t)k * ld + (size_t)v * 3;
-    const float d0 = pd[0], d1 = pd[1], d2 = pd[2];
-#pragma unroll
-    for (int r = 0; r < kSkinRows; ++r) {
-      const float f = sF[r][k];
-      p[r][0] = fmaf(f, d0, p[r][0]); p[r][1] = fmaf(f, d1, p[r][1]); p[r][2] = fmaf(f, d2, p[r][2]);
-    }
-  }
+  pose_blend_rows<kSkinRows>(p, v_template, posedirs, sF, V, NF, v);
 #pragma unroll
   for (int r = 0; r < kSkinRows; ++r) {
     if (r >= nr) break;
     float T[12];
-#pragma unroll
-    for (int i = 0; i < 12; ++i) T[i] = 0.f;
-    for (int j = 0; j < NJ; ++j) {
-      const float w = lbs_weights[(size_t)v * NJ + j];
-#pragma unroll
-      for (int i = 0; i < 12; ++i) T[i] = fmaf(w, sA[r][j * 12 + i], T[i]);
-    }
+    blend_transform(lbs_weights + (size_t)v * NJ, sA[r], NJ, T);
     const float p0 = p[r][0], p1 = p[r][1], p2 = p[r][2];
     float o0 = T[0] * p0 + T[1] * p1 + T[2] * p2 + T[3];
     float o1 = T[4] * p0 + T[5] * p1 + T[6] * p2 + T[7];
@@ -658,42 +564,16 @@ k_pose_skin_bwd(const float* __restrict__ v_template, const float* __restrict__ 
   __shared__ float sF[kSkinRows][NJ_MAX * 9];
   const int b0 = blockIdx.y * kSkinRows;
   const int nr = min(kSkinRows, B - b0);
-  for (int i = threadIdx.x; i < kSkinRows * NJ * 12; i += blockDim.x) {
-    const int r = i / (NJ * 12), k = i - r * NJ * 12;
-    sA[r][k] = r < nr ? A[(size_t)(b0 + r) * NJ * 12 + k] : 0.f;
-  }
-  for (int i = threadIdx.x; i < kSkinRows * NF; i += blockDim.x) {
-    const int r = i / NF, k = i - r * NF;
-    sF[r][k] = r < nr ? feat[(size_t)(b0 + r) * NF + k] : 0.f;
-  }
-  __syncthreads();
+  stage_rows<kSkinRows>(sA, sF, A, feat, b0, nr, NJ, NF);
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= V) return;
   float p[kSkinRows][3];
-  const float t0 = v_template[v * 3], t1 = v_template[v * 3 + 1], t2 = v_template[v * 3 + 2];
-#pragma unroll
-  for (int r = 0; r < kSkinRows; ++r) { p[r][0] = t0; p[r][1] = t1; p[r][2] = t2; }
-  const size_t ld = (size_t)V * 3;
-  for (int k = 0; k < NF; ++k) {
-    const float* pd = posedirs + (size_t)k * ld + (size_t)v * 3;
-    const float d0 = pd[0], d1 = pd[1], d2 = pd[2];
-#pragma unroll
-    for (int r = 0; r < kSkinRows; ++r) {
-      const float f = sF[r][k];
-      p[r][0] = fmaf(f, d0, p[r][0]); p[r][1] = fmaf(f, d1, p[r][1]); p[r][2] = fmaf(f, d2, p[r][2]);
-    }
-  }
+  pose_blend_rows<kSkinRows>(p, v_template, posedirs, sF, V, NF, v);
 #pragma unroll
   for (int r = 0; r < kSkinRows; ++r) {
     if (r >= nr) break;
     float T[12];
-#pragma unroll
-    for (int i = 0; i < 12; ++i) T[i] = 0.f;
-    for (int j = 0; j < NJ; ++j) {
-      const float w = lbs_weights[(size_t)v * NJ + j];
-#pragma unroll
-      for (int i = 0; i < 12; ++i) T[i] = fmaf(w, sA[r][j * 12 + i], T[i]);
-    }
+    blend_transform(lbs_weights + (size_t)v * NJ, sA[r], NJ, T);
     const size_t o = ((size_t)(b0 + r) * V + v) * 3;
     float g0 = g_verts[o], g1 = g_verts[o + 1], g2 = g_verts[o + 2];
     if (pr.on) {     // q = o @ m  ->  g_o = m g_q
@@ -757,7 +637,7 @@ k_pose_gfeat(const float* __restrict__ posedirs, const float* __restrict__ gp, i
 }
 
 // one warp per pose row, lane j = joint j: the kinematic chain in reverse (children before parents, each parent
-// adding its children's terms in lane order), then batch_rodrigues' backward (the +1e-8 inside the norm included)
+// adding its children's terms in lane order), then batch_rodrigues' backward (the eps inside the norm included)
 __global__ void __launch_bounds__(128)
 k_pose_chain_bwd(const float* __restrict__ body_pose, int P, int B, const float* __restrict__ Jg,
                  const int* __restrict__ parents, int NJ, const float* __restrict__ A, const float* __restrict__ feat,
@@ -769,17 +649,8 @@ k_pose_chain_bwd(const float* __restrict__ body_pose, int P, int B, const float*
   const bool act = j < NJ;
   const int NF = (NJ - 1) * 9;
   const int par = act ? parents[j] : -1;
-  int depth = 0;
-  {
-    int p = par;
-    for (int it = 0; it < NJ_MAX; ++it) {
-      int pp = __shfl_sync(0xffffffffu, par, p < 0 ? 0 : p);
-      if (p >= 0) { ++depth; p = pp; }
-    }
-  }
-  int maxd = depth;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) maxd = max(maxd, __shfl_xor_sync(0xffffffffu, act ? maxd : 0, o));
+  const int depth = joint_depth(par);
+  const int maxd = max_depth(depth);
   // forward values: R_j = feat_j + I, t_j = J_j - J_par, the parent's world rotation P3 = A[par][:, :3]
   float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, t[3] = {0.f, 0.f, 0.f}, P3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   const float Jx = act ? Jg[j * 3] : 0.f, Jy = act ? Jg[j * 3 + 1] : 0.f, Jz = act ? Jg[j * 3 + 2] : 0.f;
@@ -846,17 +717,10 @@ k_pose_chain_bwd(const float* __restrict__ body_pose, int P, int B, const float*
     const int q = (j - 1) * 3 + c;
     rv[c] = q < P ? body_pose[(size_t)b * P + q] : 0.f;
   }
-  const float eps = 1e-8f;
-  const float ang = sqrtf((rv[0] + eps) * (rv[0] + eps) + (rv[1] + eps) * (rv[1] + eps) + (rv[2] + eps) * (rv[2] + eps));
-  const float x = rv[0] / ang, y = rv[1] / ang, z = rv[2] / ang;
-  float s, c;
-  sincosf(ang, &s, &c);
-  const float K[9] = {0, -z, y, z, 0, -x, -y, x, 0};
-  float KK[9];
-#pragma unroll
-  for (int a = 0; a < 3; ++a)
-#pragma unroll
-    for (int bb = 0; bb < 3; ++bb) KK[a * 3 + bb] = K[a * 3] * K[bb] + K[a * 3 + 1] * K[3 + bb] + K[a * 3 + 2] * K[6 + bb];
+  const Rodrigues rq = rodrigues_terms(rv[0], rv[1], rv[2]);
+  const float ang = rq.ang, s = rq.s, c = rq.c;
+  const float* K = rq.K;
+  const float* KK = rq.KK;
   // R = I + s K + (1 - c) K K
   float gs = 0.f, gc = 0.f;
 #pragma unroll
@@ -879,7 +743,7 @@ k_pose_chain_bwd(const float* __restrict__ body_pose, int P, int B, const float*
 #pragma unroll
   for (int cc = 0; cc < 3; ++cc) {
     const int q = (j - 1) * 3 + cc;
-    if (q < P) g_pose[(size_t)b * P + q] = ga[cc] / ang + gang * (rv[cc] + eps) / ang;
+    if (q < P) g_pose[(size_t)b * P + q] = ga[cc] / ang + gang * (rv[cc] + kRodriguesEps) / ang;
   }
 }
 
@@ -1394,7 +1258,7 @@ int avc_smpl_pose_batch(const float* v_template, const float* J_regressor, const
   pr.on = post_rot != nullptr;
   if (post_rot)
     for (int i = 0; i < 9; ++i) pr.m[i] = post_rot[i];
-  k_pose_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, J);
+  k_smpl_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, J);
   k_pose_chain<<<(B + 3) / 4, 128, 0, st>>>(body_pose, pose_dim, B, go, J, parents, n_joints, A, feat);
   dim3 grid((V + 127) / 128, (B + kSkinRows - 1) / kSkinRows);
   k_pose_skin<<<grid, 128, 0, st>>>(v_template, posedirs, feat, A, lbs_weights, V, n_joints, (n_joints - 1) * 9, B, pr,
@@ -1560,7 +1424,7 @@ int avc_smpl_pose_batch_bwd(const float* v_template, const float* J_regressor, c
   pr.on = post_rot != nullptr;
   if (post_rot)
     for (int i = 0; i < 9; ++i) pr.m[i] = post_rot[i];
-  k_pose_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, J);
+  k_smpl_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, J);
   k_pose_chain<<<(B + 3) / 4, 128, 0, st>>>(body_pose, pose_dim, B, o, J, parents, n_joints, A, feat);
   const unsigned rows = (unsigned)((B + kSkinRows - 1) / kSkinRows);
   k_pose_skin_bwd<<<dim3((V + 127) / 128, rows), 128, 0, st>>>(v_template, posedirs, feat, A, lbs_weights, V, n_joints,
