@@ -42,7 +42,8 @@ class OracleTrainer:
         return ([("sdf." + k, v) for k, v in self.sp.items()] + [("col." + k, v) for k, v in self.cp.items()]
                 + [("var.variance", self.var)])
 
-    def loss(self, view, cos_anneal: float = 1.0, use_jitter: bool = True):
+    def loss(self, view, cos_anneal: float = 1.0, use_jitter: bool = True, z_vals=None):
+        """``z_vals`` (test hook, see ``neus.render``): composite on these sorted depths instead of placing samples."""
         dt = self.dtype
         igr, mw, cw = self.w
         o, d = view.rays_o.to(dt), view.rays_d.to(dt)
@@ -55,7 +56,8 @@ class OracleTrainer:
         else:
             bg = None
         out = neus.render(self.sp, self.cp, self.var, self.sconf, self.cconf, self.rconf, o, d, near, far,
-                          jitter=jit, background_rgb=bg, cos_anneal_ratio=cos_anneal)
+                          jitter=jit, background_rgb=bg, cos_anneal_ratio=cos_anneal,
+                          z_vals=None if z_vals is None else z_vals.to(dt))
         H, W = view.H, view.W
         dm = view.in_mask.reshape(H, W).bool()
         cbg = None if view.canvas_background is None else view.canvas_background.to(dt).reshape(-1, 1)
