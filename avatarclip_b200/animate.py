@@ -8,9 +8,10 @@ Two generators of models/pose_generation.py run here:
   * ``VPoserRealNVP`` (:176-285): per candidate ``num_batch`` x ``num_sample`` prior draws through the text-conditioned
     RealNVP and VPoser, each pose posed on SMPL, rendered with the UV texture from 5 cameras and scored by CLIP; the
     best of the batches is kept, then the candidates are sorted by a fresh score.
-The gradient-based generators are refused before any file is read: ``PoseOptimizer`` runs as ``python -m
-avatarclip_b200.pose_optimizer``, and ``VPoserOptimizer`` is not available (the VPoser decoder's backward is not built);
-the motion stage (``general.mode = motion``) is ``python -m avatarclip_b200.motion``.
+The gradient-based generators are refused before any file is read, each naming its own command: ``PoseOptimizer``
+runs as ``python -m avatarclip_b200.pose_optimizer`` and ``VPoserOptimizer`` as ``python -m
+avatarclip_b200.vposer_optimizer`` (the VPoser latent optimised through ``avc_vposer_decode_bwd``); the motion stage
+(``general.mode = motion``) is ``python -m avatarclip_b200.motion``.
 
 Everything on the hot path runs in libavc_b200.so: ``avc_vposer_decode``, ``avc_realnvp_decode``,
 ``avc_smpl_pose_batch``, ``avc_raster_textured_batch``, ``avc_clip_prep_nearest``, the CLIP towers,
@@ -45,7 +46,8 @@ IN_SCOPE = ("VPoserCodebook", "VPoserRealNVP")
 OUT_OF_SCOPE = {"PoseOptimizer": "optimises SMPL theta through the rasteriser's gradient, so it runs as its own "
                                  "command: python -m avatarclip_b200.pose_optimizer",
                 "VPoserOptimizer": "optimises the VPoser latent through the rasteriser's gradient and the VPoser "
-                                   "decoder's, and the decoder's backward is not built"}
+                                   "decoder's, so it runs as its own command: python -m "
+                                   "avatarclip_b200.vposer_optimizer"}
 DEFAULT_PATHS = {"vposer": "data/vposer", "codebook": "data/codebook.pth",      # BasePoseGenerator / the
                  "realnvp": "data/pose_realnvp.pth"}                           # generators' constructor defaults
 _RENDER_BYTES = 1 << 30                 # device bytes per chunk of renders (z-buffers, images, CLIP inputs)

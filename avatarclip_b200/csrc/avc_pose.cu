@@ -4,6 +4,9 @@
 //   avc_vposer_decode          VPoser 2.x decode: decoder_net (Linear, LeakyReLU, Linear, LeakyReLU, Linear) then the
 //                              6D -> matrix (Gram-Schmidt) -> quaternion -> axis-angle tail (matrot2aa), one kernel per
 //                              tile of rows
+//   avc_vposer_decode_bwd      its backward, d loss / d z from d loss / d pose_body: the forward recomputed bit for bit,
+//                              the matrot2aa tail's Jacobian by forward-mode duals, then the three Linear / LeakyReLU
+//                              input gradients, one kernel per tile of rows
 //   avc_realnvp_pack           the coupling nets' weights transposed for avc_realnvp_decode, once per checkpoint
 //   avc_realnvp_decode         VPoserRealNVP.decode (:233-240): the 8 conditional coupling blocks, the text feature folded
 //                              into each first linear's bias once per call, the whole chain in one kernel per tile of rows
@@ -16,9 +19,11 @@
 //   avc_pose_score             get_pose_feature's mean over the cameras, calculate_pose_score's cosine, get_pose's
 //                              per-batch argmax (:88-89, 94, 273-274)
 #include <cfloat>
+#include <type_traits>
 #include <vector>
 
 #include "avc_common.cuh"
+#include "avc_dual.cuh"
 #include "avc_raster.cuh"
 #include "avc_smpl.cuh"
 
@@ -74,26 +79,44 @@ __device__ __forceinline__ void dense_rows(const float* in, int ldi, int K, cons
 
 // ---------------------------------------------------------------- VPoser decode
 // ContinousRotReprDecoder + matrot2aa (torchgeometry rotation_matrix_to_quaternion / quaternion_to_angle_axis) of one
-// joint: x[6] read as a [3][2] matrix, columns a = (x0, x2, x4), c = (x1, x3, x5).
-__device__ __forceinline__ void rot6d_to_aa(const float* x, float* aa, float* rm) {
-  float a[3] = {x[0], x[2], x[4]}, c[3] = {x[1], x[3], x[5]};
-  float na = fmaxf(sqrtf(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]), 1e-12f);     // F.normalize
-  float b1[3] = {a[0] / na, a[1] / na, a[2] / na};
-  float dot = b1[0] * c[0] + b1[1] * c[1] + b1[2] * c[2];
-  float u[3] = {c[0] - dot * b1[0], c[1] - dot * b1[1], c[2] - dot * b1[2]};
-  float nu = fmaxf(sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]), 1e-12f);
-  float b2[3] = {u[0] / nu, u[1] / nu, u[2] / nu};
-  float b3[3] = {b1[1] * b2[2] - b1[2] * b2[1], b1[2] * b2[0] - b1[0] * b2[2], b1[0] * b2[1] - b1[1] * b2[0]};
+// joint: x[6] read as a [3][2] matrix, columns a = (x0, x2, x4), c = (x1, x3, x5).  S = float gives the values and
+// records each branch taken in br; S = Dual (avc_dual.cuh) gives one column of the Jacobian and takes the branches
+// recorded in br, so the backward differentiates exactly the branches of the forward whose pose was rendered, whatever
+// the duals' value arithmetic would round to.  The gradient is autograd's on the branch taken: F.normalize's clamp
+// passes none where it is active, and torchgeometry's masked quaternion carries gradient only from its selected
+// branch, 0.5 / sqrt(t) included.  At an exact identity rotation (s2 = 0) torch's backward is NaN (sqrt's backward at
+// 0); the duals give the finite k = 2 branch's derivative there, a point no test compares.
+template <class S>
+__device__ __forceinline__ void rot6d_to_aa(const S* x, S* aa, float* rm, unsigned& br) {
+  constexpr bool kRecord = std::is_same<S, float>::value;
+  if (kRecord) br = 0u;
+  auto take = [&br](unsigned bit, bool cond) {
+    if (kRecord) {
+      if (cond) br |= bit;
+      return cond;
+    }
+    return (br & bit) != 0u;
+  };
+  S a[3] = {x[0], x[2], x[4]}, c[3] = {x[1], x[3], x[5]};
+  const S la = dsqrt(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]);
+  const S na = take(1u, val(la) >= 1e-12f) ? la : konst<S>(1e-12f);            // F.normalize
+  S b1[3] = {a[0] / na, a[1] / na, a[2] / na};
+  S dot = b1[0] * c[0] + b1[1] * c[1] + b1[2] * c[2];
+  S u[3] = {c[0] - dot * b1[0], c[1] - dot * b1[1], c[2] - dot * b1[2]};
+  const S lu = dsqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]);
+  const S nu = take(2u, val(lu) >= 1e-12f) ? lu : konst<S>(1e-12f);
+  S b2[3] = {u[0] / nu, u[1] / nu, u[2] / nu};
+  S b3[3] = {b1[1] * b2[2] - b1[2] * b2[1], b1[2] * b2[0] - b1[0] * b2[2], b1[0] * b2[1] - b1[1] * b2[0]};
   // R = stack([b1, b2, b3], -1): R[i][j] = b_j[i]
-  float R[9] = {b1[0], b2[0], b3[0], b1[1], b2[1], b3[1], b1[2], b2[2], b3[2]};
+  S R[9] = {b1[0], b2[0], b3[0], b1[1], b2[1], b3[1], b1[2], b2[2], b3[2]};
   if (rm)
 #pragma unroll
-    for (int i = 0; i < 9; ++i) rm[i] = R[i];
+    for (int i = 0; i < 9; ++i) rm[i] = val(R[i]);
   // rmat_t = R^T: m(i, j) = R[j][i]
 #define M(i, j) R[(j) * 3 + (i)]
-  float q[4], t;
-  if (M(2, 2) < 1e-6f) {
-    if (M(0, 0) > M(1, 1)) {
+  S q[4], t;
+  if (take(4u, val(M(2, 2)) < 1e-6f)) {
+    if (take(8u, val(M(0, 0)) > val(M(1, 1)))) {
       t = 1.f + M(0, 0) - M(1, 1) - M(2, 2);
       q[0] = M(1, 2) - M(2, 1); q[1] = t; q[2] = M(0, 1) + M(1, 0); q[3] = M(2, 0) + M(0, 2);
     } else {
@@ -101,7 +124,7 @@ __device__ __forceinline__ void rot6d_to_aa(const float* x, float* aa, float* rm
       q[0] = M(2, 0) - M(0, 2); q[1] = M(0, 1) + M(1, 0); q[2] = t; q[3] = M(1, 2) + M(2, 1);
     }
   } else {
-    if (M(0, 0) < -M(1, 1)) {
+    if (take(16u, val(M(0, 0)) < -val(M(1, 1)))) {
       t = 1.f - M(0, 0) - M(1, 1) + M(2, 2);
       q[0] = M(0, 1) - M(1, 0); q[1] = M(2, 0) + M(0, 2); q[2] = M(1, 2) + M(2, 1); q[3] = t;
     } else {
@@ -110,13 +133,13 @@ __device__ __forceinline__ void rot6d_to_aa(const float* x, float* aa, float* rm
     }
   }
 #undef M
-  const float st = sqrtf(t);
+  const S st = dsqrt(t);
 #pragma unroll
   for (int i = 0; i < 4; ++i) q[i] = (q[i] / st) * 0.5f;
-  const float s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-  const float s = sqrtf(s2), co = q[0];
-  const float two_theta = 2.f * (co < 0.f ? atan2f(-s, -co) : atan2f(s, co));
-  const float k = s2 > 0.f ? two_theta / s : 2.f;
+  const S s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  const S s = dsqrt(s2), co = q[0];
+  const S two_theta = 2.f * (take(32u, val(co) < 0.f) ? datan2(-s, -co) : datan2(s, co));
+  const S k = take(64u, val(s2) > 0.f) ? two_theta / s : konst<S>(2.f);
   aa[0] = q[1] * k; aa[1] = q[2] * k; aa[2] = q[3] * k;
 }
 
@@ -124,14 +147,12 @@ struct VpWeights {
   const float *w1t, *b1, *w2t, *b2, *w3t, *b3;   // transposed [K][N] copies in the workspace, biases as given
 };
 
-__global__ void __launch_bounds__(256)
-k_vposer_decode(const float* __restrict__ z, int B, int L, int H, int NJ, VpWeights w, float* __restrict__ pose_out,
-                float* __restrict__ rotmat_out) {
-  __shared__ float sz[kVpRows * kVpMaxL];
-  __shared__ float sh1[kVpRows * kVpMaxH];
-  __shared__ float sh2[kVpRows * kVpMaxH];
-  __shared__ float so[kVpRows * kVpMaxOut];
-  const int row0 = blockIdx.x * kVpRows, O = NJ * 6;
+// decoder_net of the kVpRows rows from row0 (rows past B read as 0) into shared memory: sh1 / sh2 the two LeakyReLU
+// outputs, so the 6 n_joints outputs.  k_vposer_decode and k_vposer_decode_bwd both run this, so the backward sees
+// the forward's bits.
+__device__ __forceinline__ void vposer_decoder_rows(const float* __restrict__ z, int B, int L, int H, int O,
+                                                    const VpWeights& w, int row0, float* sz, float* sh1, float* sh2,
+                                                    float* so) {
   for (int i = threadIdx.x; i < kVpRows * L; i += blockDim.x) {
     const int r = i / L, row = row0 + r;
     sz[i] = row < B ? z[(size_t)row * L + (i - r * L)] : 0.f;
@@ -143,13 +164,102 @@ k_vposer_decode(const float* __restrict__ z, int B, int L, int H, int NJ, VpWeig
   __syncthreads();
   dense_rows<kVpRows>(sh2, H, H, w.w3t, O, w.b3, 0, so, O);       // decoder_net.5
   __syncthreads();
+}
+
+__global__ void __launch_bounds__(256)
+k_vposer_decode(const float* __restrict__ z, int B, int L, int H, int NJ, VpWeights w, float* __restrict__ pose_out,
+                float* __restrict__ rotmat_out) {
+  __shared__ float sz[kVpRows * kVpMaxL];
+  __shared__ float sh1[kVpRows * kVpMaxH];
+  __shared__ float sh2[kVpRows * kVpMaxH];
+  __shared__ float so[kVpRows * kVpMaxOut];
+  const int row0 = blockIdx.x * kVpRows, O = NJ * 6;
+  vposer_decoder_rows(z, B, L, H, O, w, row0, sz, sh1, sh2, so);
   for (int i = threadIdx.x; i < kVpRows * NJ; i += blockDim.x) {
     const int r = i / NJ, j = i - r * NJ, row = row0 + r;
     if (row >= B) continue;
     float aa[3];
-    rot6d_to_aa(so + r * O + j * 6, aa, rotmat_out ? rotmat_out + ((size_t)row * NJ + j) * 9 : nullptr);
+    unsigned br;
+    rot6d_to_aa(so + r * O + j * 6, aa, rotmat_out ? rotmat_out + ((size_t)row * NJ + j) * 9 : nullptr, br);
     float* p = pose_out + ((size_t)row * NJ + j) * 3;
     p[0] = aa[0]; p[1] = aa[1]; p[2] = aa[2];
+  }
+}
+
+// out[r][k] = sum_n g[r][n] W[n][k] for ROWS rows in shared memory: the input gradient of a Linear whose weight W
+// [N][K] is in nn.Linear's layout, read coalesced along k.  With leaky, out holds that Linear's LeakyReLU output on
+// entry, whose sign is its input's, and the product is scaled by LeakyReLU's derivative there (1 above 0, else 0.01,
+// as torch's backward takes it at 0) in place.
+template <int ROWS>
+__device__ __forceinline__ void dense_t_rows(const float* g, int ldg, int N, const float* __restrict__ W, int K,
+                                             bool leaky, float* out, int ldo) {
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    float acc[ROWS];
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) acc[r] = 0.f;
+    for (int n = 0; n < N; ++n) {
+      const float w = W[(size_t)n * K + k];
+#pragma unroll
+      for (int r = 0; r < ROWS; ++r) acc[r] = fmaf(g[r * ldg + n], w, acc[r]);
+    }
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) {
+      float v = acc[r];
+      if (leaky && !(out[r * ldo + k] > 0.f)) v *= kLeaky;
+      out[r * ldo + k] = v;
+    }
+  }
+}
+
+// d loss / d z of the kVpRows rows from row0 given d loss / d pose_body g_pose [B][NJ][3]: the forward recomputed by
+// vposer_decoder_rows, then per joint g6 = J^T g_aa (J [3][6] from six dual passes of rot6d_to_aa), then
+// W3^T g6 . leaky'(pre2), W2^T . leaky'(pre1), W1^T, each in place over the forward's shared buffers.  pose_out, when
+// given, receives the recomputed pose, bit for bit k_vposer_decode's.
+__global__ void __launch_bounds__(256)
+k_vposer_decode_bwd(const float* __restrict__ z, int B, int L, int H, int NJ, VpWeights w, const float* __restrict__ W1,
+                    const float* __restrict__ W2, const float* __restrict__ W3, const float* __restrict__ g_pose,
+                    float* __restrict__ g_z, float* __restrict__ pose_out) {
+  __shared__ float sz[kVpRows * kVpMaxL];
+  __shared__ float sh1[kVpRows * kVpMaxH];
+  __shared__ float sh2[kVpRows * kVpMaxH];
+  __shared__ float so[kVpRows * kVpMaxOut];
+  const int row0 = blockIdx.x * kVpRows, O = NJ * 6;
+  vposer_decoder_rows(z, B, L, H, O, w, row0, sz, sh1, sh2, so);
+  for (int i = threadIdx.x; i < kVpRows * NJ; i += blockDim.x) {
+    const int r = i / NJ, j = i - r * NJ, row = row0 + r;
+    float* x = so + r * O + j * 6;
+    float g6[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (row < B) {
+      float xv[6], aa[3];
+#pragma unroll
+      for (int c = 0; c < 6; ++c) xv[c] = x[c];
+      unsigned br;
+      rot6d_to_aa(xv, aa, nullptr, br);
+      const size_t o = ((size_t)row * NJ + j) * 3;
+      if (pose_out) { pose_out[o] = aa[0]; pose_out[o + 1] = aa[1]; pose_out[o + 2] = aa[2]; }
+      const float ga[3] = {g_pose[o], g_pose[o + 1], g_pose[o + 2]};
+#pragma unroll 1
+      for (int i6 = 0; i6 < 6; ++i6) {
+        Dual xd[6], ad[3];
+#pragma unroll
+        for (int c = 0; c < 6; ++c) xd[c] = Dual{xv[c], c == i6 ? 1.f : 0.f};
+        rot6d_to_aa(xd, ad, nullptr, br);
+        g6[i6] = fmaf(ga[0], ad[0].d, fmaf(ga[1], ad[1].d, ga[2] * ad[2].d));
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 6; ++c) x[c] = g6[c];
+  }
+  __syncthreads();
+  dense_t_rows<kVpRows>(so, O, O, W3, H, true, sh2, H);          // through decoder_net.5 and the LeakyReLU at 4
+  __syncthreads();
+  dense_t_rows<kVpRows>(sh2, H, H, W2, H, true, sh1, H);         // through decoder_net.3 and the LeakyReLU at 1
+  __syncthreads();
+  dense_t_rows<kVpRows>(sh1, H, H, W1, L, false, sz, L);         // through decoder_net.0
+  __syncthreads();
+  for (int i = threadIdx.x; i < kVpRows * L; i += blockDim.x) {
+    const int r = i / L, row = row0 + r;
+    if (row < B) g_z[(size_t)row * L + (i - r * L)] = sz[i];
   }
 }
 
@@ -1102,6 +1212,21 @@ static int raster_batch_run(const float* verts, int B, int group, const int* fac
   return 0;
 }
 
+// decoder_net's weights transposed to [K][N] into the workspace (avc_vposer_decode_workspace_bytes), as
+// k_vposer_decode and k_vposer_decode_bwd read them
+static VpWeights vposer_weights(int L, int H, int n_joints, const float* W1, const float* b1, const float* W2,
+                                const float* b2, const float* W3, const float* b3, void* workspace, cudaStream_t st) {
+  const int O = n_joints * 6;
+  Carver c(workspace);
+  float* w1t = c.take<float>((size_t)L * H);
+  float* w2t = c.take<float>((size_t)H * H);
+  float* w3t = c.take<float>((size_t)H * O);
+  k_transpose<<<(H * L + 255) / 256, 256, 0, st>>>(W1, H, L, L, 0, w1t);
+  k_transpose<<<(H * H + 255) / 256, 256, 0, st>>>(W2, H, H, H, 0, w2t);
+  k_transpose<<<(O * H + 255) / 256, 256, 0, st>>>(W3, O, H, H, 0, w3t);
+  return VpWeights{w1t, b1, w2t, b2, w3t, b3};
+}
+
 extern "C" {
 
 int avc_vposer_decode_workspace_bytes(int32_t latent, int32_t hidden, int32_t n_joints, size_t* bytes) {
@@ -1125,16 +1250,29 @@ int avc_vposer_decode(const float* z, int32_t B, int32_t latent, const float* W1
   AVC_TRY(avc_vposer_decode_workspace_bytes(latent, hidden, n_joints, &need));
   if (B < 1 || workspace_bytes < need) return AVC_E_SIZE;
   cudaStream_t st = (cudaStream_t)stream;
-  const int L = latent, H = hidden, O = n_joints * 6;
-  Carver c(workspace);
-  float* w1t = c.take<float>((size_t)L * H);
-  float* w2t = c.take<float>((size_t)H * H);
-  float* w3t = c.take<float>((size_t)H * O);
-  k_transpose<<<(H * L + 255) / 256, 256, 0, st>>>(W1, H, L, L, 0, w1t);
-  k_transpose<<<(H * H + 255) / 256, 256, 0, st>>>(W2, H, H, H, 0, w2t);
-  k_transpose<<<(O * H + 255) / 256, 256, 0, st>>>(W3, O, H, H, 0, w3t);
-  VpWeights w{w1t, b1, w2t, b2, w3t, b3};
-  k_vposer_decode<<<(B + kVpRows - 1) / kVpRows, 256, 0, st>>>(z, B, L, H, n_joints, w, pose_out, rotmat_out);
+  const VpWeights w = vposer_weights(latent, hidden, n_joints, W1, b1, W2, b2, W3, b3, workspace, st);
+  k_vposer_decode<<<(B + kVpRows - 1) / kVpRows, 256, 0, st>>>(z, B, latent, hidden, n_joints, w, pose_out,
+                                                               rotmat_out);
+  AVC_LAUNCH_TRY();
+  return 0;
+}
+
+int avc_vposer_decode_bwd_workspace_bytes(int32_t latent, int32_t hidden, int32_t n_joints, size_t* bytes) {
+  return avc_vposer_decode_workspace_bytes(latent, hidden, n_joints, bytes);
+}
+
+int avc_vposer_decode_bwd(const float* z, int32_t B, int32_t latent, const float* W1, const float* b1, int32_t hidden,
+                          const float* W2, const float* b2, const float* W3, const float* b3, int32_t n_joints,
+                          const float* g_pose, float* g_z, float* pose_out, void* workspace, size_t workspace_bytes,
+                          avc_stream_t stream) {
+  if (!z || !W1 || !b1 || !W2 || !b2 || !W3 || !b3 || !g_pose || !g_z || !workspace) return AVC_E_NULL;
+  size_t need = 0;
+  AVC_TRY(avc_vposer_decode_bwd_workspace_bytes(latent, hidden, n_joints, &need));
+  if (B < 1 || workspace_bytes < need) return AVC_E_SIZE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const VpWeights w = vposer_weights(latent, hidden, n_joints, W1, b1, W2, b2, W3, b3, workspace, st);
+  k_vposer_decode_bwd<<<(B + kVpRows - 1) / kVpRows, 256, 0, st>>>(z, B, latent, hidden, n_joints, w, W1, W2, W3,
+                                                                   g_pose, g_z, pose_out);
   AVC_LAUNCH_TRY();
   return 0;
 }

@@ -239,17 +239,54 @@ class PoseStep:
 
 
 # ---------------------------------------------------------------- the generator
-def optimizer_refusal(pg: Mapping) -> Optional[str]:
-    """Why a PoseOptimizer block's optimiser cannot run here, or None."""
-    return motion.adam_refusal(pg, "PoseOptimizer", OPTIMIZER_DEFAULTS["optim_cfg"])
+def optimizer_refusal(pg: Mapping, who: str = "PoseOptimizer") -> Optional[str]:
+    """Why a PoseOptimizer (or ``who``'s) block's optimiser cannot run here, or None."""
+    return motion.adam_refusal(pg, who, OPTIMIZER_DEFAULTS["optim_cfg"])
+
+
+def adam_step(param: torch.Tensor, grad: torch.Tensor, m: torch.Tensor, v: torch.Tensor, state: torch.Tensor,
+              betas, eps: float):
+    """One torch.optim.Adam step of param by grad in place (avc_adam_step_dev; the step count and lr in state)."""
+    _lib.check(_lib.lib().avc_adam_step_dev(_lib.ptr(param), _lib.ptr(grad), _lib.ptr(m), _lib.ptr(v), param.numel(),
+                                            _lib.ptr(state), betas[0], betas[1], eps, 1.0, _lib.stream_ptr()),
+               "avc_adam_step_dev")
+
+
+def replay_iterations(step: PoseStep, cams: torch.Tensor, prime, body, grad: Optional[torch.Tensor] = None):
+    """Capture body() (one iteration, ending in the parameter update) once as a CUDA graph and replay it once per
+    iteration of cams [T, B A, cam_bytes], copying that iteration's cameras in first.  prime() -- the iteration
+    without its update -- runs once before the capture, so that first-launch set-up stays outside the graph.  Returns
+    step.loss after each replay [T, B] and, when grad is given, grad after each replay [T, *grad.shape] (else None)."""
+    dev = step.pose.device
+    T = cams.shape[0]
+    losses = torch.empty(T, step.B, device=dev)
+    grads = torch.empty(T, *grad.shape, device=dev) if grad is not None else None
+    # capture on a side stream after one forward and backward without the update (first-launch set-up)
+    step.cams.copy_(cams[0])
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        prime()
+    torch.cuda.current_stream(dev).wait_stream(side)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        body()
+    for it in range(T):
+        step.cams.copy_(cams[it])
+        g.replay()
+        losses[it].copy_(step.loss)
+        if grads is not None:
+            grads[it].copy_(grad)
+    return losses, grads
 
 
 class PoseOptimizer(animate.BasePoseGenerator):
     """:102-135 with the reference's constructor defaults."""
+    PARAM_DIM = POSE_DIM            # the optimised parameter of one candidate
 
     def __init__(self, optim_name="Adam", optim_cfg=None, num_iteration=500, topk=5, **kwargs):
         cfg = dict(OPTIMIZER_DEFAULTS["optim_cfg"] if optim_cfg is None else optim_cfg)
-        why = optimizer_refusal(dict(optim_name=optim_name, optim_cfg=cfg))
+        why = optimizer_refusal(dict(optim_name=optim_name, optim_cfg=cfg), type(self).__name__)
         if why:
             raise NotImplementedError(why)
         super().__init__(topk=topk, **kwargs)
@@ -259,56 +296,42 @@ class PoseOptimizer(animate.BasePoseGenerator):
         self.eps = float(cfg.get("eps", ADAM_EPS))
         self.last = {}
 
+    def _cams(self, eyes: np.ndarray) -> torch.Tensor:
+        """eyes [B, T, A, 3] -> each iteration's cameras [T, B A, cam_bytes] on the device."""
+        B, T = eyes.shape[0], eyes.shape[1]
+        return look_at_cams(np.ascontiguousarray(eyes.transpose(1, 0, 2, 3)), device=self.assets.device).view(
+            T, B * eyes.shape[2], -1)
+
     def optimise(self, init: torch.Tensor, text_feature: torch.Tensor, eyes: np.ndarray,
                  record_grad: bool = False) -> torch.Tensor:
         """num_iteration Adam steps of the poses init [B, 63]; eyes [B, num_iteration, A, 3] are row b's cameras per
         iteration.  Returns the poses [B, 63]; self.last holds each iteration's loss (and pose gradient)."""
         dev = self.assets.device
-        B, T, A = eyes.shape[0], eyes.shape[1], eyes.shape[2]
+        B, A = eyes.shape[0], eyes.shape[2]
         step = PoseStep(self.assets, B, A)
         step.set_text(text_feature.to(dev).float())
         step.pose.copy_(init.to(dev).float().reshape(B, POSE_DIM))
-        cams = look_at_cams(np.ascontiguousarray(eyes.transpose(1, 0, 2, 3)), device=dev).view(T, B * A, -1)
         m = torch.zeros_like(step.pose)
         v = torch.zeros_like(step.pose)
         state = torch.tensor([0.0, self.lr, 0.0, 0.0], device=dev)
-        losses = torch.empty(T, B, device=dev)
-        grads = torch.empty(T, B, POSE_DIM, device=dev) if record_grad else None
 
         def body():
             step.run()
-            _lib.check(_lib.lib().avc_adam_step_dev(_lib.ptr(step.pose), _lib.ptr(step.grad), _lib.ptr(m), _lib.ptr(v),
-                                                    step.pose.numel(), _lib.ptr(state), self.betas[0], self.betas[1],
-                                                    self.eps, 1.0, _lib.stream_ptr()), "avc_adam_step_dev")
+            adam_step(step.pose, step.grad, m, v, state, self.betas, self.eps)
 
-        # capture on a side stream after one forward and backward without the Adam step (first-launch set-up)
-        step.cams.copy_(cams[0])
-        side = torch.cuda.Stream(dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):
-            step.run()
-        torch.cuda.current_stream(dev).wait_stream(side)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            body()
-        for it in range(T):
-            step.cams.copy_(cams[it])
-            g.replay()
-            losses[it].copy_(step.loss)
-            if grads is not None:
-                grads[it].copy_(step.grad)
+        losses, grads = replay_iterations(step, self._cams(eyes), step.run, body, step.grad if record_grad else None)
         self.last = dict(loss=losses, grad=grads)
         return step.pose.clone()
 
     def get_topk_poses(self, text: str, init: Optional[torch.Tensor] = None,
                        text_feature: Optional[torch.Tensor] = None, record_grad: bool = False) -> torch.Tensor:
-        """:133-135 -> [topk, 69].  ``init`` [topk, 63] stands in for the topk torch.randn(63) draws and
+        """:133-135 -> [topk, 69].  ``init`` [topk, PARAM_DIM] stands in for the topk torch.randn(PARAM_DIM) draws and
         ``text_feature`` [512] for the CLIP text encode of ``text``.  Afterwards ``self.last`` holds the initial
-        poses, the eyes, each iteration's loss [num_iteration, topk] (and pose gradient) and the sort's scores."""
+        parameters, the eyes, each iteration's loss [num_iteration, topk] (and gradient) and the sort's scores."""
         tf = self.get_text_feature(text) if text_feature is None else text_feature.to(self.assets.device).float()
         if init is None:
-            init = torch.stack([torch.randn(POSE_DIM) for _ in range(self.topk)])
-        init = torch.as_tensor(init, dtype=torch.float32).reshape(self.topk, POSE_DIM)
+            init = torch.stack([torch.randn(self.PARAM_DIM) for _ in range(self.topk)])
+        init = torch.as_tensor(init, dtype=torch.float32).reshape(self.topk, self.PARAM_DIM)
         T = self.num_iteration
         eyes = self.scorer.draw_eyes(self.topk * T).reshape(self.topk, T, len(self.scorer.angles), 3)
         poses = self.optimise(init, tf, eyes, record_grad)
@@ -329,8 +352,8 @@ def refusal(conf) -> Optional[str]:
     if typ in animate.IN_SCOPE:
         return f"pose_generator.type = {typ}: this command runs PoseOptimizer; run python -m avatarclip_b200.animate"
     if typ == "VPoserOptimizer":
-        return ("pose_generator.type = VPoserOptimizer is not available: it needs the VPoser decoder's backward, which "
-                "is not built")
+        return ("pose_generator.type = VPoserOptimizer: this command runs PoseOptimizer; VPoserOptimizer optimises the "
+                "VPoser latent through the decoder's backward, so it runs as python -m avatarclip_b200.vposer_optimizer")
     if typ != "PoseOptimizer":
         return f"pose_generator.type = {typ!r} is unknown (this command runs PoseOptimizer)"
     return optimizer_refusal(pg)

@@ -681,6 +681,17 @@ int avc_vposer_decode(const float* z, int32_t B, int32_t latent, const float* W1
                       const float* W2, const float* b2, const float* W3, const float* b3, int32_t n_joints,
                       float* pose_out, float* rotmat_out, void* workspace, size_t workspace_bytes,
                       avc_stream_t stream);
+/* avc_vposer_decode_bwd is the backward of avc_vposer_decode with respect to z (the decoder's weights frozen): given
+ * g_pose [B][n_joints][3] = d loss / d pose_out, g_z_out [B][latent] = d loss / d z, autograd's gradient on the branches
+ * the forward took (LeakyReLU, F.normalize's clamp, rotation_matrix_to_quaternion's four masked branches,
+ * quaternion_to_angle_axis's atan2 and k branches).  The forward is recomputed with avc_vposer_decode's arithmetic;
+ * pose_out [B][n_joints][3] (or NULL) receives it, bit for bit avc_vposer_decode's.  Same size limits and workspace as
+ * avc_vposer_decode (avc_vposer_decode_bwd_workspace_bytes). */
+int avc_vposer_decode_bwd_workspace_bytes(int32_t latent, int32_t hidden, int32_t n_joints, size_t* bytes);
+int avc_vposer_decode_bwd(const float* z, int32_t B, int32_t latent, const float* W1, const float* b1, int32_t hidden,
+                          const float* W2, const float* b2, const float* W3, const float* b3, int32_t n_joints,
+                          const float* g_pose, float* g_z_out, float* pose_out, void* workspace, size_t workspace_bytes,
+                          avc_stream_t stream);
 int avc_realnvp_pack_floats(int32_t dim, int32_t hidden, int32_t n_blocks, size_t* floats);
 int avc_realnvp_pack(const float* params, int32_t dim, int32_t feat_dim, int32_t hidden, int32_t n_blocks, float* pack,
                      avc_stream_t stream);
