@@ -39,13 +39,21 @@ The file:
     TEXCOORD_0 (origin at the top left) and no COLOR_0.  The material's baseColorTexture is a PNG in a buffer view,
     its bytes the sRGB ``to8b`` bytes the PLY holds; the sampler is LINEAR without mipmaps (a face's footprint never
     leaves its own texels) and CLAMP_TO_EDGE.
+  * Normal map (with ``--normal_map``, which needs ``--conf``): ``bake.bake_normal_map`` bakes the SDF's normals in
+    each texel's tangent frame on the same atlas.  The primitive also has TANGENT (float VEC4, per corner,
+    ``bake.corner_tangents`` of the bind pose's positions and NORMALs; w = +-1 so that w cross(N, T) points towards
+    the image's top, glTF's "+Y up"), a second PNG (linear data, no sRGB) and the material's normalTexture
+    {index 1, texCoord 0}.  The map is baked in the PLY frame.  The rotation into SMPL's frame is proper, so its
+    tangent-space values carry over exactly; the un-posing is linear-blend skinning, under which they carry over to
+    first order, the standard assumption of a skinned normal map.
 
 Left out: FBX itself (it needs Autodesk's proprietary SDK; Blender converts the .glb to FBX), the reference's all-zero
 blend shape, non-zero beta (Avatar2FBX fixes beta = 0) and ``cleanup_mesh`` (Avatar2FBX does not run it).
 
     python -m avatarclip_b200.export --mesh exp/.../meshes/00029500.ply --smpl smpl.npz \\
         --stand_pose stand_pose.npy [--motion action.npy --fps 30] [--target_faces 20000] --out avatar.glb \\
-        [--conf confs/examples/hulk.conf [--case smpl] [--checkpoint ckpt_030000.pth] [--texture_size 2048]]
+        [--conf confs/examples/hulk.conf [--case smpl] [--checkpoint ckpt_030000.pth] [--texture_size 2048]
+         [--normal_map]]
 """
 from __future__ import annotations
 
@@ -272,11 +280,14 @@ class _Glb:
         return len(self.views) - 1
 
 
-def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 30, texture=None) -> str:
+def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 30, texture=None,
+              normal_map=None) -> str:
     """Write ``rig`` (``rig_avatar``'s dictionary; host arrays or tensors) as a glTF 2.0 binary at ``path``; with
     ``motion_npy`` (rows [F, >= 72] of SMPL axis-angle, as ``drive`` reads them) also one animation of F keys at
     ``fps``; with ``texture`` = (uv [3T,2], image uint8 [H,W,3] RGB), ``bake.bake_texture``'s result, a textured
-    primitive, which also needs ``rig["normals"]`` [N,3].  Layout in the module docstring.  Returns ``path``."""
+    primitive, which also needs ``rig["normals"]`` [N,3]; with ``normal_map`` = (tangents [3T,4], image uint8
+    [H,W,3]), ``bake.corner_tangents`` and ``bake.bake_normal_map``'s image, also TANGENT and a normalTexture (it
+    needs ``texture``).  Layout in the module docstring.  Returns ``path``."""
     FLOAT, UINT, UBYTE = 5126, 5125, 5121
     pos = _np(rig["vertices"]).astype(np.float32).reshape(-1, 3)
     tri = _np(rig["triangles"]).astype(np.uint32).reshape(-1, 3)
@@ -290,6 +301,14 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
     if fps <= 0:
         raise ValueError(f"write_glb: fps must be > 0, got {fps}")
     motion = None if motion_npy is None else drive._motion_axis_angle(motion_npy)
+    if normal_map is not None:
+        if texture is None:
+            raise ValueError("write_glb: a normal map needs the colour texture (texture=)")
+        tangents = _np(normal_map[0]).astype(np.float32).reshape(-1, 4)
+        nmap = np.asarray(_np(normal_map[1]), dtype=np.uint8)
+        if tangents.shape[0] != tri.size or nmap.ndim != 3 or nmap.shape[2] != 3:
+            raise ValueError(f"write_glb: normal_map needs tangents [{tri.size}, 4] and an RGB image [H, W, 3], got "
+                             f"tangents {list(tangents.shape)}, image {list(nmap.shape)}")
 
     if texture is not None:
         uv, image = _np(texture[0]).astype(np.float32).reshape(-1, 2), np.asarray(_np(texture[1]), dtype=np.uint8)
@@ -307,6 +326,8 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
     if texture is not None:
         attrs["NORMAL"] = g.add(normals, FLOAT, "VEC3", 34962)
         attrs["TEXCOORD_0"] = g.add(uv, FLOAT, "VEC2", 34962)
+        if normal_map is not None:
+            attrs["TANGENT"] = g.add(tangents, FLOAT, "VEC4", 34962)
     elif rig.get("colors") is not None:
         col = srgb_to_linear(np.clip(_np(rig["colors"]).reshape(-1, 3), 0.0, 1.0)).astype(np.float32)
         attrs["COLOR_0"] = g.add(col, FLOAT, "VEC3", 34962)
@@ -349,6 +370,10 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
         gltf["textures"] = [{"sampler": 0, "source": 0}]
         gltf["samplers"] = [{"magFilter": 9729, "minFilter": 9729, "wrapS": 33071, "wrapT": 33071}]   # LINEAR, CLAMP
         gltf["images"] = [{"bufferView": png, "mimeType": "image/png"}]
+        if normal_map is not None:
+            gltf["materials"][0]["normalTexture"] = {"index": 1, "texCoord": 0}
+            gltf["textures"].append({"sampler": 0, "source": 1})
+            gltf["images"].append({"bufferView": g.add_bytes(bake.encode_png(nmap)), "mimeType": "image/png"})
     if motion is not None:
         q = axis_angle_to_quat(motion[:, 3:3 * nj].reshape(motion.shape[0], nj - 1, 3))     # [F, nj-1, 4]
         for k in range(1, q.shape[0]):                                 # short arc between successive keys
@@ -378,17 +403,18 @@ def write_glb(rig: dict, path: str, motion_npy: str | None = None, fps: float = 
 def export_avatar(mesh_ply: str, out_glb: str, smpl, stand_pose_npy: str, motion_npy: str | None = None,
                   fps: float = 30, resolution: int = DEFAULT_RESOLUTION, device="cuda", conf: str | None = None,
                   case: str = "smpl", checkpoint: str | None = None, texture_size: int | None = None,
-                  target_faces: int | None = None) -> str:
+                  target_faces: int | None = None, normal_map: bool = False) -> str:
     """``rig_avatar`` + ``write_glb``: the .glb of one PLY, optionally animated by ``motion_npy``.  With ``conf`` (the
     NeuS run's conf) the mesh also gets a texture of ``texture_size`` (default ``bake.DEFAULT_TEXTURE_SIZE``) baked
     from the run's colour field: the Runner is built as ``--mode validate_mesh`` builds it (its last checkpoint), or
     from ``checkpoint`` (a path, or a name under the run's checkpoints directory).  ``target_faces`` bounds the
-    faces (``reduce_mesh``); the texture atlas is then sized for the reduced mesh.  When decimation stops above the target, one line on stderr says how many faces it reached.  Returns the
-    path."""
+    faces (``reduce_mesh``); the texture atlas is then sized for the reduced mesh.  When decimation stops above the target, one line on stderr says how many faces it reached.  ``normal_map`` (needs
+    ``conf``) also bakes a tangent-space normal map from the run's SDF (``bake.bake_normal_map``); one line on stderr
+    counts its flat and back-facing texels when there are any.  Returns the path."""
     if target_faces is not None and target_faces < 1:
         raise ValueError(f"export_avatar: target_faces must be >= 1, got {target_faces}")
-    if conf is None and (checkpoint is not None or texture_size is not None):
-        raise ValueError("export_avatar: checkpoint and texture_size need conf (the NeuS run to bake from)")
+    if conf is None and (checkpoint is not None or texture_size is not None or normal_map):
+        raise ValueError("export_avatar: checkpoint, texture_size and normal_map need conf (the NeuS run to bake from)")
     if motion_npy is not None:
         drive._motion_axis_angle(motion_npy)           # reject a bad motion before the GPU work
     rig = rig_avatar(mesh_ply, smpl, stand_pose_npy, resolution, device, ply_frame=conf is not None,
@@ -407,9 +433,18 @@ def export_avatar(mesh_ply: str, out_glb: str, smpl, stand_pose_npy: str, motion
         texture = bake.bake_texture(runner, rig["vertices_ply"], rig["triangles"], T)
         rig["normals"] = bake.vertex_normals(torch.from_numpy(rig["vertices"]).to(_cuda(device)),
                                              torch.from_numpy(rig["triangles"])).cpu().numpy()
+    nmap = None
+    if normal_map:
+        image, stats = bake.bake_normal_map(runner, rig["vertices_ply"], rig["triangles"], T)
+        tangents = bake.corner_tangents(torch.from_numpy(rig["vertices"]).to(_cuda(device)), rig["triangles"],
+                                        torch.from_numpy(rig["normals"]), texture[0])
+        nmap = (tangents.cpu().numpy().reshape(-1, 4), image)
+        if stats["flat"] or stats["back_facing"]:
+            print(f"export: normal map: {stats['flat']} of {stats['used']} texels flat (no zero crossing within the "
+                  f"search, or a vanishing gradient), {stats['back_facing']} back-facing", file=sys.stderr)
     out_dir = os.path.dirname(os.path.abspath(out_glb))
     os.makedirs(out_dir, exist_ok=True)
-    return write_glb(rig, out_glb, motion_npy, fps, texture=texture)
+    return write_glb(rig, out_glb, motion_npy, fps, texture=texture, normal_map=nmap)
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -439,6 +474,8 @@ def build_parser() -> argparse.ArgumentParser:
                    help="ckpt_XXXXXX.pth under the run's checkpoints directory, or a path (default: the last one)")
     t.add_argument("--texture_size", type=int, default=None,
                    help=f"texels per side of the square texture (default {bake.DEFAULT_TEXTURE_SIZE})")
+    t.add_argument("--normal_map", action="store_true",
+                   help="also bake a tangent-space normal map from the run's SDF (glTF normalTexture and TANGENT)")
     return p
 
 
@@ -446,7 +483,8 @@ def main(argv=None) -> int:
     parser = build_parser()
     a = parser.parse_args(argv)
     if a.conf is None:
-        for flag, val in (("--case", a.case), ("--checkpoint", a.checkpoint), ("--texture_size", a.texture_size)):
+        for flag, val in (("--case", a.case), ("--checkpoint", a.checkpoint), ("--texture_size", a.texture_size),
+                          ("--normal_map", a.normal_map or None)):
             if val is not None:
                 parser.error(f"{flag} needs --conf (the NeuS run to bake the texture from)")
     if a.target_faces is not None and a.target_faces < 1:
@@ -480,7 +518,7 @@ def main(argv=None) -> int:
     try:
         out = export_avatar(a.mesh, a.out, smpl, a.stand_pose, a.motion, a.fps, a.resolution, a.device, conf=a.conf,
                             case=a.case or "smpl", checkpoint=a.checkpoint, texture_size=a.texture_size,
-                            target_faces=a.target_faces)
+                            target_faces=a.target_faces, normal_map=a.normal_map)
     except bake.AtlasTooSmall as e:
         parser.error(f"--texture_size: {e}")
     print(out)

@@ -948,6 +948,64 @@ int avc_bake_vertex_normals(const float* verts, const int32_t* faces, const int3
                             int32_t V, int32_t F, float* normals, avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Tangent-space normal map of the atlas (bake.bake_normal_map): per used texel the SDF's normal at the zero set near
+ * the texel's surface point, in the texel's (T, B, N) frame, as glTF's normalTexture.  float32 throughout; each entry
+ * point only launches (no allocation, no host sync); AVC_E_NULL for a missing pointer, AVC_E_SIZE for a bad size.
+ *
+ * avc_bake_corner_tangents: tangents [F][3][4], one per face corner.  Face f has positions P0, P1, P2 and corner UVs
+ * (u_k, v_k) = uv[f][k] (avc_bake_texel_points' uv); e1 = P1 - P0, e2 = P2 - P0, du1 = u1 - u0, dv1 = v1 - v0,
+ * du2 = u2 - u0, dv2 = v2 - v0, det = du1 dv2 - du2 dv1, s = -1 if det < 0 else 1.  t_f = s (e1 dv2 - e2 dv1) and
+ * b_f = s (e2 du1 - e1 du2) are dP/du and dP/dv times |det|.  At corner k with the unit normal n = normals[v_k]:
+ *   - xyz: o = t_f - (t_f . n) n, normalised; when |o| <= 1e-6 |t_f| (a degenerate position or UV triangle) the unit
+ *     axis e of n's smallest |component| (x before y before z on a tie) is used instead of t_f.
+ *   - w = -1 when det != 0 and cross(n, T) . b_f > 0, else +1: the bitangent B = w cross(N, T) points along decreasing
+ *     v (towards the top row of the image), glTF's "+Y up" for normalTexture.  The atlas mirrors face 2k + 1 across its
+ *     cell's diagonal, so for a face whose smooth normals agree with its winding w = -1 on faces 2k, +1 on 2k + 1.
+ *   Every face is its own UV island in the atlas, so this is what MikkTSpace computes on the split-corner mesh (its
+ *   per-island averaging has one face to average).  1 <= V, 1 <= F <= 2^29.
+ *
+ * avc_bake_texel_frames: frames [n][3][3], rows T, B, N, of texel texels[i] (index y T + x), taken with the clamped
+ * barycentrics (b0, b1, b2) avc_bake_texel_points uses for the texel's point (the same device code):
+ *   N = normalise(sum b_k normals[v_k]) ((0, 1, 0) when the sum is 0); T = (sum b_k tangents[f][k].xyz) Gram-Schmidt'd
+ *   against N with the corner tangents' fallback; B = w cross(N, T), w = +1 if sum b_k tangents[f][k].w >= 0 else -1.
+ *   An unused texel (or an index outside [0, T^2)) gets an all-0 frame.  The decode of a texel's bytes (r, g, b):
+ *   (x, y, z) = 2 byte / 255 - 1 and n = normalise(T x + B y + N z).  V, n >= 1; F, T as avc_bake_atlas_grid.
+ *
+ * The snap: each texel searches its segment p + t N, t in [-D, D] (p its avc_bake_texel_points point, N its frame's
+ * normal), for the SDF's zero set.  bracket [n][2] = (lo, hi) offsets and state [n] (0: no root; 1: sdf(lo) < 0;
+ * 2: sdf(lo) > 0) carry the search; the caller evaluates avc_neus_sdf_query on the points these entry points write.
+ * Every step is per texel, so with avc_neus_sdf_query's placement-independent bits the result does not depend on how
+ * the texels are chunked.  D finite and > 0, else AVC_E_BADCFG.
+ *   avc_bake_snap_samples: samples [n][16][3], sample k at t_k = float(2k - 15) * D / 15 (float32, in that order).
+ *   avc_bake_snap_bracket: from sdf [n][16] at those samples.  Candidates on the scale q = 0 .. 30: sample k (q = 2k)
+ *     when its sdf is exactly 0, the interval [t_k, t_k+1] (q = 2k + 1) when its ends have strictly opposite signs
+ *     (NaN is neither).  The winner has the least |q - 15| (nearest t = 0), the larger q (the outside, +t) on a tie.
+ *     An interval gives (t_k, t_k+1) and state 1 or 2 by the sign of sdf(t_k); a zero sample (t_k, t_k) and state 1;
+ *     none (0, 0) and state 0.
+ *   avc_bake_snap_midpoints: out [n][3] = p + m N, m = (lo + hi) * 0.5.  After the last bisection these are the
+ *     snapped points.
+ *   avc_bake_snap_bisect: from sdf_mid [n] at the midpoints: state 0 is left alone; sdf(m) = 0 sets lo = hi = m; else
+ *     lo = m when sdf(m) has the sign of sdf(lo) (state), hi = m otherwise.  bake.py runs 12 steps.
+ * avc_bake_normal_encode: from grad [n][3] (avc_neus_sdf_eval's gradient at the snapped points), writes the 3 bytes of
+ *   texel texels[i] of image [T][T][3] (other texels untouched).  State 0 or |grad| < 1e-6 (or NaN): (128, 128, 255),
+ *   counted in counts[0].  Else n = grad / |grad|, c = (T . n, B . n, N . n), bytes min(max(rint(127.5 c + 127.5), 0),
+ *   255), counted in counts[1] when c.z <= 0 (the SDF's normal faces away from the mesh's).  counts [2] (DEVICE) is
+ *   zeroed first; integer atomics only.  1 <= n, 1 <= T <= 16384.
+ * ------------------------------------------------------------------------------------------ */
+int avc_bake_corner_tangents(const float* verts, const int32_t* faces, const float* normals, const float* uv,
+                             int32_t V, int32_t F, float* tangents, avc_stream_t stream);
+int avc_bake_texel_frames(const int32_t* faces, const float* normals, const float* tangents, int32_t V, int32_t F,
+                          int32_t T, const int32_t* texels, int32_t n, float* frames, avc_stream_t stream);
+int avc_bake_snap_samples(const float* points, const float* frames, int32_t n, float D, float* samples,
+                          avc_stream_t stream);
+int avc_bake_snap_bracket(const float* sdf, int32_t n, float D, float* bracket, int32_t* state, avc_stream_t stream);
+int avc_bake_snap_midpoints(const float* points, const float* frames, const float* bracket, int32_t n, float* out,
+                            avc_stream_t stream);
+int avc_bake_snap_bisect(const float* sdf_mid, int32_t n, float* bracket, const int32_t* state, avc_stream_t stream);
+int avc_bake_normal_encode(const float* frames, const float* grad, const int32_t* state, const int32_t* texels,
+                           int32_t n, int32_t T, uint8_t* image, int32_t* counts, avc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Mesh decimation (avatarclip_b200/export.py, decimate_mesh): quadric-error edge collapse (Garland & Heckbert 1997)
  * to target_faces, in rounds of independent collapses.  oracle/decimate.py restates it in fp64 numpy.
  *
