@@ -21,8 +21,6 @@ constexpr int kThreads = 256;
 constexpr int kMinCell = 8;          // texels per cell side: the two inset triangles need legs of at least 4 texels
 constexpr int kMaxTexture = 16384;   // T * T texel indices fit int32
 
-inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // m = ceil(sqrt(ceil(F / 2))) in integers
 int grid_side(int32_t F) {
   const long long n = ((long long)F + 1) / 2;
@@ -356,8 +354,8 @@ int avc_bake_texel_points(const float* verts, const int32_t* faces, int32_t V, i
   AVC_TRY(avc_bake_atlas_grid(F, T, &m, &c));
   cudaStream_t st = (cudaStream_t)stream;
   const Atlas a{F, V, T, m, c};
-  k_bake_texel<<<blocks((long long)T * T, kThreads), kThreads, 0, st>>>(verts, faces, a, owner, points);
-  if (uv) k_bake_uv<<<blocks(F, kThreads), kThreads, 0, st>>>(a, uv);
+  k_bake_texel<<<ceil_div((long long)T * T, kThreads), kThreads, 0, st>>>(verts, faces, a, owner, points);
+  if (uv) k_bake_uv<<<ceil_div(F, kThreads), kThreads, 0, st>>>(a, uv);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -366,7 +364,7 @@ int avc_bake_vertex_normals(const float* verts, const int32_t* faces, const int3
                             int32_t V, int32_t F, float* normals, avc_stream_t stream) {
   if (!verts || !faces || !offsets || !vf || !normals) return AVC_E_NULL;
   if (V < 1 || F < 1 || F > (1 << 29)) return AVC_E_SIZE;
-  k_bake_normals<<<blocks(V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(verts, faces, offsets, vf, V, normals);
+  k_bake_normals<<<ceil_div(V, kThreads), kThreads, 0, (cudaStream_t)stream>>>(verts, faces, offsets, vf, V, normals);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -375,7 +373,7 @@ int avc_bake_corner_tangents(const float* verts, const int32_t* faces, const flo
                              int32_t V, int32_t F, float* tangents, avc_stream_t stream) {
   if (!verts || !faces || !normals || !uv || !tangents) return AVC_E_NULL;
   if (V < 1 || F < 1 || F > (1 << 29)) return AVC_E_SIZE;
-  k_bake_tangents<<<blocks(F, kThreads), kThreads, 0, (cudaStream_t)stream>>>(verts, faces, normals, uv, F, tangents);
+  k_bake_tangents<<<ceil_div(F, kThreads), kThreads, 0, (cudaStream_t)stream>>>(verts, faces, normals, uv, F, tangents);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -387,8 +385,8 @@ int avc_bake_texel_frames(const int32_t* faces, const float* normals, const floa
   int32_t m = 0, c = 0;
   AVC_TRY(avc_bake_atlas_grid(F, T, &m, &c));
   const Atlas a{F, V, T, m, c};
-  k_bake_frames<<<blocks(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(faces, normals, tangents, a, texels, n,
-                                                                             frames);
+  k_bake_frames<<<ceil_div(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(faces, normals, tangents, a, texels, n,
+                                                                               frames);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -400,8 +398,8 @@ int avc_bake_snap_samples(const float* points, const float* frames, int32_t n, f
   if (!points || !frames || !samples) return AVC_E_NULL;
   if (n < 1) return AVC_E_SIZE;
   if (!snap_d_ok(D)) return AVC_E_BADCFG;
-  k_snap_samples<<<blocks((long long)n * kSnapSamples, kThreads), kThreads, 0, (cudaStream_t)stream>>>(points, frames,
-                                                                                                    n, D, samples);
+  k_snap_samples<<<ceil_div((long long)n * kSnapSamples, kThreads), kThreads, 0, (cudaStream_t)stream>>>(points, frames,
+                                                                                                      n, D, samples);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -410,7 +408,7 @@ int avc_bake_snap_bracket(const float* sdf, int32_t n, float D, float* bracket, 
   if (!sdf || !bracket || !state) return AVC_E_NULL;
   if (n < 1) return AVC_E_SIZE;
   if (!snap_d_ok(D)) return AVC_E_BADCFG;
-  k_snap_bracket<<<blocks(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(sdf, n, D, (float2*)bracket, state);
+  k_snap_bracket<<<ceil_div(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(sdf, n, D, (float2*)bracket, state);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -419,8 +417,8 @@ int avc_bake_snap_midpoints(const float* points, const float* frames, const floa
                             avc_stream_t stream) {
   if (!points || !frames || !bracket || !out) return AVC_E_NULL;
   if (n < 1) return AVC_E_SIZE;
-  k_snap_midpoints<<<blocks(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(points, frames, (const float2*)bracket,
-                                                                                n, out);
+  k_snap_midpoints<<<ceil_div(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(points, frames, (const float2*)bracket,
+                                                                                  n, out);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -428,7 +426,7 @@ int avc_bake_snap_midpoints(const float* points, const float* frames, const floa
 int avc_bake_snap_bisect(const float* sdf_mid, int32_t n, float* bracket, const int32_t* state, avc_stream_t stream) {
   if (!sdf_mid || !bracket || !state) return AVC_E_NULL;
   if (n < 1) return AVC_E_SIZE;
-  k_snap_bisect<<<blocks(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(sdf_mid, n, (float2*)bracket, state);
+  k_snap_bisect<<<ceil_div(n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(sdf_mid, n, (float2*)bracket, state);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -439,8 +437,8 @@ int avc_bake_normal_encode(const float* frames, const float* grad, const int32_t
   if (n < 1 || T < 1 || T > kMaxTexture) return AVC_E_SIZE;
   cudaStream_t st = (cudaStream_t)stream;
   AVC_CUDA_TRY(cudaMemsetAsync(counts, 0, 2 * sizeof(int32_t), st));
-  k_normal_encode<<<blocks(n, kThreads), kThreads, 0, st>>>(frames, grad, state, texels, n, (unsigned)T * (unsigned)T,
-                                                            image, counts);
+  k_normal_encode<<<ceil_div(n, kThreads), kThreads, 0, st>>>(frames, grad, state, texels, n, (unsigned)T * (unsigned)T,
+                                                              image, counts);
   AVC_LAUNCH_TRY();
   return 0;
 }

@@ -6,13 +6,15 @@
 //                      reduced values, no host round trip), packed 21 bits per axis into a 64-bit key
 //   k_cl_vinsert       open-addressing table of vertex ids keyed by voxel: CAS an empty slot, or atomicMin the id into
 //                      the slot of the same voxel, so each slot ends holding the first vertex of its voxel
-//   k_cl_vflag + scan  the first vertex of each voxel numbers its output vertex: an ordered exclusive scan
+//   k_cl_flag          flags the first vertex of each voxel; exclusive_scan (avc_scan.cu, in index order) of the flags
+//                      numbers the output vertices
 //   k_cl_vaccum/final  fp64 position sums (exact for float32 inputs at mesh scale, so order-independent) and integer
 //                      colour sums by atomics, then the means
 //   k_cl_tremap        triangles to output vertices; two corners in one voxel -> dropped
 //   k_cl_tinsert       the same table scheme keyed by the rotation that puts the smallest index first: each slot ends
 //                      holding the first triangle of its rotation class (a reversed triangle is another class)
-//   k_cl_tflag + scan  kept triangles compacted in input order, each in the rotation it first appeared in
+//   k_cl_flag/temit    kept triangles compacted in input order by exclusive_scan, each in the rotation it first
+//                      appeared in
 // Every stage is linear in V + F: no per-vertex or per-voxel loops over neighbours, so a fan of many triangles around one
 // vertex or many vertices in one voxel costs no more than spread-out ones.
 #include "avc_common.cuh"
@@ -22,13 +24,10 @@ using namespace avc;
 namespace {
 
 constexpr int CL_THREADS = 256;
-constexpr int SCAN_ITEMS = 8, SCAN_TILE = CL_THREADS * SCAN_ITEMS, SCAN_TOP = 1024;
 constexpr int KEY_BITS = 21;                                  // per axis; the largest voxel index is resolution + 1
 constexpr int KEY_MAX = (1 << KEY_BITS) - 1;
 constexpr int MAX_RESOLUTION = KEY_MAX - 1;
 constexpr int MAX_ELEMS = 1 << 30;                             // tables of 2^31 slots still index with int
-
-inline int blocks(long long n, int t) { return (int)((n + t - 1) / t); }
 
 __device__ __forceinline__ int f2o(float f) {                  // float order == int order
   const int i = __float_as_int(f);
@@ -128,81 +127,6 @@ k_cl_flag(const int* __restrict__ slot, const int* __restrict__ tab, int n, int*
   if (i >= n) return;
   const int s = slot[i];
   flag[i] = (s >= 0 && tab[s] == i) ? 1 : 0;
-}
-
-// ---------------------------------------------------------------- ordered exclusive scan of 0/1 flags (in place)
-template <int NT>
-__device__ __forceinline__ int block_exclusive_scan(int x, int* warp_tot, int& total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  int inc = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += y;
-  }
-  __syncthreads();                      // warp_tot may still be read by a previous call
-  if (lane == 31) warp_tot[w] = inc;
-  __syncthreads();
-  if (w == 0) {
-    int t = lane < NT / 32 ? warp_tot[lane] : 0, ti = t;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, ti, o);
-      if (lane >= o) ti += y;
-    }
-    if (lane < NT / 32) warp_tot[lane] = ti - t;
-    if (lane == 31) warp_tot[32] = ti;
-  }
-  __syncthreads();
-  total = warp_tot[32];
-  return warp_tot[w] + inc - x;
-}
-
-__global__ void __launch_bounds__(CL_THREADS) k_scan_reduce(const int* __restrict__ a, int n, int* __restrict__ sums) {
-  __shared__ int wt[33];
-  const long long base = (long long)blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-  int s = 0;
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; ++k) s += base + k < n ? a[base + k] : 0;
-  int total;
-  block_exclusive_scan<CL_THREADS>(s, wt, total);
-  if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(SCAN_TOP) k_scan_top(int* sums, int nb, int32_t* total_out) {
-  __shared__ int wt[33];
-  int carry = 0;
-  for (int c0 = 0; c0 < nb; c0 += SCAN_TOP) {
-    const int i = c0 + threadIdx.x;
-    const int x = i < nb ? sums[i] : 0;
-    int total;
-    const int ex = block_exclusive_scan<SCAN_TOP>(x, wt, total);
-    if (i < nb) sums[i] = carry + ex;
-    carry += total;
-  }
-  if (threadIdx.x == 0) *total_out = carry;
-}
-
-__global__ void __launch_bounds__(CL_THREADS) k_scan_down(int* a, int n, const int* __restrict__ sums) {
-  __shared__ int wt[33];
-  const long long base = (long long)blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-  int x[SCAN_ITEMS], s = 0;
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; ++k) { x[k] = base + k < n ? a[base + k] : 0; s += x[k]; }
-  int total;
-  int run = sums[blockIdx.x] + block_exclusive_scan<CL_THREADS>(s, wt, total);
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; ++k) {
-    if (base + k < n) a[base + k] = run;
-    run += x[k];
-  }
-}
-
-void exclusive_scan(int* a, int n, int* sums, int32_t* total, cudaStream_t st) {
-  const int nb = blocks(n, SCAN_TILE);
-  k_scan_reduce<<<nb, CL_THREADS, 0, st>>>(a, n, sums);
-  k_scan_top<<<1, SCAN_TOP, 0, st>>>(sums, nb, total);
-  k_scan_down<<<nb, CL_THREADS, 0, st>>>(a, n, sums);
 }
 
 // ---------------------------------------------------------------- vertex means
@@ -318,7 +242,7 @@ Layout layout(int V, int F) {
   L.ttab = take(ht * sizeof(int));
   L.tslot = take((size_t)F * sizeof(int));
   L.tscan = take((size_t)F * sizeof(int));
-  L.scan_sums = take((size_t)blocks((V > F ? V : F), SCAN_TILE) * sizeof(int));
+  L.scan_sums = take(exclusive_scan_sums(V > F ? V : F) * sizeof(int));
   L.total = off;
   return L;
 }
@@ -360,22 +284,22 @@ int avc_mesh_cluster(const float* verts, const uint8_t* colors, int32_t V, const
   AVC_CUDA_TRY(cudaMemsetAsync(vtab, 0xff, (size_t)(L.vmask + 1) * sizeof(int), st));
   AVC_CUDA_TRY(cudaMemsetAsync(sums, 0, L.csum + (size_t)V * 3 * sizeof(unsigned) - L.sums, st));  // sums, cnt, csum
   k_cl_init<<<1, 32, 0, st>>>(bounds, counts);
-  k_cl_bounds<<<min(blocks(V, CL_THREADS), 264), CL_THREADS, 0, st>>>(verts, V, bounds);
-  k_cl_vkey<<<blocks(V, CL_THREADS), CL_THREADS, 0, st>>>(verts, V, bounds, resolution, vkey);
-  k_cl_vinsert<<<blocks(V, CL_THREADS), CL_THREADS, 0, st>>>(vkey, V, vtab, L.vmask, vslot);
-  k_cl_flag<<<blocks(V, CL_THREADS), CL_THREADS, 0, st>>>(vslot, vtab, V, vscan);
+  k_cl_bounds<<<min(ceil_div(V, CL_THREADS), 264), CL_THREADS, 0, st>>>(verts, V, bounds);
+  k_cl_vkey<<<ceil_div(V, CL_THREADS), CL_THREADS, 0, st>>>(verts, V, bounds, resolution, vkey);
+  k_cl_vinsert<<<ceil_div(V, CL_THREADS), CL_THREADS, 0, st>>>(vkey, V, vtab, L.vmask, vslot);
+  k_cl_flag<<<ceil_div(V, CL_THREADS), CL_THREADS, 0, st>>>(vslot, vtab, V, vscan);
   exclusive_scan(vscan, V, scan_sums, counts, st);
-  k_cl_vaccum<<<blocks(V, CL_THREADS), CL_THREADS, 0, st>>>(verts, colors, V, vslot, vtab, vscan, vcl, sums, cnt,
-                                                            csum);
-  k_cl_vfinal<<<blocks(V, CL_THREADS), CL_THREADS, 0, st>>>(sums, cnt, csum, counts, verts_out,
-                                                            colors ? colors_out : nullptr);
+  k_cl_vaccum<<<ceil_div(V, CL_THREADS), CL_THREADS, 0, st>>>(verts, colors, V, vslot, vtab, vscan, vcl, sums, cnt,
+                                                              csum);
+  k_cl_vfinal<<<ceil_div(V, CL_THREADS), CL_THREADS, 0, st>>>(sums, cnt, csum, counts, verts_out,
+                                                              colors ? colors_out : nullptr);
   if (F > 0) {
     AVC_CUDA_TRY(cudaMemsetAsync(ttab, 0xff, (size_t)(L.tmask + 1) * sizeof(int), st));
-    k_cl_tremap<<<blocks(F, CL_THREADS), CL_THREADS, 0, st>>>(tris, F, V, vcl, rtri);
-    k_cl_tinsert<<<blocks(F, CL_THREADS), CL_THREADS, 0, st>>>(rtri, F, ttab, L.tmask, tslot);
-    k_cl_flag<<<blocks(F, CL_THREADS), CL_THREADS, 0, st>>>(tslot, ttab, F, tscan);
+    k_cl_tremap<<<ceil_div(F, CL_THREADS), CL_THREADS, 0, st>>>(tris, F, V, vcl, rtri);
+    k_cl_tinsert<<<ceil_div(F, CL_THREADS), CL_THREADS, 0, st>>>(rtri, F, ttab, L.tmask, tslot);
+    k_cl_flag<<<ceil_div(F, CL_THREADS), CL_THREADS, 0, st>>>(tslot, ttab, F, tscan);
     exclusive_scan(tscan, F, scan_sums, counts + 1, st);
-    k_cl_temit<<<blocks(F, CL_THREADS), CL_THREADS, 0, st>>>(rtri, tslot, ttab, tscan, F, tris_out);
+    k_cl_temit<<<ceil_div(F, CL_THREADS), CL_THREADS, 0, st>>>(rtri, tslot, ttab, tscan, F, tris_out);
   }
   AVC_LAUNCH_TRY();
   return 0;

@@ -82,6 +82,75 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// x reduced over the CTA by op, the result in every thread: an xor tree in each warp, then the warp results folded onto
+// init in warp order.  The fold order is fixed, so a floating-point sum is the same on every run; init decides the sign
+// of a zero sum.  red holds blockDim.x / 32 values (blockDim.x a multiple of 32).
+template <class T, class Op>
+__device__ __forceinline__ T block_reduce(T x, T* red, Op op, T init) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x = op(x, __shfl_xor_sync(0xffffffffu, x, o));
+  __syncthreads();                      // red may still be read by a previous call
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
+  __syncthreads();
+  for (int w = 0, nw = blockDim.x >> 5; w < nw; ++w) init = op(init, red[w]);
+  return init;
+}
+
+// The exclusive prefix sum of x over the CTA's NT threads in thread order, and in total the CTA's sum.  warp_tot holds
+// 33 ints.
+template <int NT>
+__device__ __forceinline__ int block_exclusive_scan(int x, int* warp_tot, int& total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int inc = x;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  __syncthreads();                      // warp_tot may still be read by a previous call
+  if (lane == 31) warp_tot[w] = inc;
+  __syncthreads();
+  if (w == 0) {
+    int t = lane < NT / 32 ? warp_tot[lane] : 0, ti = t;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, ti, o);
+      if (lane >= o) ti += y;
+    }
+    if (lane < NT / 32) warp_tot[lane] = ti - t;
+    if (lane == 31) warp_tot[32] = ti;
+  }
+  __syncthreads();
+  total = warp_tot[32];
+  return warp_tot[w] + inc - x;
+}
+
+// avc_scan.cu: the in-place exclusive scan of a[0, n) (n >= 1) in index order over the whole device, and the sum of a
+// to *total.  sums is a workspace of exclusive_scan_sums(n) ints.
+size_t exclusive_scan_sums(int n);
+void exclusive_scan(int* a, int n, int* sums, int32_t* total, cudaStream_t st);
+
+// float -> uint32 whose unsigned order is the float order
+__device__ __forceinline__ unsigned ordered_bits(float f) {
+  unsigned u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// key = (ordered value bits, ~index): the larger key is the larger value, on ties the smaller index (a 64-bit atomicMax
+// or max reduction selects the first argmax); sel_index decodes the index
+__device__ __forceinline__ unsigned long long sel_key(float v, int i) {
+  return ((unsigned long long)ordered_bits(v) << 32) | (unsigned)(0xffffffffu - (unsigned)i);
+}
+__device__ __forceinline__ int sel_index(unsigned long long key) {
+  return (int)(0xffffffffu - (unsigned)(key & 0xffffffffu));
+}
+
+// key = (bits of z, id) for z >= 0 (a depth, a collapse cost): the smaller key is the smaller z, on ties the smaller
+// id, so a 64-bit atomicMin keeps the nearest
+__device__ __forceinline__ unsigned long long depth_key(float z, int id) {
+  return ((unsigned long long)__float_as_uint(z) << 32) | (unsigned)id;
+}
+
 // A carve-out allocator over the caller-provided workspace (256-byte aligned pieces).
 struct Carver {
   char* base;

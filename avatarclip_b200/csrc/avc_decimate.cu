@@ -12,7 +12,8 @@
 //   k_dc_cap         one block: the longest prefix of the selection in key order that removes no more faces than allowed
 //   k_dc_apply       the collapses (their neighbourhoods are disjoint, so no two touch the same vertex or face)
 //   k_dc_filter      the live faces that remain, and the next round's gathered faces
-//   k_dc_flag_* + k_dc_scan + k_dc_emit   surviving vertices and faces compacted in input order
+//   k_dc_flag_v + exclusive_scan + k_dc_emit_*   surviving vertices and faces compacted in input order by the
+//                    device-wide scan of avc_scan.cu
 // The lists built by atomics each round (live faces, CSR entries, the selection) come out in an order that depends on
 // scheduling; nothing computed from them does: counts, minima and the collapses of disjoint neighbourhoods.
 #include "avc_common.cuh"
@@ -22,7 +23,7 @@ using namespace avc;
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kScanThreads = 1024;
+constexpr int kCapThreads = 1024;
 constexpr int kMaxDeg = 32;   // an edge with an endpoint in more live faces is not a candidate this round: the link and
                               // flip tests loop O(deg^2) per edge, and a fan of thousands would stall its warp
 constexpr double kBoundaryWeight = 10.0;    // boundary penalty weight per squared edge length
@@ -32,8 +33,6 @@ constexpr unsigned long long kNoKey = ~0ull;
 constexpr int kMaxElems = 1 << 29;          // avc_video_adjacency's face limit; 3 F edge ids fit in an int
 
 enum { C_LIVE = 0, C_NEXT, C_SEL, C_REM, C_NV, C_NF, C_WORDS = 8 };
-
-inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t); }
 
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
@@ -298,7 +297,7 @@ k_dc_keys(const float* __restrict__ pos, const double* __restrict__ Q, const int
   const D3 vr{(double)(float)v.x, (double)(float)v.y, (double)(float)v.z};
   if (!no_flip(pos, off, vf, lf, a, b, vr) || !no_flip(pos, off, vf, lf, b, a, vr)) return;
   const int id = 3 * live[h / 3] + (h - 3 * (h / 3));
-  const unsigned long long k = ((unsigned long long)__float_as_uint(__double2float_rn(cost)) << 32) | (unsigned)id;
+  const unsigned long long k = depth_key(__double2float_rn(cost), id);
   key[h] = k;
   atomicMin(vmin + a, k);
   atomicMin(vmin + b, k);
@@ -329,24 +328,13 @@ k_dc_select(const int* __restrict__ lf, int* ctr, const int* __restrict__ off, c
   atomicAdd(ctr + C_REM, hnf[h]);
 }
 
-template <class T, class Op>
-__device__ __forceinline__ T block_reduce(T x, T* sh, Op op) {
-  for (int o = 16; o > 0; o >>= 1) x = op(x, __shfl_xor_sync(0xffffffffu, x, o));
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = x;
-  __syncthreads();
-  x = sh[0];
-  for (int w = 1; w < kScanThreads / 32; ++w) x = op(x, sh[w]);
-  return x;
-}
-
 // thr[0]: the collapses applied are the selected keys < thr[0]: the longest prefix in key order that removes at most
 // live - target faces, and at least the smallest
-__global__ void __launch_bounds__(kScanThreads)
+__global__ void __launch_bounds__(kCapThreads)
 k_dc_cap(const int* __restrict__ ctr, const int* __restrict__ sel, const unsigned long long* __restrict__ key,
          const int* __restrict__ hnf, int target, unsigned long long* thr) {
-  __shared__ unsigned long long shk[kScanThreads / 32];
-  __shared__ int shi[kScanThreads / 32];
+  __shared__ unsigned long long shk[kCapThreads / 32];
+  __shared__ int shi[kCapThreads / 32];
   const int n = ctr[C_SEL];
   const long long budget = (long long)ctr[C_LIVE] - target;
   auto sum = [](int x, int y) { return x + y; };
@@ -355,14 +343,14 @@ k_dc_cap(const int* __restrict__ ctr, const int* __restrict__ sel, const unsigne
     return;
   }
   unsigned long long mn = kNoKey;
-  for (int i = threadIdx.x; i < n; i += kScanThreads) mn = min(mn, key[sel[i]]);
-  mn = block_reduce(mn, shk, [](unsigned long long x, unsigned long long y) { return x < y ? x : y; });
+  for (int i = threadIdx.x; i < n; i += kCapThreads) mn = min(mn, key[sel[i]]);
+  mn = block_reduce(mn, shk, [](unsigned long long x, unsigned long long y) { return x < y ? x : y; }, kNoKey);
   unsigned long long ans = 0;
   for (int bit = 63; bit >= 0; --bit) {
     const unsigned long long cand = ans | (1ull << bit);
     int s = 0;
-    for (int i = threadIdx.x; i < n; i += kScanThreads) s += key[sel[i]] < cand ? hnf[sel[i]] : 0;
-    s = block_reduce(s, shi, sum);
+    for (int i = threadIdx.x; i < n; i += kCapThreads) s += key[sel[i]] < cand ? hnf[sel[i]] : 0;
+    s = block_reduce(s, shi, sum, 0);
     if (s <= budget) ans = cand;
   }
   if (threadIdx.x == 0) *thr = ans > mn ? ans : mn + 1;
@@ -421,44 +409,6 @@ k_dc_filter(const int* __restrict__ live, int* ctr, const int* __restrict__ aliv
 }
 
 // ---------------------------------------------------------------- output in input order
-// one block: in-place exclusive scan of x[0, n), the total to *total
-__global__ void __launch_bounds__(kScanThreads) k_dc_scan(int* x, int n, int* total) {
-  __shared__ int warp_tot[kScanThreads / 32];
-  __shared__ int carry;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int base = 0; base < n; base += kScanThreads) {
-    const int i = base + threadIdx.x;
-    const int v = i < n ? x[i] : 0;
-    int s = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += y;
-    }
-    if (lane == 31) warp_tot[w] = s;
-    __syncthreads();
-    if (w == 0) {
-      int t = warp_tot[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, t, o);
-        if (lane >= o) t += y;
-      }
-      warp_tot[lane] = t;
-    }
-    __syncthreads();
-    const int c = carry;
-    const int excl = c + (w ? warp_tot[w - 1] : 0) + s - v;
-    if (i < n) x[i] = excl;
-    __syncthreads();
-    if (threadIdx.x == kScanThreads - 1) carry = excl + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
-}
-
 __global__ void __launch_bounds__(kThreads)
 k_dc_flag_v(const int* __restrict__ remap, int V, int* __restrict__ vscan) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -500,7 +450,7 @@ __global__ void k_dc_counts(const int* __restrict__ ctr, int rounds, int32_t* co
 struct Ws {
   float *pos, *col;
   double* Q;
-  int *remap, *lock, *bnd, *tri, *alive, *live, *next, *lf, *off, *vf, *hnf, *sel, *vscan, *fscan, *ctr;
+  int *remap, *lock, *bnd, *tri, *alive, *live, *next, *lf, *off, *vf, *hnf, *sel, *vscan, *fscan, *sums, *ctr;
   unsigned long long *key, *vmin, *thr;
   void* adj;
   size_t adj_bytes, total;
@@ -529,6 +479,7 @@ Ws carve(void* base, int V, int F) {
   w.next = c.take<int>(F);
   w.sel = c.take<int>(F);
   w.fscan = c.take<int>(F);
+  w.sums = c.take<int>(exclusive_scan_sums(V > F ? V : F));
   w.ctr = c.take<int>(C_WORDS);
   size_t adj = 0;
   avc_video_adjacency_workspace_bytes(V, &adj);
@@ -571,10 +522,10 @@ int avc_mesh_decimate(const float* verts, const float* colors, int32_t V, const 
   const Ws w = carve(workspace, V, F);
   float* col = colors ? w.col : nullptr;
   AVC_CUDA_TRY(cudaMemsetAsync(w.ctr, 0, sizeof(int) * C_WORDS, st));
-  k_dc_init_v<<<blocks(V, kThreads), kThreads, 0, st>>>(verts, colors, V, w.pos, col, w.remap, w.lock);
-  k_dc_init_f<<<blocks(F, kThreads), kThreads, 0, st>>>(tris, F, V, w.tri, w.alive, w.live, w.ctr);
+  k_dc_init_v<<<ceil_div(V, kThreads), kThreads, 0, st>>>(verts, colors, V, w.pos, col, w.remap, w.lock);
+  k_dc_init_f<<<ceil_div(F, kThreads), kThreads, 0, st>>>(tris, F, V, w.tri, w.alive, w.live, w.ctr);
   AVC_TRY(avc_video_adjacency(w.tri, V, F, w.off, w.vf, w.adj, w.adj_bytes, stream));
-  k_dc_quadric<<<blocks(V, kThreads), kThreads, 0, st>>>(w.pos, w.tri, w.alive, V, w.off, w.vf, w.Q);
+  k_dc_quadric<<<ceil_div(V, kThreads), kThreads, 0, st>>>(w.pos, w.tri, w.alive, V, w.off, w.vf, w.Q);
   AVC_LAUNCH_TRY();
 
   int host[C_WORDS];
@@ -583,7 +534,7 @@ int avc_mesh_decimate(const float* verts, const float* colors, int32_t V, const 
   int live_n = host[C_LIVE], rounds = 0;
   int *live = w.live, *next = w.next;
   while (live_n > target_faces) {
-    const unsigned nb = blocks(live_n, kThreads), nh = blocks(3LL * live_n, kThreads);
+    const int nb = ceil_div(live_n, kThreads), nh = ceil_div(3LL * live_n, kThreads);
     k_dc_gather<<<nb, kThreads, 0, st>>>(live, w.ctr, w.tri, w.lf);
     AVC_TRY(avc_video_adjacency(w.lf, V, live_n, w.off, w.vf, w.adj, w.adj_bytes, stream));
     AVC_CUDA_TRY(cudaMemsetAsync(w.bnd, 0, sizeof(int) * (size_t)V, st));
@@ -593,7 +544,7 @@ int avc_mesh_decimate(const float* verts, const float* colors, int32_t V, const 
     k_dc_keys<<<nh, kThreads, 0, st>>>(w.pos, w.Q, w.lf, live, w.ctr, w.off, w.vf, w.hnf, w.lock, w.bnd, w.key,
                                        w.vmin);
     k_dc_select<<<nh, kThreads, 0, st>>>(w.lf, w.ctr, w.off, w.vf, w.hnf, w.key, w.vmin, w.sel);
-    k_dc_cap<<<1, kScanThreads, 0, st>>>(w.ctr, w.sel, w.key, w.hnf, target_faces, w.thr);
+    k_dc_cap<<<1, kCapThreads, 0, st>>>(w.ctr, w.sel, w.key, w.hnf, target_faces, w.thr);
     k_dc_apply<<<nb, kThreads, 0, st>>>(w.ctr, w.sel, w.key, w.thr, w.lf, live, w.off, w.vf, w.pos, col, w.Q,
                                         w.remap, w.tri, w.alive);
     k_dc_filter<<<nb, kThreads, 0, st>>>(live, w.ctr, w.alive, next);
@@ -607,13 +558,13 @@ int avc_mesh_decimate(const float* verts, const float* colors, int32_t V, const 
     int* t = live; live = next; next = t;
   }
 
-  k_dc_flag_v<<<blocks(V, kThreads), kThreads, 0, st>>>(w.remap, V, w.vscan);
-  k_dc_scan<<<1, kScanThreads, 0, st>>>(w.vscan, V, w.ctr + C_NV);
+  k_dc_flag_v<<<ceil_div(V, kThreads), kThreads, 0, st>>>(w.remap, V, w.vscan);
+  exclusive_scan(w.vscan, V, w.sums, w.ctr + C_NV, st);
   AVC_CUDA_TRY(cudaMemcpyAsync(w.fscan, w.alive, sizeof(int) * (size_t)F, cudaMemcpyDeviceToDevice, st));
-  k_dc_scan<<<1, kScanThreads, 0, st>>>(w.fscan, F, w.ctr + C_NF);
-  k_dc_emit_v<<<blocks(V, kThreads), kThreads, 0, st>>>(w.remap, w.vscan, w.pos, col, V, verts_out,
-                                                        colors ? colors_out : nullptr);
-  k_dc_emit_f<<<blocks(F, kThreads), kThreads, 0, st>>>(w.alive, w.fscan, w.tri, w.vscan, F, tris_out);
+  exclusive_scan(w.fscan, F, w.sums, w.ctr + C_NF, st);
+  k_dc_emit_v<<<ceil_div(V, kThreads), kThreads, 0, st>>>(w.remap, w.vscan, w.pos, col, V, verts_out,
+                                                          colors ? colors_out : nullptr);
+  k_dc_emit_f<<<ceil_div(F, kThreads), kThreads, 0, st>>>(w.alive, w.fscan, w.tri, w.vscan, F, tris_out);
   k_dc_counts<<<1, 1, 0, st>>>(w.ctr, rounds, counts);
   AVC_LAUNCH_TRY();
   return 0;

@@ -257,8 +257,6 @@ k_skin_frames(const float* __restrict__ tpose, const int32_t* __restrict__ neare
   }
 }
 
-inline int blocks(long long n, int t) { return (int)((n + t - 1) / t); }
-
 }  // namespace
 
 extern "C" {
@@ -266,8 +264,8 @@ extern "C" {
 int avc_nearest_vertex(const float* query, int32_t N, const float* ref, int32_t M, int32_t* nearest, avc_stream_t stream) {
   if (!query || !ref || !nearest) return AVC_E_NULL;
   if (N < 1 || M < 1) return AVC_E_SIZE;
-  k_nearest_vertex<double><<<blocks(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M,
-                                                                                                     nearest);
+  k_nearest_vertex<double><<<ceil_div(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M,
+                                                                                                       nearest);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -276,8 +274,8 @@ int avc_nearest_vertex_f32(const float* query, int32_t N, const float* ref, int3
                            avc_stream_t stream) {
   if (!query || !ref || !nearest) return AVC_E_NULL;
   if (N < 1 || M < 1) return AVC_E_SIZE;
-  k_nearest_vertex<float><<<blocks(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M,
-                                                                                                    nearest);
+  k_nearest_vertex<float><<<ceil_div(N, NN_THREADS * NN_QPT), NN_THREADS, 0, (cudaStream_t)stream>>>(query, N, ref, M,
+                                                                                                      nearest);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -299,10 +297,10 @@ int avc_mesh_components(const int32_t* faces, int32_t F, int32_t V, int32_t* lab
   int* sizes = (int*)workspace;
   unsigned long long* key = (unsigned long long*)((char*)workspace + need - 16);
   cudaStream_t st = (cudaStream_t)stream;
-  k_cc_init<<<blocks(V, 256), 256, 0, st>>>(V, labels, sizes, key);
-  if (F > 0) k_cc_hook<<<blocks(F, 256), 256, 0, st>>>(faces, F, V, labels);
-  k_cc_flatten<<<blocks(V, 256), 256, 0, st>>>(V, labels, sizes);
-  k_cc_best<<<blocks(V, 256), 256, 0, st>>>(V, labels, sizes, key);
+  k_cc_init<<<ceil_div(V, 256), 256, 0, st>>>(V, labels, sizes, key);
+  if (F > 0) k_cc_hook<<<ceil_div(F, 256), 256, 0, st>>>(faces, F, V, labels);
+  k_cc_flatten<<<ceil_div(V, 256), 256, 0, st>>>(V, labels, sizes);
+  k_cc_best<<<ceil_div(V, 256), 256, 0, st>>>(V, labels, sizes, key);
   k_cc_kept<<<1, 1, 0, st>>>(key, kept);
   AVC_LAUNCH_TRY();
   return 0;
@@ -316,8 +314,8 @@ int avc_lbs_rel_transforms(const float* v_template, const float* J_regressor, co
   if (V < 1 || n_frames < 1) return AVC_E_SIZE;
   cudaStream_t st = (cudaStream_t)stream;
   k_smpl_joints<<<1, 256, 0, st>>>(v_template, J_regressor, V, n_joints, joints_out);
-  k_drive_chain<<<blocks(n_frames, CHAIN_WARPS), CHAIN_WARPS * 32, 0, st>>>(joints_out, pose, pose2rot, parents,
-                                                                            n_joints, n_frames, A_out);
+  k_drive_chain<<<ceil_div(n_frames, CHAIN_WARPS), CHAIN_WARPS * 32, 0, st>>>(joints_out, pose, pose2rot, parents,
+                                                                              n_joints, n_frames, A_out);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -327,7 +325,7 @@ int avc_inv_lbs(const float* verts, const int32_t* nearest, int32_t N, const flo
   if (!verts || !lbs_weights || !A || !tpose_out) return AVC_E_NULL;
   if (n_joints < 1 || n_joints > NJ_MAX) return AVC_E_BADCFG;
   if (N < 1 || M < 1 || (!nearest && M < N)) return AVC_E_SIZE;
-  k_inv_lbs<<<blocks(N, 256), 256, 0, (cudaStream_t)stream>>>(verts, nearest, N, lbs_weights, n_joints, A, tpose_out);
+  k_inv_lbs<<<ceil_div(N, 256), 256, 0, (cudaStream_t)stream>>>(verts, nearest, N, lbs_weights, n_joints, A, tpose_out);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -340,7 +338,7 @@ int avc_lbs_frames(const float* tpose, const int32_t* nearest, int32_t N, const 
   if (N < 1 || M < 1 || (!nearest && M < N)) return AVC_E_SIZE;
   if (frame_begin < 0 || frame_count < 1 || frame_begin > n_frames - frame_count) return AVC_E_SIZE;
   const int groups = (frame_count + SKIN_FRAMES - 1) / SKIN_FRAMES;
-  dim3 grid(blocks(N, 256), groups < 65535 ? groups : 65535);
+  dim3 grid(ceil_div(N, 256), groups < 65535 ? groups : 65535);
   k_skin_frames<<<grid, 256, 0, (cudaStream_t)stream>>>(tpose, nearest, N, lbs_weights, n_joints, A, frame_begin,
                                                         frame_count, out);
   AVC_LAUNCH_TRY();

@@ -23,8 +23,6 @@ using namespace avc;
 
 namespace {
 
-inline int blocks_for(int64_t n, int threads) { return (int)((n + threads - 1) / threads); }
-
 // -------------------------------------------------------------------------------- engine dispatch
 // engine 0: fp32 FFMA tiles on the fp32 buffers; engine 1: wgmma tiles on the two-term bf16 copies.
 // B operands are addressed by their offset in the packed-weight buffer (same offset in the bf16 split).
@@ -144,9 +142,9 @@ int prepare_weights(const NeusPlan& pl, const NeusWs& w, const float* params, cu
   AVC_TRY(zero_pack(pl, w.pack, st));
   AVC_TRY(pack_weights(pl, params, w.pack, st));
   if (pl.cfg.engine == 1) {
-    tc::k_split_bf16<<<blocks_for(pl.pack_floats, 256), 256, 0, st>>>(w.pack, 1, (int)pl.pack_floats,
-                                                                      (int)pl.pack_floats, w.pk_hi, w.pk_lo,
-                                                                      (int)pl.pack_floats);
+    tc::k_split_bf16<<<ceil_div(pl.pack_floats, 256), 256, 0, st>>>(w.pack, 1, (int)pl.pack_floats,
+                                                                    (int)pl.pack_floats, w.pk_hi, w.pk_lo,
+                                                                    (int)pl.pack_floats);
     AVC_LAUNCH_TRY();
   }
   return 0;
@@ -174,15 +172,15 @@ EncodeTargets make_targets(const NeusPlan& pl, const NeusWs& w) {
 // The launches below are shared by the render and the kernel self-test (avc_neus_kernel_test).
 int encode_samples(const float* rays_o, const float* rays_d, const float* z, int nz, int pitch, int Rc, float scale,
                    int multires, int E, int EP, const EncodeTargets& t, cudaStream_t st) {
-  k_encode_samples<<<blocks_for((int64_t)nz * Rc * 8, 256), 256, 0, st>>>(rays_o, rays_d, z, nz, pitch, Rc, scale,
-                                                                         multires, E, EP, t);
+  k_encode_samples<<<ceil_div((int64_t)nz * Rc * 8, 256), 256, 0, st>>>(rays_o, rays_d, z, nz, pitch, Rc, scale,
+                                                                       multires, E, EP, t);
   AVC_LAUNCH_TRY();
   return 0;
 }
 
 int encode_points(const float* pts, int64_t P, float scale, int multires, int E, int EP, const EncodeTargets& t,
                   cudaStream_t st) {
-  k_encode_points<<<blocks_for(P * 8, 256), 256, 0, st>>>(pts, P, scale, multires, E, EP, t);
+  k_encode_points<<<ceil_div(P * 8, 256), 256, 0, st>>>(pts, P, scale, multires, E, EP, t);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -190,8 +188,8 @@ int encode_points(const float* pts, int64_t P, float scale, int multires, int E,
 int encode_fine(const float* rays_o, const float* rays_d, const float* z_vals, int S, int64_t Rc, float sample_dist,
                 float scale, int multires, int E, int EP, float* cin, float* mid_z, float* inside, const EncodeTargets& t,
                 cudaStream_t st) {
-  k_encode_fine<<<blocks_for(Rc * S * 8, 256), 256, 0, st>>>(rays_o, rays_d, z_vals, S, Rc, sample_dist, scale, multires,
-                                                            E, EP, cin, mid_z, inside, t);
+  k_encode_fine<<<ceil_div(Rc * S * 8, 256), 256, 0, st>>>(rays_o, rays_d, z_vals, S, Rc, sample_dist, scale, multires,
+                                                          E, EP, cin, mid_z, inside, t);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -203,8 +201,8 @@ int sdf_head(const NeusPlan& pl, const float* inL, const float* pack, int64_t P,
              cudaStream_t st) {
   const LinDim& dl = pl.sdf[pl.L];
   OutSdf os{sdf_out, 1.0f / pl.cfg.sdf_scale, nz, pitch};
-  k_thin_nt<1, OutSdf><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(inL, dl.Kp, dl.K, pack + pl.pk_wsdf, dl.Kp,
-                                                                    pack + pl.pk_bsdf, P, os);
+  k_thin_nt<1, OutSdf><<<ceil_div(P, 8 * kThinPPW), 256, 0, st>>>(inL, dl.Kp, dl.K, pack + pl.pk_wsdf, dl.Kp,
+                                                                  pack + pl.pk_bsdf, P, os);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -212,8 +210,8 @@ int sdf_head(const NeusPlan& pl, const float* inL, const float* pack, int64_t P,
 // rgb6 = sigmoid of both colour heads on the last hidden colour activation ch[Lc]
 int color_heads(const NeusPlan& pl, const float* chL, const float* pack, int64_t P, float* rgb6, cudaStream_t st) {
   OutHeads oh{rgb6};
-  k_thin_nt<6, OutHeads><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(chL, pl.Hc, pl.Hc, pack + pl.pk_W6, pl.Hc,
-                                                                      pack + pl.pk_b6, P, oh);
+  k_thin_nt<6, OutHeads><<<ceil_div(P, 8 * kThinPPW), 256, 0, st>>>(chL, pl.Hc, pl.Hc, pack + pl.pk_W6, pl.Hc,
+                                                                    pack + pl.pk_b6, P, oh);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -221,8 +219,8 @@ int color_heads(const NeusPlan& pl, const float* chL, const float* pack, int64_t
 // nbar += cbar_0 . W0[:, 3:6]   (the normal columns of colour lin0)
 int nbar_add_color(const NeusPlan& pl, const float* cbar0, const float* pack, int64_t P, float* nbar, cudaStream_t st) {
   OutNbarAdd on{nbar};
-  k_thin_nt<6, OutNbarAdd><<<blocks_for(P, 8 * kThinPPW), 256, 0, st>>>(cbar0, pl.Hc, pl.Hc, pack + pl.pk_c0xT, pl.Hc,
-                                                                        nullptr, P, on);
+  k_thin_nt<6, OutNbarAdd><<<ceil_div(P, 8 * kThinPPW), 256, 0, st>>>(cbar0, pl.Hc, pl.Hc, pack + pl.pk_c0xT, pl.Hc,
+                                                                      nullptr, P, on);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -230,7 +228,7 @@ int nbar_add_color(const NeusPlan& pl, const float* cbar0, const float* pack, in
 // cbar_Lc = (y6bar . W6) * [ch[Lc] > 0]; the fp32 copy may be NULL
 int heads_dgrad(const NeusPlan& pl, const float* y6bar, const float* pack, const float* chL, int64_t P, float* cbar,
                 const Split16& c16, cudaStream_t st) {
-  k_heads_dgrad<<<blocks_for(P * pl.Hc / 4, 256), 256, 0, st>>>(y6bar, pack + pl.pk_W6, pl.Hc, chL, P, cbar, c16);
+  k_heads_dgrad<<<ceil_div(P * pl.Hc / 4, 256), 256, 0, st>>>(y6bar, pack + pl.pk_W6, pl.Hc, chL, P, cbar, c16);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -241,15 +239,15 @@ int chain_start(const NeusPlan& pl, const float* pack, const float* zprev, int64
   const LinDim& dL = pl.sdf[pl.L];
   const LinDim& dp = pl.sdf[pl.L - 1];
   int64_t tot = P * (int64_t)(dp.Np / 4 > pl.EP ? dp.Np / 4 : pl.EP);   // threads: 4 qt columns each, 1 ge entry each
-  k_chain_start<<<blocks_for(tot, 256), 256, 0, st>>>(pack + pl.pk_wsdf, dL.K, dL.skip ? 1 : 0, pl.E, pl.EP, zprev, dp.N,
-                                                      dp.Np, P, qt, ge, qt16);
+  k_chain_start<<<ceil_div(tot, 256), 256, 0, st>>>(pack + pl.pk_wsdf, dL.K, dL.skip ? 1 : 0, pl.E, pl.EP, zprev, dp.N,
+                                                    dp.Np, P, qt, ge, qt16);
   AVC_LAUNCH_TRY();
   return 0;
 }
 
 // n = D(y)^T ge -> cin[p][3:6] and grad_out (or NULL)
 int normals(const NeusPlan& pl, const float* ge, int64_t P, float* cin, float* grad_out, cudaStream_t st) {
-  k_normal<<<blocks_for(P, 128), 128, 0, st>>>(ge, pl.EP, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, cin, grad_out);
+  k_normal<<<ceil_div(P, 128), 128, 0, st>>>(ge, pl.EP, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, cin, grad_out);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -257,8 +255,8 @@ int normals(const NeusPlan& pl, const float* ge, int64_t P, float* cin, float* g
 // gebar = D(y) nbar -> gebar and ubar_0 (fp32 copy or NULL, its split u16), pitch Kp_0
 int dge(const NeusPlan& pl, const float* cin, const float* nbar, int64_t P, float* ubar0, float* gebar, const Split16& u16,
         cudaStream_t st) {
-  k_dge<<<blocks_for(P * 8, 256), 256, 0, st>>>(cin, nbar, pl.EP, pl.E, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, ubar0,
-                                                pl.sdf[0].Kp, gebar, u16);
+  k_dge<<<ceil_div(P * 8, 256), 256, 0, st>>>(cin, nbar, pl.EP, pl.E, pl.cfg.sdf_multires, pl.cfg.sdf_scale, P, ubar0,
+                                              pl.sdf[0].Kp, gebar, u16);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -266,7 +264,7 @@ int dge(const NeusPlan& pl, const float* cin, const float* nbar, int64_t P, floa
 // the encoding half of skip layer l's input adjoint: ubar_l[p][K_l - E + e] = gebar[p][e] / sqrt(2)
 int fill_gebar(const NeusPlan& pl, int l, const float* gebar, int64_t P, float* ubar, const Split16& u16, cudaStream_t st) {
   const LinDim& d = pl.sdf[l];
-  k_fill_gebar<<<blocks_for(P * pl.E, 256), 256, 0, st>>>(gebar, pl.EP, pl.E, P, ubar, d.Kp, d.K - pl.E, u16);
+  k_fill_gebar<<<ceil_div(P * pl.E, 256), 256, 0, st>>>(gebar, pl.EP, pl.E, P, ubar, d.Kp, d.K - pl.E, u16);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -289,13 +287,13 @@ __global__ void k_assemble_sdf_feat(const float* __restrict__ sdf, const float* 
 }
 
 int points_to_cin(const float* pts, int64_t P, float* cin, cudaStream_t st) {
-  k_points_to_cin<<<blocks_for(P, 256), 256, 0, st>>>(pts, P, cin);
+  k_points_to_cin<<<ceil_div(P, 256), 256, 0, st>>>(pts, P, cin);
   AVC_LAUNCH_TRY();
   return 0;
 }
 
 int assemble_sdf_feat(const NeusPlan& pl, const float* sdf, const float* feat, int64_t P, float* out, cudaStream_t st) {
-  k_assemble_sdf_feat<<<blocks_for(P * (pl.F + 1), 256), 256, 0, st>>>(sdf, feat, pl.Fp, pl.F, P, out);
+  k_assemble_sdf_feat<<<ceil_div(P * (pl.F + 1), 256), 256, 0, st>>>(sdf, feat, pl.Fp, pl.F, P, out);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -400,21 +398,21 @@ int gradient_chain(const NeusPlan& pl, const NeusWs& w, int64_t P, float* grad_o
 // The per-kernel launches are shared by the render and the kernel self-test (avc_neus_kernel_test).
 int coarse_z(const float* near, const float* far, const float* jitter, int n, int pitch, int Rc, float* z,
              cudaStream_t st) {
-  k_coarse_z<<<blocks_for((int64_t)Rc * n, 256), 256, 0, st>>>(near, far, jitter, n, pitch, Rc, z);
+  k_coarse_z<<<ceil_div((int64_t)Rc * n, 256), 256, 0, st>>>(near, far, jitter, n, pitch, Rc, z);
   AVC_LAUNCH_TRY();
   return 0;
 }
 
 int upsample(const float* rays_o, const float* rays_d, const float* z, const float* sdf, int n, int pitch, int Rc,
              float inv_s, int per, float* newz, cudaStream_t st) {
-  k_upsample<<<blocks_for(Rc, 8), 256, 0, st>>>(rays_o, rays_d, z, sdf, n, pitch, Rc, inv_s, per, newz);
+  k_upsample<<<ceil_div(Rc, 8), 256, 0, st>>>(rays_o, rays_d, z, sdf, n, pitch, Rc, inv_s, per, newz);
   AVC_LAUNCH_TRY();
   return 0;
 }
 
 int merge(const float* z, const float* sdf, int n, int pitch, const float* newz, const float* news, int per, int Rc,
           float* zo, float* so, int pitch_o, cudaStream_t st) {
-  k_merge<<<blocks_for(Rc, 8), 256, 0, st>>>(z, sdf, n, pitch, newz, news, per, Rc, zo, so, pitch_o);
+  k_merge<<<ceil_div(Rc, 8), 256, 0, st>>>(z, sdf, n, pitch, newz, news, per, Rc, zo, so, pitch_o);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -473,8 +471,8 @@ CompositeArgs make_composite_args(const NeusPlan& pl, const NeusWs& w, const Chu
 // Compositing forward of one chunk; adds the chunk's eikonal sums into ctx.  Only the per-ray outputs of `out` are used.
 int composite_forward(const CompositeArgs& A, const avc_neus_outputs& out, float* ray_part, float* ctx,
                       cudaStream_t st) {
-  k_composite_fwd<<<blocks_for(A.Rc, 8), 256, 0, st>>>(A, out.color_fine, out.extra_color_fine, out.s_val, out.cdf_fine,
-                                                       out.weight_sum, out.weight_max, out.weights, ray_part);
+  k_composite_fwd<<<ceil_div(A.Rc, 8), 256, 0, st>>>(A, out.color_fine, out.extra_color_fine, out.s_val, out.cdf_fine,
+                                                     out.weight_sum, out.weight_max, out.weights, ray_part);
   AVC_LAUNCH_TRY();
   k_reduce_ray_part<<<1, 1024, 0, st>>>(ray_part, A.Rc, 0, ctx + CTX_EIK_NUM);
   k_reduce_ray_part<<<1, 1024, 0, st>>>(ray_part, A.Rc, 1, ctx + CTX_EIK_DEN);
@@ -484,7 +482,7 @@ int composite_forward(const CompositeArgs& A, const avc_neus_outputs& out, float
 
 // Compositing backward of one chunk; adds the chunk's inv_s adjoint into ctx.
 int composite_backward(const CompositeArgs& A, const CompositeBwdArgs& G, float* ctx, cudaStream_t st) {
-  k_composite_bwd<<<blocks_for(A.Rc, 8), 256, 0, st>>>(A, G);
+  k_composite_bwd<<<ceil_div(A.Rc, 8), 256, 0, st>>>(A, G);
   AVC_LAUNCH_TRY();
   k_reduce_ray_part<<<1, 1024, 0, st>>>(G.ray_part, A.Rc, 2, ctx + CTX_INVS_BAR);
   AVC_LAUNCH_TRY();
@@ -494,7 +492,7 @@ int composite_backward(const CompositeArgs& A, const CompositeBwdArgs& G, float*
 // Eikonal normaliser of one chunk, added into ctx (k_relax_count writes ray_part[r][1]).
 int relax_count(const float* rays_o, const float* rays_d, const float* z_vals, int S, int64_t Rc, float sample_dist,
                 float* ray_part, float* ctx, cudaStream_t st) {
-  k_relax_count<<<blocks_for(Rc, 8), 256, 0, st>>>(rays_o, rays_d, z_vals, S, Rc, sample_dist, ray_part);
+  k_relax_count<<<ceil_div(Rc, 8), 256, 0, st>>>(rays_o, rays_d, z_vals, S, Rc, sample_dist, ray_part);
   k_reduce_ray_part<<<1, 1024, 0, st>>>(ray_part, Rc, 1, ctx + CTX_EIK_DEN);
   AVC_LAUNCH_TRY();
   return 0;
@@ -559,15 +557,15 @@ template <int NI>
 int thin_tn(cudaStream_t st, const float* S, int lds, float s_scale, const float* Hm, int ldh, int NC, int64_t P,
             float* out, int si, int sc, float* bout, int split = NI, float* out2 = nullptr, float* bout2 = nullptr) {
   const int rows = 128;
-  k_thin_tn<NI><<<blocks_for(P, rows), 256, 0, st>>>(S, lds, s_scale, Hm, ldh, NC, P, rows, out, si, sc, bout, split,
-                                                     out2, bout2);
+  k_thin_tn<NI><<<ceil_div(P, rows), 256, 0, st>>>(S, lds, s_scale, Hm, ldh, NC, P, rows, out, si, sc, bout, split,
+                                                   out2, bout2);
   AVC_LAUNCH_TRY();
   return 0;
 }
 
 int colsum(cudaStream_t st, const float* X, int ld, int NC, int64_t P, float scale, float* out) {
   const int rows = 64;
-  k_colsum<<<blocks_for(P, rows), 256, 0, st>>>(X, ld, NC, P, rows, scale, out);
+  k_colsum<<<ceil_div(P, rows), 256, 0, st>>>(X, ld, NC, P, rows, scale, out);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -801,11 +799,11 @@ int avc_tc_epi_test(int32_t kind, const float* A, const float* B, int64_t M, int
   __nv_bfloat16* xl = cv.take<__nv_bfloat16>(M * ldm);
   if (cv.used() > workspace_bytes) return AVC_E_SIZE;
   cudaStream_t st = (cudaStream_t)stream;
-  tc::k_split_bf16<<<blocks_for(M * ld, 256), 256, 0, st>>>(A, M, K, K, ah, al, ld);
-  tc::k_split_bf16<<<blocks_for((int64_t)N * ld, 256), 256, 0, st>>>(B, N, K, K, bh, bl, ld);
+  tc::k_split_bf16<<<ceil_div(M * ld, 256), 256, 0, st>>>(A, M, K, K, ah, al, ld);
+  tc::k_split_bf16<<<ceil_div((int64_t)N * ld, 256), 256, 0, st>>>(B, N, K, K, bh, bl, ld);
   const float* xs = (kind == 0 || kind == 12) ? Y : X;      // the operand that is read as a bf16 pair
   if (kind == 0 || kind == 12 || kind == 4 || kind % 100 == 11)
-    tc::k_split_bf16<<<blocks_for(M * ldm, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldm);
+    tc::k_split_bf16<<<ceil_div(M * ldm, 256), 256, 0, st>>>(xs, M, ldx, ldx, xh, xl, ldm);
   AVC_LAUNCH_TRY();
   const tc::SplitPtr a{ah, al, ld}, b{bh, bl, ld};
   const Split16 none{nullptr, nullptr, ldx};
@@ -1292,9 +1290,9 @@ int avc_adam_step(float* params, const float* grads, float* exp_avg, float* exp_
   const double b1 = round_beta(beta1), b2 = round_beta(beta2);
   double bc1 = 1.0 - pow(b1, (double)step);
   double bc2 = 1.0 - pow(b2, (double)step);
-  k_adam<<<blocks_for(n, 256), 256, 0, (cudaStream_t)stream>>>(params, grads, exp_avg, exp_avg_sq, n, lr, (float)b1,
-                                                               (float)b2, eps, (float)bc1, (float)sqrt(bc2), grad_scale,
-                                                               (float)(1.0 - b1), (float)(1.0 - b2));
+  k_adam<<<ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(params, grads, exp_avg, exp_avg_sq, n, lr, (float)b1,
+                                                             (float)b2, eps, (float)bc1, (float)sqrt(bc2), grad_scale,
+                                                             (float)(1.0 - b1), (float)(1.0 - b2));
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -1306,8 +1304,8 @@ int avc_adam_step_dev(float* params, const float* grads, float* exp_avg, float* 
   cudaStream_t st = (cudaStream_t)stream;
   const double b1 = round_beta(beta1), b2 = round_beta(beta2);
   k_adam_state<<<1, 32, 0, st>>>(state, b1, b2);
-  k_adam_dev<<<blocks_for(n, 256), 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, n, state, (float)b1, (float)b2, eps,
-                                                 grad_scale, (float)(1.0 - b1), (float)(1.0 - b2));
+  k_adam_dev<<<ceil_div(n, 256), 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, n, state, (float)b1, (float)b2, eps,
+                                               grad_scale, (float)(1.0 - b1), (float)(1.0 - b2));
   AVC_LAUNCH_TRY();
   return 0;
 }

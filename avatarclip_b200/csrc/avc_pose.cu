@@ -516,28 +516,6 @@ __global__ void k_resolve_batch(const unsigned long long* __restrict__ zbuf, con
 }
 
 // ---------------------------------------------------------------- scores and selection
-__device__ __forceinline__ unsigned ordered_bits(float f) {
-  unsigned u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-// key = (ordered value bits, ~index): the larger key is the larger value, on ties the smaller index
-__device__ __forceinline__ unsigned long long sel_key(float v, int i) {
-  return ((unsigned long long)ordered_bits(v) << 32) | (unsigned)(0xffffffffu - (unsigned)i);
-}
-
-__device__ __forceinline__ double block_sum_d(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) red[w] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int k = 0; k < nw; ++k) s += red[k];
-  return s;
-}
-
 // one CTA per row: F.cosine_similarity(X[i], y) = sum_j (x_j / max(|x|, eps)) (y_j / max(|y|, eps)), sums in fp64
 __global__ void k_rows_cos(const float* __restrict__ X, const float* __restrict__ y, int D, float eps,
                            float* __restrict__ cos_out) {
@@ -548,25 +526,11 @@ __global__ void k_rows_cos(const float* __restrict__ X, const float* __restrict_
     const double a = X[(size_t)i * D + j], b = y[j];
     xx += a * a; xy += a * b; yy += b * b;
   }
-  xx = block_sum_d(xx, red);
-  xy = block_sum_d(xy, red);
-  yy = block_sum_d(yy, red);
+  const auto add = [](double u, double v) { return u + v; };
+  xx = block_reduce(xx, red, add, 0.0);
+  xy = block_reduce(xy, red, add, 0.0);
+  yy = block_reduce(yy, red, add, 0.0);
   if (threadIdx.x == 0) cos_out[i] = (float)(xy / (fmax(sqrt(xx), (double)eps) * fmax(sqrt(yy), (double)eps)));
-}
-
-__device__ __forceinline__ unsigned long long block_max_u64(unsigned long long v, unsigned long long* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    unsigned long long u = __shfl_xor_sync(0xffffffffu, v, o);
-    v = u > v ? u : v;
-  }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) red[w] = v;
-  __syncthreads();
-  unsigned long long m = 0;
-  for (int k = 0; k < nw; ++k) m = red[k] > m ? red[k] : m;
-  return m;
 }
 
 // one CTA: k rounds, each the largest key below the previous round's (keys are distinct)
@@ -579,8 +543,8 @@ __global__ void __launch_bounds__(1024) k_topk(const float* __restrict__ v, int 
       const unsigned long long key = sel_key(v[i], i);
       if (key < prev && key > best) best = key;
     }
-    best = block_max_u64(best, red);
-    if (threadIdx.x == 0) idx_out[r] = (int)(0xffffffffu - (unsigned)(best & 0xffffffffu));
+    best = block_reduce(best, red, [](unsigned long long x, unsigned long long y) { return x > y ? x : y; }, 0ull);
+    if (threadIdx.x == 0) idx_out[r] = sel_index(best);
     prev = best;
   }
 }
@@ -627,9 +591,10 @@ __global__ void k_pose_score(const float* __restrict__ emb, int A, int B, int Dm
     const double f = (float)(s / A), t = text[j];
     xx += f * f; xy += f * t; yy += t * t;
   }
-  xx = block_sum_d(xx, red);
-  xy = block_sum_d(xy, red);
-  yy = block_sum_d(yy, red);
+  const auto add = [](double u, double v) { return u + v; };
+  xx = block_reduce(xx, red, add, 0.0);
+  xy = block_reduce(xy, red, add, 0.0);
+  yy = block_reduce(yy, red, add, 0.0);
   if (threadIdx.x == 0) {
     const float sc = (float)(xy / (fmax(sqrt(xx), 1e-8) * fmax(sqrt(yy), 1e-8)));
     score_out[b] = sc;
@@ -639,7 +604,7 @@ __global__ void k_pose_score(const float* __restrict__ emb, int A, int B, int Dm
 
 __global__ void k_group_best(const unsigned long long* __restrict__ keys, int n, int* __restrict__ best) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g < n) best[g] = (int)(0xffffffffu - (unsigned)(keys[g] & 0xffffffffu));
+  if (g < n) best[g] = sel_index(keys[g]);
 }
 
 // ================================================================ backward of the pose optimiser's chain
@@ -1171,9 +1136,10 @@ __global__ void k_pose_clip_loss(const float* __restrict__ emb, int A, int B, in
     const double f = (float)(s / A), t = text[j];
     xx += f * f; xy += f * t; yy += t * t;
   }
-  xx = block_sum_d(xx, red);
-  xy = block_sum_d(xy, red);
-  yy = block_sum_d(yy, red);
+  const auto add = [](double u, double v) { return u + v; };
+  xx = block_reduce(xx, red, add, 0.0);
+  xy = block_reduce(xy, red, add, 0.0);
+  yy = block_reduce(yy, red, add, 0.0);
   const double lf = sqrt(xx), nf = fmax(lf, 1e-8), nt = fmax(sqrt(yy), 1e-8);
   const double cs = xy / (nf * nt);
   if (threadIdx.x == 0 && loss) loss[b] = (float)(1.0 - (double)(float)cs);

@@ -7,10 +7,6 @@
 
 namespace {
 
-__device__ __forceinline__ unsigned long long pack_depth(float z, int face) {
-  return ((unsigned long long)__float_as_uint(z) << 32) | (unsigned int)face;   // z > 0: uint order == float order
-}
-
 // one face: walk the bounding box, z-test with a 64-bit atomicMin (depth bits, face index).  Both windings are drawn
 // (fill_back=True doubles every face with reversed winding and the rasteriser culls back faces: exactly one copy of
 // each triangle survives), the lighting normal is the one facing the camera.
@@ -38,7 +34,7 @@ __device__ __forceinline__ void raster_face(int f, const float4* __restrict__ pr
       float zp = 1.f / (w0 / a.z + w1 / b.z + w2 / c.z);
       if (zp <= near || zp >= far) continue;
       // image row 0 is the top: row = is - 1 - yi
-      atomicMin(&zbuf[(size_t)(is - 1 - yi) * is + xi], pack_depth(zp, f));
+      atomicMin(&zbuf[(size_t)(is - 1 - yi) * is + xi], avc::depth_key(zp, f));
     }
   }
 }

@@ -161,43 +161,30 @@ __global__ void k_clip_prep_nearest(const float* __restrict__ img, int B, int n,
 }
 
 // ---------------------------------------------------------------- codebook search
-// float -> uint32 whose unsigned order is the float order
-__device__ __forceinline__ unsigned ordered_bits(float f) {
-  unsigned u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 // one block per codebook row: cos[i] = sum_j (C[i][j] - e[j]) / max(|C[i] - e|, 1e-12) * d[j] / max(|d|, 1e-12);
 // sums in fp64.  key = (ordered cos bits, ~index): the 64-bit atomicMax keeps the largest cos, on ties the smallest i.
 __global__ void k_codebook_cos(const float* __restrict__ C, const float* __restrict__ e, const float* __restrict__ d,
                                int N, int D, float* __restrict__ cos_out, unsigned long long* __restrict__ key) {
   const int i = blockIdx.x;
-  __shared__ double red[3][32];
+  __shared__ double red[32];
   double cc = 0.0, cd = 0.0, dd = 0.0;
   for (int j = threadIdx.x; j < D; j += blockDim.x) {
     const double a = (double)(C[(size_t)i * D + j] - e[j]), g = (double)d[j];
     cc += a * a; cd += a * g; dd += g * g;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    cc += __shfl_xor_sync(0xffffffffu, cc, o);
-    cd += __shfl_xor_sync(0xffffffffu, cd, o);
-    dd += __shfl_xor_sync(0xffffffffu, dd, o);
-  }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (lane == 0) { red[0][w] = cc; red[1][w] = cd; red[2][w] = dd; }
-  __syncthreads();
+  const auto add = [](double u, double v) { return u + v; };
+  cc = block_reduce(cc, red, add, 0.0);
+  cd = block_reduce(cd, red, add, 0.0);
+  dd = block_reduce(dd, red, add, 0.0);
   if (threadIdx.x == 0) {
-    cc = cd = dd = 0.0;
-    for (int k = 0; k < nw; ++k) { cc += red[0][k]; cd += red[1][k]; dd += red[2][k]; }
     const float c = (float)(cd / (fmax(sqrt(cc), 1e-12) * fmax(sqrt(dd), 1e-12)));
     cos_out[i] = c;
-    atomicMax(key, ((unsigned long long)ordered_bits(c) << 32) | (unsigned)(0xffffffffu - (unsigned)i));
+    atomicMax(key, sel_key(c, i));
   }
 }
 
 __global__ void k_codebook_best(const unsigned long long* __restrict__ key, int* __restrict__ best) {
-  *best = (int)(0xffffffffu - (unsigned)(*key & 0xffffffffu));
+  *best = sel_index(*key);
 }
 
 }  // namespace

@@ -1,7 +1,7 @@
 // avc_video.cu -- video frames of one large vertex-coloured mesh over many frames (avatarclip_b200/video.py): the
 // vertex -> incident-face lists once per mesh, then per chunk of frames one launch of each stage over every frame.
-//   k_vid_count / k_vid_scan / k_vid_fill / k_vid_sort   CSR adjacency: count, exclusive scan, fill, then each
-//                                                         vertex's list sorted by face id (independent of scheduling)
+//   k_vid_count / exclusive_scan / k_vid_fill / k_vid_sort   CSR adjacency: count, the device-wide exclusive scan of
+//                     avc_scan.cu, fill, then each vertex's list sorted by face id (independent of scheduling)
 //   k_vid_project     per (frame, vertex): world -> camera [R | t] -> supersampled pixel coordinates and depth
 //   k_vid_normals     per (frame, vertex): sum of the un-normalised face cross products in CSR order (no float atomics)
 //   k_vid_raster      per (frame, face): z-buffer by a 64-bit atomicMin of (depth bits | face id)
@@ -15,13 +15,10 @@ using namespace avc;
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kScanThreads = 1024;
 constexpr float kNear = 1e-2f;
 constexpr float kAmbient = 0.25f, kDiffuse = 0.75f;
 constexpr float kGrey = 200.f;
 constexpr int kMaxFrames = 65535;     // grid.y
-
-inline unsigned blocks(long long n, int t) { return (unsigned)((n + t - 1) / t); }
 
 // ---------------------------------------------------------------- adjacency
 __global__ void k_vid_count(const int* __restrict__ faces, int F, int V, int* __restrict__ counts) {
@@ -29,44 +26,6 @@ __global__ void k_vid_count(const int* __restrict__ faces, int F, int V, int* __
   if (i >= 3LL * F) return;
   const int v = faces[i];
   if (v >= 0 && v < V) atomicAdd(counts + v, 1);
-}
-
-// one block: in-place exclusive scan of offsets[0, V) with offsets[V] = the total, tile by tile
-__global__ void __launch_bounds__(kScanThreads) k_vid_scan(int* offsets, int V) {
-  __shared__ int warp_tot[kScanThreads / 32];
-  __shared__ int carry;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int base = 0; base < V; base += kScanThreads) {
-    const int i = base + threadIdx.x;
-    const int x = i < V ? offsets[i] : 0;
-    int s = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += y;
-    }
-    if (lane == 31) warp_tot[w] = s;
-    __syncthreads();
-    if (w == 0) {
-      int t = warp_tot[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, t, o);
-        if (lane >= o) t += y;
-      }
-      warp_tot[lane] = t;
-    }
-    __syncthreads();
-    const int c = carry;
-    const int excl = c + (w ? warp_tot[w - 1] : 0) + s - x;
-    if (i < V) offsets[i] = excl;
-    __syncthreads();
-    if (threadIdx.x == kScanThreads - 1) carry = excl + x;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) offsets[V] = carry;
 }
 
 __global__ void k_vid_fill(const int* __restrict__ faces, int F, int V, int* __restrict__ cursor, int* __restrict__ vf) {
@@ -134,10 +93,6 @@ k_vid_normals(const float* __restrict__ verts, const int* __restrict__ faces, co
   nrm[(size_t)fr * c.V + v] = make_float4(nx, ny, nz, 0.f);
 }
 
-__device__ __forceinline__ unsigned long long vid_key(float z, int face) {
-  return ((unsigned long long)__float_as_uint(z) << 32) | (unsigned)face;   // z > 0: uint order == float order
-}
-
 // one thread per (frame, face): walk the pixel-centre bounding box, both windings
 __global__ void __launch_bounds__(kThreads)
 k_vid_raster(const float4* __restrict__ proj, const int* __restrict__ faces, VidCfg c,
@@ -170,7 +125,7 @@ k_vid_raster(const float4* __restrict__ proj, const int* __restrict__ faces, Vid
       const float w2 = 1.f - w0 - w1;
       if (w0 < 0.f || w1 < 0.f || w2 < 0.f) continue;
       const float zp = 1.f / (w0 / a.z + w1 / b.z + w2 / d.z);
-      atomicMin(Z + (size_t)yi * c.is + xi, vid_key(zp, f));
+      atomicMin(Z + (size_t)yi * c.is + xi, depth_key(zp, f));
     }
   }
 }
@@ -246,6 +201,7 @@ int avc_video_adjacency_workspace_bytes(int32_t V, size_t* bytes) {
   if (V < 1) return AVC_E_SIZE;
   Carver c(nullptr);
   c.take<int>(V);
+  c.take<int>(exclusive_scan_sums(V));
   *bytes = c.used();
   return 0;
 }
@@ -259,12 +215,13 @@ int avc_video_adjacency(const int32_t* faces, int32_t V, int32_t F, int32_t* off
   cudaStream_t st = (cudaStream_t)stream;
   Carver c(workspace);
   int* cursor = c.take<int>(V);
+  int* sums = c.take<int>(exclusive_scan_sums(V));
   AVC_CUDA_TRY(cudaMemsetAsync(offsets, 0, sizeof(int) * ((size_t)V + 1), st));
-  k_vid_count<<<blocks(3LL * F, kThreads), kThreads, 0, st>>>(faces, F, V, offsets);
-  k_vid_scan<<<1, kScanThreads, 0, st>>>(offsets, V);
+  k_vid_count<<<ceil_div(3LL * F, kThreads), kThreads, 0, st>>>(faces, F, V, offsets);
+  exclusive_scan(offsets, V, sums, offsets + V, st);
   AVC_CUDA_TRY(cudaMemcpyAsync(cursor, offsets, sizeof(int) * (size_t)V, cudaMemcpyDeviceToDevice, st));
-  k_vid_fill<<<blocks(3LL * F, kThreads), kThreads, 0, st>>>(faces, F, V, cursor, vf);
-  k_vid_sort<<<blocks(V, kThreads), kThreads, 0, st>>>(offsets, V, vf);
+  k_vid_fill<<<ceil_div(3LL * F, kThreads), kThreads, 0, st>>>(faces, F, V, cursor, vf);
+  k_vid_sort<<<ceil_div(V, kThreads), kThreads, 0, st>>>(offsets, V, vf);
   AVC_LAUNCH_TRY();
   return 0;
 }
@@ -306,11 +263,11 @@ int avc_video_render(const float* verts, int64_t frame_stride, const int32_t* fa
   AVC_CUDA_TRY(cudaMemsetAsync(zbuf, 0xff, sizeof(unsigned long long) * (size_t)n_frames * is * is, st));
   const VidCfg cfg{V, F, image_size, supersample, is, (long long)frame_stride};
   const uchar3 bg = make_uchar3(background[0], background[1], background[2]);
-  k_vid_project<<<dim3(blocks(V, kThreads), n_frames), kThreads, 0, st>>>(verts, cams, cfg, proj);
-  k_vid_normals<<<dim3(blocks(V, kThreads), n_frames), kThreads, 0, st>>>(verts, faces, offsets, vf, cfg, nrm);
-  k_vid_raster<<<dim3(blocks(F, kThreads), n_frames), kThreads, 0, st>>>(proj, faces, cfg, zbuf);
-  k_vid_resolve<<<dim3(blocks((long long)image_size * image_size, kThreads), n_frames), kThreads, 0, st>>>(
-      zbuf, proj, nrm, faces, colors, cams, cfg, bg, rgb_out, face_out);
+  k_vid_project<<<dim3(ceil_div(V, kThreads), n_frames), kThreads, 0, st>>>(verts, cams, cfg, proj);
+  k_vid_normals<<<dim3(ceil_div(V, kThreads), n_frames), kThreads, 0, st>>>(verts, faces, offsets, vf, cfg, nrm);
+  k_vid_raster<<<dim3(ceil_div(F, kThreads), n_frames), kThreads, 0, st>>>(proj, faces, cfg, zbuf);
+  k_vid_resolve<<<dim3(ceil_div((long long)image_size * image_size, kThreads), n_frames), kThreads, 0, st>>>(
+        zbuf, proj, nrm, faces, colors, cams, cfg, bg, rgb_out, face_out);
   AVC_LAUNCH_TRY();
   return 0;
 }

@@ -46,7 +46,7 @@ __global__ void k_raster_project(const float* __restrict__ v, int V, RasterCam c
 
 }  // namespace
 
-#include "avc_raster.cuh"      // pack_depth, k_raster_faces (the z-buffer pass)
+#include "avc_raster.cuh"      // k_raster_faces (the z-buffer pass)
 
 namespace {
 
@@ -107,11 +107,10 @@ __global__ void k_dilate_count(const uint8_t* __restrict__ m, int n, int it, uin
 __global__ void __launch_bounds__(1024, 1)
 k_mask_compact(const uint8_t* __restrict__ dil, int n, int W, int cap, uint8_t* __restrict__ in_mask,
                int* __restrict__ pix, int* __restrict__ count) {
-  __shared__ int warp_tot[32];
-  __shared__ int carry;
+  __shared__ int warp_tot[33];
   const int total = W * W;
   const int per = (total + 1023) / 1024;
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int t = threadIdx.x;
   const float scale = (float)n / (float)W;
   int begin = t * per, end = min(total, begin + per);
   int mine = 0;
@@ -122,32 +121,14 @@ k_mask_compact(const uint8_t* __restrict__ dil, int n, int W, int cap, uint8_t* 
     in_mask[p] = (uint8_t)v;
     mine += v;
   }
-  int inc = mine;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int u = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += u;
-  }
-  if (lane == 31) warp_tot[w] = inc;
-  __syncthreads();
-  if (w == 0) {
-    int v = warp_tot[lane], s = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int u = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += u;
-    }
-    warp_tot[lane] = s - v;
-    if (lane == 31) carry = s;
-  }
-  __syncthreads();
-  int off = warp_tot[w] + inc - mine;
+  int kept;
+  int off = block_exclusive_scan<1024>(mine, warp_tot, kept);
   for (int p = begin; p < end; ++p)
     if (in_mask[p]) {
       if (off < cap) pix[off] = p;
       ++off;
     }
-  if (t == 0) *count = carry;
+  if (t == 0) *count = kept;
 }
 
 __global__ void k_view_targets(const float* __restrict__ rgb, int n, int W, int threshold_mask,

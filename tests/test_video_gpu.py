@@ -62,13 +62,18 @@ def _motion_inputs(files, smpl, image_size):
 
 # ---------------------------------------------------------------- kernels against the oracle
 def test_adjacency_matches_oracle(files):
+    """The template mesh, and a triangle strip over more than 2 x 1024 x 1024 vertices (its last vertex in no face):
+    more 2048-element scan tiles than one pass of the tile-sum scan covers, so its running carry is used."""
     from avatarclip_b200 import drive, video
     mesh = drive.read_ply(files["ply"])
-    V = mesh.vertices.shape[0]
-    adj = video.adjacency(mesh.triangles, V)
-    off, vf = OV.adjacency(mesh.triangles.cpu().numpy(), V)
-    assert np.array_equal(adj.offsets.cpu().numpy(), off)
-    assert np.array_equal(adj.vf.cpu().numpy(), vf)
+    Vs = 3 * 2 ** 20 + 7
+    i = torch.arange(Vs - 3, dtype=torch.int32, device="cuda")
+    strip = torch.stack([i, i + 1 + i % 2, i + 2 - i % 2], 1)
+    for faces, V in ((mesh.triangles, mesh.vertices.shape[0]), (strip, Vs)):
+        adj = video.adjacency(faces, V)
+        off, vf = OV.adjacency(faces.cpu().numpy(), V)
+        assert np.array_equal(adj.offsets.cpu().numpy(), off)
+        assert np.array_equal(adj.vf.cpu().numpy(), vf)
 
 
 def test_template_motion_matches_oracle(files, smpl):
