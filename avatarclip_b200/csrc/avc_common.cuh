@@ -126,13 +126,13 @@ __device__ __forceinline__ int block_exclusive_scan(int x, int* warp_tot, int& t
 }
 
 // avc_scan.cu: the in-place exclusive scan of a[0, n) (n >= 1) in index order over the whole device, and the sum of a
-// to *total.  sums is a workspace of exclusive_scan_sums(n) ints.
+// to *total (it must fit in an int32).  sums is a workspace of exclusive_scan_sums(n) ints; what it held is not read.
 size_t exclusive_scan_sums(int n);
 void exclusive_scan(int* a, int n, int* sums, int32_t* total, cudaStream_t st);
 
-// float -> uint32 whose unsigned order is the float order
+// float -> uint32 whose unsigned order is the float order; -0.0 maps to +0.0's bits, so the two zeros are equal
 __device__ __forceinline__ unsigned ordered_bits(float f) {
-  unsigned u = __float_as_uint(f);
+  const unsigned u = __float_as_uint(f) == 0x80000000u ? 0u : __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -145,8 +145,8 @@ __device__ __forceinline__ int sel_index(unsigned long long key) {
   return (int)(0xffffffffu - (unsigned)(key & 0xffffffffu));
 }
 
-// key = (bits of z, id) for z >= 0 (a depth, a collapse cost): the smaller key is the smaller z, on ties the smaller
-// id, so a 64-bit atomicMin keeps the nearest
+// key = (bits of z, id) for z >= +0 (a depth, a collapse cost): the smaller key is the smaller z, on ties the smaller
+// id, so a 64-bit atomicMin keeps the nearest (a -0.0 z keys above every positive one)
 __device__ __forceinline__ unsigned long long depth_key(float z, int id) {
   return ((unsigned long long)__float_as_uint(z) << 32) | (unsigned)id;
 }

@@ -537,6 +537,24 @@ int avc_neus_kernel_test(int32_t kind, const int64_t* dims, const float* fscal, 
  *   19 k_text_eot_rows  dims {B, T, Wd};  in {tok i[B][T], x[B*T][Wd]};  out {eot[B][Wd]} */
 int avc_clip_kernel_test(int32_t kind, const int32_t* dims, const void* const* in, void* const* out,
                          avc_stream_t stream);
+/* The shared pieces of the mesh, view and pose kernels (avc_common.cuh, avc_scan.cu), each alone on caller buffers
+ * (avc_common_test.cu).  dims is a HOST int64 array, in / out are HOST arrays of DEVICE pointers ("i" int32, "u" uint32,
+ * "q" uint64, "d" fp64, everything else fp32); nothing else is touched.
+ *   0 block_reduce      dims {op (0 fp64 add onto +0.0, 1 int32 add onto 0, 2 uint64 min onto ~0, 3 uint64 max onto 0),
+ *     threads (a multiple of 32, <= 1024), blocks};  in {x[3][blocks threads] of the op's type};  out {r[3][blocks
+ *     threads]}: three back-to-back calls on one red per CTA, thread t's results of x[0], x[1], x[2] at r[., t]
+ *   1 block_exclusive_scan<NT>  dims {NT (32 | 128 | 256 | 1024), blocks, rounds};  in {x i[blocks][rounds NT]};
+ *     out {ex i[blocks][rounds NT], total i[blocks][NT]}: per CTA one call per round on one warp_tot with a running
+ *     carry (ex = carry + the round's scan), total = every thread's carry after the last round
+ *   2 keys              dims {n};  in {v[n]};  out {ordered_bits u[n], sel_key(v[i], i) q[n], sel_index of it i[n],
+ *     depth_key(v[i], i) q[n]}
+ *   3 selection         dims {n, threads, blocks};  in {v[n], z[n] or NULL};  out {q[1] the 64-bit atomicMax of
+ *     sel_key(v[i], i), q[1] the atomicMin of depth_key(z[i], i) (~0 when z is NULL), i[1] sel_index of the max},
+ *     grid-stride over n from every thread
+ *   4 exclusive_scan    dims {n >= 1};  out {a i[n] (scanned in place), sums i[exclusive_scan_sums(n)], total i[1]}
+ *   5 exclusive_scan_sums  dims {n};  out {HOST int64 [1]} */
+int avc_common_kernel_test(int32_t kind, const int64_t* dims, const void* const* in, void* const* out,
+                           avc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Per-step view preparation of Runner.train_clip (SURVEY.md 8f rank 1), all on the device.

@@ -89,9 +89,10 @@ def dilate_and_canvas(mask, max_ray_num, iterations=10):
 
 
 def nearest_resize(a, W):
-    """F.interpolate(..., size=(W, W)) default (nearest): src = floor(dst * n / W)."""
+    """F.interpolate(..., size=(W, W)) default (nearest): src = floor(dst * scale) with scale = n / W and the product
+    both rounded to float32, as torch forms them: a float64 product floors differently at some sizes (33 -> 1023)."""
     n = a.shape[0]
-    idx = np.minimum(np.floor(np.arange(W) * (np.float32(n) / np.float32(W))).astype(np.int64), n - 1)
+    idx = np.minimum(np.floor(np.arange(W, dtype=np.float32) * (np.float32(n) / np.float32(W))).astype(np.int64), n - 1)
     return a[idx][:, idx]
 
 
